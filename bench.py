@@ -1,13 +1,18 @@
 #!/usr/bin/env python3
-"""bench.py -- reads/s of the HISAT2 alignment path on B200 (BASELINE.json), FASTA in -> SAM out.
+"""bench.py -- reads/s of the HISAT2 alignment path on H100, FASTA in -> SAM out.
 
   python bench.py --gpus N --steps K --warmup W            our CUDA path
   python bench.py --impl reference --gpus N --steps K ...  reference CPU path (unmodified hisat2-align-s)
+  python bench.py ... --dump-outputs DIR                   also write a sample of the last timed step's SAM as .npy
+  python bench.py ... --index oracle/_ref/data/22_20-21M   the same workload shape on another linear index
 
-Workload (config.workload): BASELINE.json configs[2], the configuration the metric is quoted on -- the linear
-22_20-21M example index, a FIXED set of 10 M synthetic 2x101-bp pairs (seeded generator, tools/simreads_fast.c),
---no-spliced-alignment -- sharded over the N ranks by contiguous pair ranges (strong scaling).  One "step" =
-one pass of the whole path over the rank's shard, in device batches of 4 M reads.
+Workload (config.workload): the shape of BASELINE.json configs[2] on an index that ships with the repository --
+the linear tests/golden/tiny index (80 kbp cut from the 22_20-21M example region, chrA carrying a mutated
+duplicate), a FIXED set of 10 M synthetic 2x101-bp pairs drawn from its chrA (seeded generator,
+tools/simreads_fast.c), --no-spliced-alignment -- sharded over the N ranks by contiguous pair ranges (strong
+scaling).  One "step" = one pass of the whole path over the rank's shard, in device batches of 4 M reads.
+--index runs the same shape on another linear index: the reads come from the first record of <index>.fa, the graph
+extra from <index>_snp (e.g. the 22_20-21M example index that oracle/make_data.sh stages next to the reference).
   e2e   : FASTA bytes in host memory -> SAM bytes in host memory through ht2gpu_run_reads (multi-threaded
           parser, H2D, alignment kernel, SAM kernels, D2H), host wall clock, max over ranks.  THE headline.
   value : the same job counted on the device only: reads / sum of the CUDA-event times of the alignment and
@@ -31,22 +36,23 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-DATA = os.path.join(ROOT, "data")
-INDEX = os.path.join(DATA, "22_20-21M")
-FASTA = os.path.join(DATA, "22_20-21M.fa")
+INDEX = os.path.join(ROOT, "tests", "golden", "tiny")
+FASTA = INDEX + ".fa"
 REFBIN = os.path.join(ROOT, "oracle", "_ref", "hisat2-align-s")
 RDLEN = 101
 DIGITS = 8
 RECSZ = 2 + DIGITS + 1 + RDLEN + 1
-WORKLOAD = ("BASELINE configs[2]: 22_20-21M linear index, fixed set of %d synthetic 2x101bp pairs (seed 1, --fr, -I 0 -X 1000), "
+WORKLOAD = ("%s linear index, fixed set of %d synthetic 2x101bp pairs from its first sequence (seed 1, --fr, -I 0 -X 1000), "
             "--no-spliced-alignment -k 5, sharded over the ranks by contiguous pair ranges")
 L2_NOTE = ("inputs larger than L2: every step streams the whole read set (110 B of FASTA per read in, ~360 B of SAM per read out) through "
-           "the device; the 7 MB index image is L2-resident by construction (SURVEY 0.4); no flush between steps")
+           "the device; the index image is L2-resident; no flush between steps")
+SAM_SAMPLE_BYTES = 1 << 21     # --dump-outputs: the first 2 MB of SAM text of every batch of the last timed step ...
+SAM_SAMPLE_TOTAL = 1 << 24     # ... until 16 MB are taken (about 45 k records, 7 MB of .npy)
 
 
 def workload_config(pairs):
     """The `config` object, identical for both arms."""
-    return {"workload": WORKLOAD % pairs, "read_len": RDLEN, "pairs_total": pairs, "l2": L2_NOTE}
+    return {"workload": WORKLOAD % (os.path.relpath(INDEX, ROOT), pairs), "read_len": RDLEN, "pairs_total": pairs, "l2": L2_NOTE}
 
 
 def huge_buffer(nbytes):
@@ -80,9 +86,10 @@ _ref = None
 
 
 def ref_seq():
+    """Upper-case bases of the first record of FASTA: fragments never span two records."""
     global _ref
     if _ref is None:
-        _ref = open(FASTA, "rb").read().split(b"\n", 1)[1].replace(b"\n", b"").upper()
+        _ref = open(FASTA, "rb").read().split(b">")[1].split(b"\n", 1)[1].replace(b"\n", b"").upper()
     return _ref
 
 
@@ -166,7 +173,7 @@ def reference_arm(args, rank):
     if rank != 0:
         return
     if not (os.path.exists(REFBIN) and os.path.exists(INDEX + ".1.ht2")):
-        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/hisat2-align-s or data/22_20-21M index not present"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/hisat2-align-s not built"}))
         return
     npairs = args.ref_sample_pairs
     f1, f2 = reference_sample(npairs, "ref")
@@ -194,15 +201,74 @@ def reference_arm(args, rank):
 # ---------------------------------------------------------------------------------------------------------
 # our side
 # ---------------------------------------------------------------------------------------------------------
-def run_steps(idx, d1, d2, steps, batch_reads, threads):
-    """K passes over the shard; returns (wall seconds, summed stats)."""
+def run_steps(idx, d1, d2, steps, batch_reads, threads, last_sink=None):
+    """K passes over the shard; returns (wall seconds, summed stats).  `last_sink` sees the SAM text of the last pass."""
     acc = {}
     t0 = time.perf_counter()
-    for _ in range(steps):
-        _, st = idx.run_reads(data1=d1, data2=d2, collect=False, batch_reads=batch_reads, threads=threads)
+    for i in range(steps):
+        _, st = idx.run_reads(data1=d1, data2=d2, collect=False, batch_reads=batch_reads, threads=threads,
+                              sink=last_sink if i == steps - 1 else None)
         for k, v in st.items():
             acc[k] = acc.get(k, 0) + v
     return time.perf_counter() - t0, acc
+
+
+class SamSample(object):
+    """SAM sink of the last timed step: keeps the first SAM_SAMPLE_BYTES of every batch, cut back to whole records, until
+    SAM_SAMPLE_TOTAL bytes are taken (a fixed sample: the same arguments give the same batches), and counts the bytes of
+    the whole step.  It runs inside the timed region: one copy of at most 2 MB per batch."""
+    def __init__(self):
+        self.parts = []
+        self.taken = 0
+        self.batches = 0
+        self.total_bytes = 0
+
+    def __call__(self, ptr, n):
+        take = min(n, SAM_SAMPLE_BYTES, SAM_SAMPLE_TOTAL - self.taken)
+        if take > 0:
+            b = ctypes.string_at(ptr, take)
+            self.parts.append(b[:b.rfind(b"\n") + 1])
+            self.taken += take
+        self.batches += 1
+        self.total_bytes += n
+
+
+def dump_outputs(out_dir, sample, ref_names):
+    """The sampled SAM records as float64 columns, one .npy per SAM field, plus a CRC-32 of every whole record.
+    Records without an AS:i / NM:i tag (unaligned reads) have 0 there and 0 in has_as / has_nm."""
+    import zlib
+    rid = {n.encode(): i for i, n in enumerate(ref_names)}
+    cols = {k: [] for k in ("read_id", "flag", "ref_id", "pos", "mapq", "rnext_id", "pnext", "tlen", "as_score", "has_as", "nm", "has_nm",
+                            "record_crc32")}
+    for part in sample.parts:
+        for rec in part.splitlines():
+            f = rec.split(b"\t")
+            tags = dict((t[:2], t[5:]) for t in f[11:] if t[2:5] == b":i:")
+            ref = rid.get(f[2], -1)
+            for k, v in (("read_id", int(f[0][1:])), ("flag", int(f[1])), ("ref_id", ref), ("pos", int(f[3])), ("mapq", int(f[4])),
+                         ("rnext_id", ref if f[6] == b"=" else rid.get(f[6], -1)), ("pnext", int(f[7])), ("tlen", int(f[8])),
+                         ("as_score", int(tags.get(b"AS", 0))), ("has_as", int(b"AS" in tags)),
+                         ("nm", int(tags.get(b"NM", 0))), ("has_nm", int(b"NM" in tags)),
+                         ("record_crc32", zlib.crc32(rec))):
+                cols[k].append(v)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in cols.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.asarray(v, dtype=np.float64))
+    np.save(os.path.join(out_dir, "step_sam_bytes.npy"), np.asarray([sample.total_bytes, sample.batches], dtype=np.float64))
+    return len(cols["flag"])
+
+
+def gpu_info(dev):
+    """Name and power limit of the device the numbers were measured on."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(dev), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, timeout=10).stdout.decode().strip()
+        info["power_limit_w"] = float(out)
+    except Exception:
+        pass
+    return info
 
 
 def extra_line(h2, base, d1, d2, n_reads, threads, **opts):
@@ -248,18 +314,26 @@ def extra_rna_line(h2, base, threads):
 
 
 def main():
+    global INDEX, FASTA
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours")
+    ap.add_argument("--index", default=INDEX, help="linear index (prefix of <index>.N.ht2 and <index>.fa); default: tests/golden/tiny")
     ap.add_argument("--pairs", type=int, default=10000000, help="pairs of the whole job (fixed as N grows)")
     ap.add_argument("--batch-reads", type=int, default=4000000, help="reads per device batch")
     ap.add_argument("--ref-sample-pairs", type=int, default=500000, help="pairs per step of the CPU reference (bounded sample)")
     ap.add_argument("--threads", type=int, default=0, help="host parser threads per rank (0 = cores / local ranks, at most 64)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write a fixed sample of the last step's SAM records (rank 0) as DIR/<field>.npy")
     args = ap.parse_args()
+    INDEX, FASTA = os.path.abspath(args.index), os.path.abspath(args.index) + ".fa"
+    for f in (INDEX + ".1.ht2", FASTA):
+        if not os.path.exists(f):
+            raise SystemExit("bench.py: %s not found (--index %s)" % (f, args.index))
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -302,9 +376,10 @@ def main():
     run_steps(idx, d1, d2, warm, args.batch_reads, threads)
     # ---- timed region: K steps, FASTA bytes in host memory -> SAM bytes in host memory
     sampler = ClockSampler(local)
+    sam_sample = SamSample() if args.dump_outputs and rank == 0 else None
     barrier()
     sampler.start()
-    wall, acc = run_steps(idx, d1, d2, args.steps, args.batch_reads, threads)
+    wall, acc = run_steps(idx, d1, d2, args.steps, args.batch_reads, threads, last_sink=sam_sample)
     torch.cuda.synchronize()
     clocks = sampler.stop()
     barrier()
@@ -341,6 +416,7 @@ def main():
         dist.all_reduce(tk, op=dist.ReduceOp.MAX)
         dist.all_reduce(tot, op=dist.ReduceOp.SUM)
     kernel_ms, e2e_ms, align_ms = float(tk[0]), float(tk[1]), float(tk[2])
+    dumped = dump_outputs(args.dump_outputs, sam_sample, idx.ref_names()) if sam_sample is not None else None
     idx.close()
     if rank != 0:
         if dist is not None:
@@ -353,8 +429,8 @@ def main():
     pk_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk_path):
         peaks = json.load(open(pk_path))
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_kind = "measured sustained copy bandwidth (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_kind = "measured sustained copy bandwidth (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data-sheet HBM3 bandwidth"
     # dominant kernel = the alignment kernel; one launch = one device batch
     per_launch_bytes = alg_per_read * sub.n
     achieved = per_launch_bytes / (align_ms_batch / 1e3) / 1e9
@@ -390,12 +466,17 @@ def main():
         "lf_map": lf_map,
         "gpu_launches": int(tot[1]),
         "clocks": clocks,
+        "gpu": gpu_info(local),
         "roofline": {"bound": "hbm", "kernel": "ht2_align_pool_kernel<8,4,false>", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": achieved / peak, "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_kind,
                      "algorithmic_bytes_per_read": alg_per_read, "reads_per_launch": sub.n, "launch_ms": align_ms_batch,
                      "note": "algorithmic bytes = sides touched x 32 B (rank sides) + ftab/SA-sample entries + 2-bit reference bytes, counted in-kernel; "
                              "launch time = CUDA events around back-to-back launches on the launch stream"},
     }
+    if dumped is not None:
+        line["dump_outputs"] = {"dir": args.dump_outputs, "sam_records": dumped,
+                                "note": "the last timed step ran a Python SAM sink that copies at most 2 MB per batch (16 MB in all) "
+                                        "inside the timed region; a run without --dump-outputs uses no sink"}
     if dist is not None:
         dist.destroy_process_group()
     if world == 1 and not args.no_extras:
@@ -404,7 +485,7 @@ def main():
         s1, s2 = d1[:ke * RECSZ], d2[:ke * RECSZ]
         try:
             ex["configs1_SE_1M_reads"] = extra_line(h2, INDEX, d1[:min(hi - lo, 1000000) * RECSZ], None, min(hi - lo, 1000000), threads)
-            ex["graph_index_22_20-21M_snp_PE"] = extra_line(h2, INDEX + "_snp", s1, s2, 2 * ke, threads)
+            ex["graph_index_%s_snp_PE" % os.path.basename(INDEX)] = extra_line(h2, INDEX + "_snp", s1, s2, 2 * ke, threads)
             ex["sensitive_PE (bowtie2_dp 1, score-min L,0,-0.5)"] = extra_line(h2, INDEX, s1, s2, 2 * ke, threads, bowtie2_dp=1, score_min_type=ord("L"),
                                                                               score_min_const=0.0, score_min_coeff=-0.5)
             ex["very_sensitive_PE (bowtie2_dp 2, -k 30, score-min L,0,-1)"] = extra_line(h2, INDEX, s1, s2, 2 * ke, threads, bowtie2_dp=2, khits=30,

@@ -1,4 +1,4 @@
-"""hisat2_b200 -- B200-native implementation of HISAT2's per-read alignment
+"""hisat2_b200 -- H100-native (sm_90a) implementation of HISAT2's per-read alignment
 hot path behind a C ABI (include/ht2gpu.h).  Python here is plumbing only:
 ctypes bindings, batching helpers and the multi-GPU launcher glue."""
 from .api import Index, ReadBatch, AlignResult, Ht2GpuError, load_library  # noqa: F401

@@ -540,9 +540,10 @@ class Index(object):
             other.load_splicesites(*self._ss)
         return other
 
-    def run_reads(self, path1=None, path2=None, data1=None, data2=None, fastq=False, collect=True, peers=(), **kw):
+    def run_reads(self, path1=None, path2=None, data1=None, data2=None, fastq=False, collect=True, peers=(), sink=None, **kw):
         """ht2gpu_run_reads(_multi): FASTA/FASTQ (files or bytes in host memory) -> SAM records through the overlapped
-        pipeline, on this index's device and on the devices of `peers`.  Returns (sam bytes or None, stats dict)."""
+        pipeline, on this index's device and on the devices of `peers`.  Returns (sam bytes or None, stats dict).
+        `sink(ptr, n)`, if given, sees the SAM text of every batch in read order while it is valid (pinned host memory)."""
         ri = CReadsInput()
         keep = []
         if path1 is not None:
@@ -564,9 +565,11 @@ class Index(object):
         def _sink(ctx, ptr, n):
             if collect:
                 chunks.append(C.string_at(ptr, n))
+            if sink is not None:
+                sink(ptr, n)
             total[0] += n
             return 0
-        cb = SINK_FN(_sink) if collect else SINK_FN()     # NULL sink: the text still lands in pinned host memory
+        cb = SINK_FN(_sink) if (collect or sink is not None) else SINK_FN()     # NULL sink: the text still lands in pinned host memory
         st = CRunStats()
         hs = (C.c_void_p * (1 + len(peers)))(self._h, *[p._h for p in peers])
         self._check(self._lib.ht2gpu_run_reads_multi(hs, len(hs), C.byref(ri), cb, None, C.byref(st)), "ht2gpu_run_reads")

@@ -1,9 +1,10 @@
-"""Build helpers: compile the CUDA library (sm_100a) and the test-side oracle.
+"""Build helpers: compile the CUDA library (sm_90a) and the test-side oracle.
 
 `build_lib()` runs nvcc on hisat2_b200/csrc and leaves hisat2_b200/libht2gpu.so
-in-tree (git-ignored, shipped to the GPU box by gpurun).  nvcc cross-compiles
-without a GPU.  `build_oracle()` compiles oracle/'s C restatement and, when
-/root/reference is present, the unmodified reference into oracle/_ref/.
+in-tree (git-ignored).  nvcc cross-compiles without a GPU.  `build_oracle()`
+compiles oracle/'s C restatement and, when the reference sources are present
+($HT2_REFERENCE), the unmodified reference plus the staged test data into
+oracle/_ref/.
 """
 import os
 import subprocess
@@ -14,7 +15,7 @@ CSRC = os.path.join(ROOT, "hisat2_b200", "csrc")
 LIB = os.path.join(ROOT, "hisat2_b200", "libht2gpu.so")
 CLI = os.path.join(ROOT, "hisat2_b200", "hisat2-b200")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++14",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++14",
     "-Xcompiler", "-fPIC", "-cudart", "static",
 ]
 LIB_SRCS = ["ht2_gpu.cu", "ht2_index.cpp", "ht2_host.cpp", "ht2_reads.cpp", "ht2_pipeline.cpp", "ht2_compat.cpp"]

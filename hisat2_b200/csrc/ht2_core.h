@@ -1,6 +1,6 @@
 // ht2_core.h -- per-read HISAT2 alignment state machine (host+device).
 //
-// This is the B200 re-implementation of the reference's per-read hot path
+// This is the GPU re-implementation of the reference's per-read hot path
 // HI_Aligner::go (hi_aligner.h:4048) and everything below it, written as a
 // self-contained, allocation-free state machine over a fixed-size per-read
 // workspace so that one GPU thread can run one read (pair) to completion.
@@ -352,7 +352,7 @@ HT2_HD int ht2_max_gaps(int64_t minsc, int open, int ext) {
 }
 
 // ------------------------------------------------------------------------
-// 2 x s16 SIMD-in-word: the DPX instructions of sm_90+/sm_100 (VIADDMNMX / VIMNMX3 .S16x2), with
+// 2 x s16 SIMD-in-word: the DPX instructions of sm_90 (VIADDMNMX / VIMNMX3 .S16x2), with
 // portable forms for the host test build
 // ------------------------------------------------------------------------
 HT2_HD uint32_t ht2_v2_addmax(uint32_t a, uint32_t b, uint32_t c) {   // per half: max(a + b, c), signed

@@ -267,7 +267,7 @@ __device__ __forceinline__ uint32_t rg_code(const Ht2Work* W)
 // the returned old word tells which ones were really won), run one segment of each claimed slot on its 32 lanes,
 // and publish the new states with atomicOr.  No lock, no scan over the slot array, no waiting for another warp's
 // segments (round 1 serialised the gather under a block lock: 20 % of all executed instructions were warps
-// spinning on it, profiles/r02_*).  The target state is a block-wide hint: warps stay on it while it has
+// spinning on it).  The target state is a block-wide hint: warps stay on it while it has
 // plenty of claimable slots and otherwise re-elect the most populous state from per-state counters, so the warps
 // of an SM execute the same code most of the time (instruction fetch is the scarce resource: the L1.5 I-cache and
 // the GPC instruction cache saturate when every warp walks different code) while groups are drawn from a pool
@@ -591,6 +591,9 @@ ht2_sam_scan_kernel(unsigned long long* blk, uint32_t nBlk)
 // the D2H copy of batch i-1 overlap the kernels of batch i.  The alignment workspaces (dWork) are shared by all
 // slots: kernels of different slots are chained through the device's WorkPool.
 #define HT2GPU_N_SLOTS 3
+// device memory a handle leaves free beside its workspace pool: slot buffers of 4 M-read batches, the per-thread
+// stack of the pool kernel, and headroom for other work on the device
+#define HT2_MEM_RESERVE ((size_t)10 << 30)
 struct SamSlot {
     bool         init;
     cudaStream_t stream;
@@ -760,8 +763,21 @@ static int finishOpen(ht2gpu_handle* h)
     CK(cudaMemcpy(h->dMinsc, h->P.minscTab, sizeof(h->P.minscTab), cudaMemcpyHostToDevice));
     {   // the device's workspace pool for this launch geometry
         std::lock_guard<std::mutex> lk(gPoolMu);
-        WorkPool* wp = NULL;
-        for (WorkPool* q : gPools) if (q->device == h->device && q->nWork == h->nWork) wp = q;
+        auto findPool = [&](size_t n) { WorkPool* r = NULL; for (WorkPool* q : gPools) if (q->device == h->device && q->nWork == n) r = q; return r; };
+        const size_t nThreads = (size_t)h->nSM * h->bpsm * (size_t)h->tpb;
+        const size_t dpBytes = nThreads * (sizeof(Ht2SwScratch) + (size_t)HT2_SW_POOL_WORDS * sizeof(uint32_t));
+        WorkPool* wp = findPool(h->nWork);
+        if (!wp && h->opt.slots_per_lane <= 0 && !h->graph && h->poolWarps == 8 && h->rgK == 4) {
+            // The default geometry's workspace (368 kB per slot, ~50 GB on an H100) must leave room for what else the
+            // process and the device need: the DP scratch of this handle, slot buffers, stack, other processes.  Where
+            // it does not, or where the process already has the half-size pool, linear indexes run with 2 slots per
+            // lane: half the memory, about 12 % less kernel throughput (DESIGN.md 3).  Graph indexes have one geometry.
+            size_t freeB = 0, totalB = 0;
+            CK(cudaMemGetInfo(&freeB, &totalB));
+            WorkPool* half = findPool(h->nWork / 2);
+            const size_t need = h->nWork * sizeof(Ht2Work) + (h->P.bowtie2Dp ? dpBytes : 0) + HT2_MEM_RESERVE;
+            if (half || need > freeB) { h->rgK = 2; h->nWork /= 2; wp = half; }
+        }
         if (!wp) {
             wp = new WorkPool();
             wp->device = h->device; wp->nWork = h->nWork; wp->refs = 0;
@@ -774,7 +790,6 @@ static int finishOpen(ht2gpu_handle* h)
             gPools.push_back(wp);
         }
         if (h->P.bowtie2Dp && !wp->dSw) {   // dynamic-programming scratch (ht2_sw.h): per executing thread, not per read slot
-            const size_t nThreads = (size_t)h->nSM * h->bpsm * (size_t)h->tpb;
             CK(cudaMalloc(&wp->dSw, nThreads * sizeof(Ht2SwScratch)));
             CK(cudaMalloc(&wp->dSwPool, nThreads * (size_t)HT2_SW_POOL_WORDS * sizeof(uint32_t)));
         }
@@ -1058,7 +1073,10 @@ static int launchAlign(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* 
         else ht2_align_pool_kernel<8, 4, true, false><<<grid, 256, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
     } else {
         switch (h->poolWarps * 100 + h->rgK) {
-            case 802:  ht2_align_pool_kernel<8, 2, false, false><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work); break;
+            case 802:
+                if (nospl) ht2_align_pool_kernel<8, 2, false, true><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
+                else ht2_align_pool_kernel<8, 2, false, false><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
+                break;
             case 408:  ht2_align_pool_kernel<4, 8, false, false><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work); break;
             default:
                 if (nospl) ht2_align_pool_kernel<8, 4, false, true><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);

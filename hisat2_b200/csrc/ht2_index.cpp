@@ -228,7 +228,7 @@ void readBody(FileBuf& f, Blob& b, Ht2Gfm& g)
 
 // Densify the suffix-array sample of a LINEAR index.  The .ht2 files sample every 2^offRate-th row (offRate 4 by
 // default: gfm.h:5682 getOffset walks ~7.5 LF steps per resolved row, a third of all LF steps of a read); the
-// image spends HBM instead -- 180 GB per GPU -- and keeps every 2^HT2_DENSE_OFFRATE-th row, so that
+// image spends HBM instead -- 80 GB per H100 -- and keeps every 2^HT2_DENSE_OFFRATE-th row, so that
 // tryOffset succeeds after ~1.5 steps.  The value of a row is a property of the index, not of the sampling:
 // new[r] = old[row'] + steps for the first sampled row' on r's LF walk, exactly what getOffset returns.
 #ifndef HT2_DENSE_OFFRATE

@@ -16,7 +16,7 @@
 // result replaces the anchor with a full-length hit.
 //
 // Restated here: swFill IS the striped kernel, two rows per 32-bit word as signed 16-bit halves instead of
-// 16 (or 8) per SSE register, because sm_100a executes max(a + b, c) on s16x2 and the 3-input max in ONE
+// 16 (or 8) per SSE register, because sm_90a executes max(a + b, c) on s16x2 and the 3-input max in ONE
 // instruction each (the DPX family: __viaddmax_s16x2, __vimax3_s16x2) while the byte-wise video
 // instructions (__vsubus4, __vmaxu4) are emulated (about 6 and 4 instructions, measured in the SASS): a
 // column costs 8 SIMD instructions per word = 4 per cell.  Saturating subtraction a (-) b is
@@ -187,7 +187,7 @@ __device__ __forceinline__ static uint32_t swShift1(uint32_t w, uint32_t lane, u
 // integer instructions.  This evaluates the saturating recurrences at the top of this file DIRECTLY -- no lazy-F
 // loop: the striped kernel's lazy-F pass, cheap with 2 (swFill) or 16 (SSE) rows per vector, degenerates when
 // the vector is a warp wide, because a reference-gap chain below the read's diagonal crosses a vector position
-// every R rows and each crossing costs a pass (measured: ~20 passes per column, profiles/r02_*dp2*).  Cell values
+// every R rows and each crossing costs a pass (about 20 passes per column on the --bowtie2-dp 2 fixtures).  Cell values
 // are those of swFill; they are stored skewed, step-major (word q of lane L at step t), so that every store is a
 // coalesced line: cell (row, col) = half k & 1 of word ((col + L) * 32 + L) * RW + k / 2, L = row / R, k = row % R,
 // RW = ceil(R / 2) (swRaw).  All 32 lanes must call this with the same arguments.

@@ -4,7 +4,7 @@ read-id ranges, index image broadcast once, SAM chunks gathered in rank order.
 The reference's only parallelism is `-p N` threads pulling reads from one
 input (hisat2.cpp:3657-3696) with `--reorder` restoring input order
 (outq.cpp:51-99).  Reads are independent under --no-spliced-alignment, so the
-B200 equivalent shards reads across ranks with NO data-path collective: the
+GPU equivalent shards reads across ranks with NO data-path collective: the
 only collective is the start-up broadcast of the packed index image (NCCL over
 NVLink/NVSwitch when the backend is nccl, gloo in the CPU tests).
 """

@@ -1,4 +1,4 @@
-/* ht2gpu.h -- C ABI of the B200 HISAT2 alignment hot path.
+/* ht2gpu.h -- C ABI of the H100 HISAT2 alignment hot path.
  *
  * The reference has no FFI for alignment ("Alignment APIs: TODO",
  * hisat2lib/ht2.h:133-138); its seam is the per-thread C++ call

@@ -1,13 +1,14 @@
 #!/bin/bash
-# oracle/make_data.sh -- stage the benchmark/test DATA under <repo>/data/
-# (git-ignored, shipped to the GPU box by gpurun): the reference's bundled
+# oracle/make_data.sh -- stage the reference-comparison test DATA under
+# oracle/_ref/data/ (git-ignored, beside the reference binaries that the tests
+# using it run): the reference's bundled
 # example index / FASTA / reads (data files, not sources), the linear
 # 22_20-21M index built with the reference's own hisat2-build-s (index
 # construction is out of scope, SURVEY.md section 2), and seeded synthetic reads.
 set -e
 cd "$(dirname "$0")"
 REF=${REF:-/root/reference}
-D=../data
+D=_ref/data
 mkdir -p $D
 cp --update=none $REF/example/index/22_20-21M_snp.*.ht2 $D/
 cp --update=none $REF/example/reference/22_20-21M.fa $REF/example/reference/22_20-21M.snp $D/

@@ -26,7 +26,7 @@ G = os.path.join(ROOT, "tests", "golden")
 REF = os.path.join(ROOT, "oracle", "_ref")
 
 def main():
-    _, seq = simreads.load_fasta_codes(os.path.join(ROOT, "data", "22_20-21M.fa"))
+    _, seq = simreads.load_fasta_codes(os.path.join(ROOT, "oracle", "_ref", "data", "22_20-21M.fa"))
     rng = np.random.default_rng(11)
     def mutate(a, rate):
         a = a.copy()

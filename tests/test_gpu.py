@@ -13,8 +13,13 @@ from conftest import GOLDEN, REFDIR, ROOT, sam_lines
 
 pytestmark = pytest.mark.gpu
 
-DATA = os.path.join(ROOT, "data")
+DATA = os.path.join(REFDIR, "data")
 REFBIN = os.path.join(REFDIR, "hisat2-align-s")
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+import refsets  # noqa: E402
+
+# md5 of the unmodified reference's SAM for every read set of tools/refsets.py (+ the reads it flags, where a case can)
+REF_SETS = refsets.load_expected()
 
 
 @pytest.fixture(scope="module")
@@ -25,21 +30,23 @@ def h2(lib):
     return hisat2_b200
 
 
-@pytest.fixture(scope="module")
+# Index handles are per test: the device workspace lives as long as a handle of the process does (~50 GB on an
+# H100), and tests that run the command line front end start a second process that needs its own.
+@pytest.fixture
 def tiny(h2):
     idx = h2.Index(os.path.join(GOLDEN, "tiny"))
     yield idx
     idx.close()
 
 
-@pytest.fixture(scope="module")
-def chr22(h2):
-    base = os.path.join(DATA, "22_20-21M")
-    if not os.path.exists(base + ".1.ht2"):
-        pytest.skip("data/22_20-21M index not staged (oracle/make_data.sh)")
-    idx = h2.Index(base)
-    yield idx
-    idx.close()
+@pytest.fixture(scope="session")
+def sets(tmp_path_factory):
+    """The read sets of tools/refsets.py, generated from the committed tiny fixtures."""
+    return refsets.generate(str(tmp_path_factory.mktemp("sets")))
+
+
+def set_files(sets, name):
+    return os.path.join(sets, name + "_1.fa"), os.path.join(sets, name + "_2.fa")
 
 
 def n_batches(units, batch_reads, paired=False):
@@ -85,19 +92,14 @@ def test_tiny_pe_matches_golden_reference_sam(h2, tiny):
     assert {99, 147, 83, 163}.issubset(flags) and (73 in flags or 89 in flags) and 77 in flags
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
 @pytest.mark.parametrize("name", ["sim10k", "hard20k", "len36", "len150", "len500"])
-def test_chr22_paired_matches_reference_binary_run_here(h2, chr22, name, tmp_path):
-    """BASELINE configs[2]-shaped input (2x101 bp pairs): SAM identical to the reference."""
-    f1, f2 = os.path.join(DATA, name + "_1.fa"), os.path.join(DATA, name + "_2.fa")
-    if not os.path.exists(f1):
-        pytest.skip(f1 + " not staged")
+def test_chr22_paired_matches_reference_binary_run_here(h2, tiny, sets, name):
+    """BASELINE configs[2]-shaped input (2x101 bp pairs; also short, long, ragged, with indels and Ns) simulated from the
+    tiny fixture: SAM identical to the reference's (md5 of its output, tests/golden/ref_sets.json)."""
+    f1, f2 = set_files(sets, name)
     batch = h2.ReadBatch.from_fasta(f1, path2=f2)
-    sam, res = gpu_sam(chr22, batch)
-    out = str(tmp_path / "ref.sam")
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", os.path.join(DATA, "22_20-21M"), "-1", f1, "-2", f2, "-S", out,
-                    "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    assert sam_lines(sam) == sam_lines(open(out, "rb").read())
+    sam, res = gpu_sam(tiny, batch)
+    assert refsets.sam_md5(sam) == REF_SETS["md5"]["paired/" + name]
 
 
 def test_in_kernel_seed_search_matches_oracle(h2, tiny, oracle_bin):
@@ -196,26 +198,20 @@ def test_pipeline_reads_in_sam_out_matches_golden(h2, tiny):
         tiny.run_reads(path1=g("tiny_pe_1.fa"), path2=g("tiny_se.fa"))
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
-def test_pipeline_and_cli_match_reference_binary_at_scale(h2, chr22, tmp_path):
-    """200k pairs of the chr22 set through ht2gpu_run_reads (50k-read batches: nine batches over three slots)
-    and through the hisat2-b200 command line: both byte-identical to the reference binary run here."""
-    f1, f2 = os.path.join(DATA, "sim200k_1.fa"), os.path.join(DATA, "sim200k_2.fa")
-    if not os.path.exists(f1):
-        pytest.skip(f1 + " not staged")
-    out = str(tmp_path / "ref.sam")
-    base = os.path.join(DATA, "22_20-21M")
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", base, "-1", f1, "-2", f2, "-S", out,
-                    "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    want = sam_lines(open(out, "rb").read())
-    sam, st = chr22.run_reads(path1=f1, path2=f2, batch_reads=50000)
+def test_pipeline_and_cli_match_reference_binary_at_scale(h2, tiny, sets, tmp_path):
+    """200k pairs through ht2gpu_run_reads (50k-read batches: nine batches over three slots) and through the hisat2-b200
+    command line: both identical to the reference's SAM."""
+    f1, f2 = set_files(sets, "sim200k")
+    want = REF_SETS["md5"]["paired/sim200k"]
+    sam, st = tiny.run_reads(path1=f1, path2=f2, batch_reads=50000)
     assert st["n_batches"] == n_batches(200000, 50000, paired=True) and st["n_err_reads"] == 0
-    assert sam_lines(chr22.sam_header() + sam) == want
+    assert refsets.sam_md5(tiny.sam_header() + sam) == want
+    tiny.close()                    # the CLI below is a second process on the device
     cli = os.path.join(ROOT, "hisat2_b200", "hisat2-b200")
     out2 = str(tmp_path / "cli.sam")
-    subprocess.run([cli, "--no-spliced-alignment", "-f", "-x", base, "-1", f1, "-2", f2, "-S", out2, "--batch", "120000"], check=True,
-                   stderr=subprocess.DEVNULL)
-    assert sam_lines(open(out2, "rb").read()) == want
+    subprocess.run([cli, "--no-spliced-alignment", "-f", "-x", os.path.join(GOLDEN, "tiny"), "-1", f1, "-2", f2, "-S", out2, "--batch", "120000"],
+                   check=True, stderr=subprocess.DEVNULL)
+    assert refsets.sam_md5(open(out2, "rb").read()) == want
 
 
 def _option_cases():
@@ -285,23 +281,16 @@ def test_graph_index_alignment_matches_golden_reference_sam(h2):
     index.close()
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
 @pytest.mark.parametrize("name,paired", [("reads", False), ("hard20k", False), ("alt20k", False), ("sim200k", False), ("sim10k", True),
                                          ("alt20k", True), ("hard20k", True)])
-def test_bundled_graph_index_matches_reference_binary_run_here(h2, name, paired, tmp_path):
-    """The reference's bundled example index 22_20-21M_snp (BASELINE configs[0] literally): SAM identical to the
-    reference run on this box, incl. 20k reads / pairs that carry ALT alleles (3.5k alignments through ALTs)."""
-    base = os.path.join(DATA, "22_20-21M_snp")
-    f1, f2 = os.path.join(DATA, name + "_1.fa"), os.path.join(DATA, name + "_2.fa")
-    if not (os.path.exists(base + ".1.ht2") and os.path.exists(f1)):
-        pytest.skip("data/ not staged")
-    index = h2.Index(base)
+def test_bundled_graph_index_matches_reference_binary_run_here(h2, sets, name, paired):
+    """The graph (SNP) index tiny_snp (BASELINE configs[0]-shaped): SAM identical to the reference's, incl. 20k reads /
+    pairs that carry ALT alleles."""
+    f1, f2 = set_files(sets, name)
+    index = h2.Index(os.path.join(GOLDEN, "tiny_snp"))
     batch = h2.ReadBatch.from_fasta(f1, path2=f2 if paired else None)
     sam, _ = gpu_sam(index, batch)
-    out = str(tmp_path / "ref.sam")
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", base] + (["-1", f1, "-2", f2] if paired else ["-U", f1]) +
-                   ["-S", out, "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    assert sam_lines(sam) == sam_lines(open(out, "rb").read())
+    assert refsets.sam_md5(sam) == REF_SETS["md5"]["graph_%s/%s" % ("pe" if paired else "se", name)]
     index.close()
 
 
@@ -316,38 +305,22 @@ def test_warp_wide_dp_fill_equals_lane_fill_cell_by_cell(h2):
     assert r["mismatches"] == 0
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
-@pytest.mark.parametrize("index,name,paired,flags,opts", [
-    ("22_20-21M", "hard20k", False, ["--bowtie2-dp", "2"], dict(bowtie2_dp=2)),
-    ("22_20-21M", "hard20k", True, ["--sensitive"], dict(bowtie2_dp=1, score_min_type=ord("L"), score_min_const=0.0, score_min_coeff=-0.5)),
-    ("22_20-21M_snp", "alt20k", True, ["--very-sensitive"], dict(bowtie2_dp=2, khits=30, score_min_type=ord("L"), score_min_const=0.0, score_min_coeff=-1.0)),
-    ("22_20-21M", "len150", False, ["--bowtie2-dp", "1", "--score-min", "L,0,-0.4", "--gbar", "2"],
-     dict(bowtie2_dp=1, gbar=2, score_min_type=ord("L"), score_min_const=0.0, score_min_coeff=-0.4)),
-])
-def test_dynamic_programming_extension_matches_reference_binary_run_here(h2, index, name, paired, flags, opts, tmp_path):
+@pytest.mark.parametrize("case", range(len(refsets.DP_CASES)))
+def test_dynamic_programming_extension_matches_reference_binary_run_here(h2, sets, case):
     """--bowtie2-dp / --sensitive / --very-sensitive (SURVEY a30: the SwAligner seed extension): SAM identical to
-    the reference run on this box wherever no read hit a fixed device capacity (such reads are flagged, and
-    must be rare)."""
-    base = os.path.join(DATA, index)
-    f1, f2 = os.path.join(DATA, name + "_1.fa"), os.path.join(DATA, name + "_2.fa")
-    if not (os.path.exists(base + ".1.ht2") and os.path.exists(f1)):
-        pytest.skip("data/ not staged")
-    idx = h2.Index(base, **opts)
+    the reference's wherever no read hit a fixed device capacity (such reads are flagged, must be rare, and are
+    exactly the ones recorded with the expected output)."""
+    index, name, paired, flags, opts = refsets.DP_CASES[case]
+    f1, f2 = set_files(sets, name)
+    idx = h2.Index(os.path.join(GOLDEN, index), **opts)
     batch = h2.ReadBatch.from_fasta(f1, path2=f2 if paired else None)
     res = idx.align(batch)
     errs = np.nonzero(res.reads["err"])[0]
     assert len(errs) <= 0.002 * len(res.reads["err"])
+    bad = sorted(set(batch.names[int(u) * (2 if paired else 1)].split(b"/")[0].decode() for u in errs))
+    assert bad == REF_SETS["flagged"].get("dp/%d" % case, [])
     sam = idx.sam_header() + idx.format_sam(batch, res)
-    out = str(tmp_path / "ref.sam")
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", base] + flags + (["-1", f1, "-2", f2] if paired else ["-U", f1]) +
-                   ["-S", out, "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    got, want = sam_lines(sam), sam_lines(open(out, "rb").read())
-    if len(errs) == 0:
-        assert got == want
-    else:
-        bad = set(batch.names[int(u) * (2 if paired else 1)].split(b"/")[0] for u in errs)
-        keep = lambda ls: [l for l in ls if l.split(b"\t")[0] not in bad]
-        assert keep(got) == keep(want)
+    assert refsets.sam_md5(sam, bad) == REF_SETS["md5"]["dp/%d" % case]
     idx.close()
 
 
@@ -470,13 +443,10 @@ def test_populated_splice_site_db_matches_reference(h2, tmp_path):
         idx.close()
 
 
-def test_seed_search_bundled_graph_index_matches_oracle(h2, oracle_bin):
-    """The reference's bundled example index (22_20-21M_snp: 3,689 SNPs/indels, 958,359 rows over
-    954,773 nodes): every H/G/C record of 20k hard reads equals the pinned oracle's."""
-    base = os.path.join(DATA, "22_20-21M_snp")
-    fa = os.path.join(DATA, "hard20k_1.fa")
-    if not (os.path.exists(base + ".1.ht2") and os.path.exists(fa)):
-        pytest.skip("data/ not staged")
+def test_seed_search_bundled_graph_index_matches_oracle(h2, sets, oracle_bin):
+    """The graph fixture tiny_snp: every H/G/C record of 20k hard reads equals the pinned oracle's."""
+    base = os.path.join(GOLDEN, "tiny_snp")
+    fa = set_files(sets, "hard20k")[0]
     index = h2.Index(base)
     assert index.is_graph()
     batch = h2.ReadBatch.from_fasta(fa)
@@ -560,89 +530,77 @@ def test_slot_buffers_have_their_own_capacities(h2, tmp_path):
     idx.close()
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
 @pytest.mark.parametrize("name", ["reads", "hard20k", "sim200k", "len36", "len150", "len250", "len500", "len1000"])
-def test_chr22_matches_reference_binary_run_here(h2, chr22, name, tmp_path):
-    """BASELINE configs[0]/[1]-shaped inputs: SAM byte-identical to the unmodified
-    reference run on this box (-p N --reorder)."""
-    fa = os.path.join(DATA, name + "_1.fa")
-    if not os.path.exists(fa):
-        pytest.skip(fa + " not staged")
-    batch = h2.ReadBatch.from_fasta(fa)
-    sam, res = gpu_sam(chr22, batch)
+def test_chr22_matches_reference_binary_run_here(h2, tiny, sets, name):
+    """BASELINE configs[0]/[1]-shaped single-end inputs: SAM identical to the reference's."""
+    batch = h2.ReadBatch.from_fasta(set_files(sets, name)[0])
+    sam, res = gpu_sam(tiny, batch)
+    assert refsets.sam_md5(sam) == REF_SETS["md5"]["se/" + name]
+
+
+@pytest.mark.skipif(not (os.path.exists(REFBIN) and os.path.exists(os.path.join(DATA, "22_20-21M.1.ht2"))),
+                    reason="oracle/_ref and its staged data (oracle/make_data.sh) not built")
+@pytest.mark.parametrize("index,name,paired", [("22_20-21M", "sim10k", True), ("22_20-21M", "hard20k", True), ("22_20-21M", "len500", False),
+                                               ("22_20-21M_snp", "alt20k", True), ("22_20-21M_snp", "reads", False)])
+def test_example_region_indexes_match_reference_binary_run_here(h2, index, name, paired, tmp_path):
+    """Where oracle/_ref and its staged data are present: the 1 Mbp 22_20-21M example region (many local indexes; the
+    bundled graph index with 3,689 SNPs / indels) against the reference binary run on the same machine."""
+    base = os.path.join(DATA, index)
+    f1, f2 = os.path.join(DATA, name + "_1.fa"), os.path.join(DATA, name + "_2.fa")
+    idx = h2.Index(base)
+    batch = h2.ReadBatch.from_fasta(f1, path2=f2 if paired else None)
+    sam, _ = gpu_sam(idx, batch)
+    idx.close()
     out = str(tmp_path / "ref.sam")
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", os.path.join(DATA, "22_20-21M"), "-U", fa, "-S", out,
-                    "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
+    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", base] + (["-1", f1, "-2", f2] if paired else ["-U", f1]) +
+                   ["-S", out, "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
     assert sam_lines(sam) == sam_lines(open(out, "rb").read())
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
 @pytest.mark.parametrize("name", ["len250", "len1000"])
-def test_long_pairs_capacity_errors_are_flagged_never_silent(h2, chr22, name, tmp_path):
+def test_long_pairs_capacity_errors_are_flagged_never_silent(h2, tiny, sets, name):
     """2x250 bp and 2x1000 bp pairs with indels and Ns.  Capacities are compile-time (1 024 bases, 128 edits per
     trial alignment, 48 nested extensions): a pair that needs more is flagged (err != 0, counted in n_err_reads), the
-    call succeeds, and every OTHER pair is byte-identical to the reference.  2x250 no longer flags anything."""
-    f1, f2 = os.path.join(DATA, name + "_1.fa"), os.path.join(DATA, name + "_2.fa")
-    if not os.path.exists(f1):
-        pytest.skip(f1 + " not staged")
+    call succeeds, and every OTHER pair is identical to the reference.  2x250 flags nothing."""
+    f1, f2 = set_files(sets, name)
     batch = h2.ReadBatch.from_fasta(f1, path2=f2)
-    res = chr22.align(batch)
+    res = tiny.align(batch)
     bad = set(np.flatnonzero(res.reads["err"] != 0).tolist())
     assert len(bad) == res.n_err_reads and len(bad) <= (0 if name == "len250" else 150)
-    sam = chr22.sam_header() + chr22.format_sam(batch, res)
-    out = str(tmp_path / "ref.sam")
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", os.path.join(DATA, "22_20-21M"), "-1", f1, "-2", f2, "-S", out,
-                    "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    badnames = set(batch.names[2 * u].split(b"/")[0] for u in bad)
-    def keep(lines):
-        return [l for l in lines if l.startswith(b"@") or l.split(b"\t")[0] not in badnames]
-    assert keep(sam_lines(sam)) == keep(sam_lines(open(out, "rb").read()))
+    badnames = sorted(set(batch.names[2 * u].split(b"/")[0].decode() for u in bad))
+    assert badnames == REF_SETS["flagged"].get("long/" + name, [])
+    sam = tiny.sam_header() + tiny.format_sam(batch, res)
+    assert refsets.sam_md5(sam, badnames) == REF_SETS["md5"]["long/" + name]
 
 
-@pytest.mark.skipif(not os.path.exists(REFBIN), reason="oracle/_ref not built on this box")
-def test_full_size_byte_parity_1M_reads_and_500k_pairs(h2, chr22, tmp_path):
+def test_full_size_byte_parity_1M_reads_and_500k_pairs(h2, tiny):
     """BASELINE configs[1] size (1M x 101 bp SE) and the configs[2] shape (500k pairs 2x101): the bench workload's own
-    generator, FASTA bytes through ht2gpu_run_reads, byte-compared with the unmodified
-    reference run on this box; plus determinism of a second pass."""
+    generator, FASTA bytes through ht2gpu_run_reads, identical to the reference's SAM; plus determinism of a second pass."""
     sys.path.insert(0, ROOT)
     import bench
-    base = os.path.join(DATA, "22_20-21M")
     d1, d2 = bench.sim_fasta(0, 1000000)
-    f1, f2 = str(tmp_path / "m1.fa"), str(tmp_path / "m2.fa")
-    d1.tofile(f1)
-    nthr = str(min(32, os.cpu_count() or 1))
-    out = str(tmp_path / "ref.sam")
-    # 1M single-end reads
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", base, "-U", f1, "-S", out, "-p", nthr, "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    sam, st = chr22.run_reads(data1=d1)
+    hdr = tiny.sam_header()
+    sam, st = tiny.run_reads(data1=d1)
     assert st["n_reads"] == 1000000 and st["n_err_reads"] == 0
-    want = open(out, "rb").read()
-    body = want[want.index(b"\nr00000000\t") + 1:]
-    assert sam == body
+    assert refsets.sam_md5(hdr + sam) == REF_SETS["md5"]["full/se1M"]
     assert sam.count(b"\tYT:Z:UU") >= 1000000 and sam.count(b"\n") >= 1000000
-    sam2, _ = chr22.run_reads(data1=d1, batch_reads=300000)
+    sam2, _ = tiny.run_reads(data1=d1, batch_reads=300000)
     assert sam2 == sam                      # batch composition does not change a byte
-    del sam, sam2, want, body
-    # 500k pairs
+    del sam, sam2
     k = 500000
-    d1[:k * bench.RECSZ].tofile(f1); d2[:k * bench.RECSZ].tofile(f2)
-    subprocess.run([REFBIN, "--no-spliced-alignment", "-f", "-x", base, "-1", f1, "-2", f2, "-S", out, "-p", nthr, "--reorder"], check=True, stderr=subprocess.DEVNULL)
-    sam, st = chr22.run_reads(data1=d1[:k * bench.RECSZ], data2=d2[:k * bench.RECSZ])
+    sam, st = tiny.run_reads(data1=d1[:k * bench.RECSZ], data2=d2[:k * bench.RECSZ])
     assert st["n_units"] == k and st["n_err_reads"] == 0
-    want = open(out, "rb").read()
-    assert sam == want[want.index(b"\nr00000000\t") + 1:]
+    assert refsets.sam_md5(hdr + sam) == REF_SETS["md5"]["full/pe500k"]
 
 
-def test_two_devices_one_process_equal_one_device(h2, tmp_path):
+def test_two_devices_one_process_equal_one_device(h2, sets, tmp_path):
     """hisat2-b200 --gpus 2 / ht2gpu_run_reads_multi: batches round-robin over two devices of one process (index
     replicated device to device), output in input order -- byte-identical to the single-device run."""
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two CUDA devices")
-    base = os.path.join(DATA, "22_20-21M")
-    f1, f2 = os.path.join(DATA, "sim200k_1.fa"), os.path.join(DATA, "sim200k_2.fa")
-    if not os.path.exists(f1):
-        pytest.skip(f1 + " not staged")
+    base = os.path.join(GOLDEN, "tiny")
+    f1, f2 = set_files(sets, "sim200k")
     a = h2.Index(base, device=0)
     one, _ = a.run_reads(path1=f1, path2=f2, batch_reads=40000)
     b = a.peer(1)
@@ -657,15 +615,13 @@ def test_two_devices_one_process_equal_one_device(h2, tmp_path):
     assert body[body.index(b"\n@PG") + 1:].split(b"\n", 1)[1] == one
 
 
-def test_torchrun_two_ranks_concatenate_to_the_single_rank_output(h2, tmp_path):
+def test_torchrun_two_ranks_concatenate_to_the_single_rank_output(h2, sets, tmp_path):
     """The bench's N-rank layout on hardware: two torchrun ranks (NCCL broadcast of the index image, contiguous pair
     ranges) each write their shard's SAM; the rank-order concatenation equals the one-GPU output byte for byte."""
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two CUDA devices")
-    f1, f2 = os.path.join(DATA, "sim200k_1.fa"), os.path.join(DATA, "sim200k_2.fa")
-    if not os.path.exists(f1):
-        pytest.skip(f1 + " not staged")
+    f1, f2 = set_files(sets, "sim200k")
     script = str(tmp_path / "rank.py")
     open(script, "w").write("""
 import os, sys
@@ -684,10 +640,10 @@ lo, hi = shard_range(200000, rank, world)
 sam, st = idx.run_reads(path1=%r, path2=%r, skip=lo, upto=hi - lo, batch_reads=60000)
 open(os.path.join(%r, "part%%d.sam" %% rank), "wb").write(sam)
 dist.barrier(); dist.destroy_process_group()
-""" % (ROOT, os.path.join(DATA, "22_20-21M"), f1, f2, str(tmp_path)))
+""" % (ROOT, os.path.join(GOLDEN, "tiny"), f1, f2, str(tmp_path)))
     subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
                     "--master-port", "29517", script], check=True, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-    a = h2.Index(os.path.join(DATA, "22_20-21M"), device=0)
+    a = h2.Index(os.path.join(GOLDEN, "tiny"), device=0)
     one, _ = a.run_reads(path1=f1, path2=f2)
     a.close()
     assert open(str(tmp_path / "part0.sam"), "rb").read() + open(str(tmp_path / "part1.sam"), "rb").read() == one

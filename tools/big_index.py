@@ -5,7 +5,7 @@ hisat2-build-s (index construction is out of scope), then
   * parity: 200 k reads / 100 k pairs, SAM byte-compared with the reference binary run on this box;
   * throughput of the alignment path (FASTA -> SAM through ht2gpu_run_reads) and of the seed kernel alone
     (LF mapping: algorithmic GB/s against the HBM copy peak).
-Run on the GPU box:  python tools/big_index.py --mbp 512 --out profiles/r02_big_index.json
+Run on a GPU machine:  python tools/big_index.py --mbp 512 --out big_index.json
 Everything lands in data_big/ (git- and gpurun-ignored: the index is rebuilt where it is used)."""
 import argparse, ctypes, json, os, subprocess, sys, time
 import numpy as np
@@ -80,7 +80,7 @@ def main():
     os.makedirs(B, exist_ok=True)
     base = os.path.join(B, "synth%d" % args.mbp)
     res = {"what": "HBM-resident regime: %d Mbp synthetic reference (random 64-Mbp chromosomes, N gaps, 20 repeat families), "
-                   "hisat2-build-s default parameters" % args.mbp, "box": "B200 x1, gpurun, round 2"}
+                   "hisat2-build-s default parameters" % args.mbp, "gpu": bench.gpu_info(0)}
     t0 = time.time()
     chroms = make_reference(args.mbp)
     if not os.path.exists(base + ".1.ht2"):
@@ -93,7 +93,7 @@ def main():
     idx = h2.Index(base)
     res["open_s"] = round(time.time() - t0, 1)
     res["image_MB"] = round(idx.image().nbytes / 1e6, 1)
-    res["l2_MB"] = 126
+    res["l2_MB"] = 50
     hdr = idx.sam_header()
     per = 200000 // len(chroms)
     # ---- parity against the reference on this box
@@ -135,7 +135,7 @@ def main():
         if best is None or sr.ms_kernel < best[0]:
             best = (sr.ms_kernel, sr.n_lf, sr.alg_bytes)
         sr.close()
-    peak = 6565.8
+    peak = 3350.0     # H100 SXM data-sheet HBM3 bandwidth, unless MEASURED_PEAKS.json says otherwise
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peak = float(json.load(open(pk)).get("hbm_gbs", peak))

@@ -5,7 +5,7 @@ reads.  CPU only.  Every SAM difference must be confined to reads the host build
 error; anything else is reported as UNEXPLAINED.
 
   python tools/fuzz_parity.py SEED N            # tiny fixtures (tests/golden), all options incl. presets
-  python tools/fuzz_parity.py SEED N --big      # chr22 sets (data/, oracle/make_data.sh), dp-centred
+  python tools/fuzz_parity.py SEED N --big      # chr22 sets (oracle/_ref/data/, oracle/make_data.sh), dp-centred
   ... --spliced                                   # spliced mode (--no-temp-splicesite) instead of --no-spliced-alignment
 
 Option spelling follows the reference's parser quirks exactly like the CLI does (hisat2_b200_main.cpp):
@@ -16,7 +16,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(ROOT, "tests", "golden")
-D = os.path.join(ROOT, "data")
+D = os.path.join(ROOT, "oracle", "_ref", "data")
 R = os.path.join(ROOT, "oracle", "_ref", "hisat2-align-s")
 TMP = tempfile.mkdtemp(prefix="ht2fuzz")
 

@@ -1,14 +1,14 @@
 #!/usr/bin/env python3
-"""Short run for ncu: align <reads.fa> (default data/sim200k_1.fa) `iters` times."""
+"""Short run for ncu: align <reads.fa> (default oracle/_ref/data/sim200k_1.fa) `iters` times."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import hisat2_b200 as h2
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-fa = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "data", "sim200k_1.fa")
+fa = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "oracle", "_ref", "data", "sim200k_1.fa")
 iters = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 opts = dict(kv.split("=") for kv in sys.argv[3:])
 opts = {k: int(v) for k, v in opts.items()}
-idx = h2.Index(os.path.join(ROOT, "data", os.environ.get("HT2_INDEX", "22_20-21M")), **opts)
+idx = h2.Index(os.path.join(ROOT, "oracle", "_ref", "data", os.environ.get("HT2_INDEX", "22_20-21M")), **opts)
 print("opts", opts)
 if fa.startswith("synth"):          # bench.py's synthetic workload, e.g. synth:1000000
     import numpy as np

@@ -4,10 +4,10 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import hisat2_b200 as h2
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-fa = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "data", "sim200k_1.fa")
+fa = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "oracle", "_ref", "data", "sim200k_1.fa")
 batch = h2.ReadBatch.from_fasta(fa)
 for name in ("22_20-21M", "22_20-21M_snp"):
-    idx = h2.Index(os.path.join(ROOT, "data", name))
+    idx = h2.Index(os.path.join(ROOT, "oracle", "_ref", "data", name))
     best = None
     for i in range(3):
         r = idx.seed_search(batch, max_range=4)

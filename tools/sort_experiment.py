@@ -8,7 +8,7 @@ import hisat2_b200 as h2
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 fa = sys.argv[1]
 batch = h2.ReadBatch.from_fasta(fa)
-idx = h2.Index(os.path.join(ROOT, "data", "22_20-21M"))
+idx = h2.Index(os.path.join(ROOT, "oracle", "_ref", "data", "22_20-21M"))
 def time_batch(b, label):
     best = None
     for i in range(3):

@@ -17,7 +17,7 @@ else:
 ref = None
 for cfg in sys.argv[2:]:
     opts = {k: int(v) for k, v in (kv.split("=") for kv in cfg.split(","))}
-    idx = h2.Index(os.path.join(ROOT, "data", os.environ.get("HT2_INDEX", "22_20-21M")), **opts)
+    idx = h2.Index(os.path.join(ROOT, "oracle", "_ref", "data", os.environ.get("HT2_INDEX", "22_20-21M")), **opts)
     best = None
     for i in range(3):
         r = idx.align(batch)
