@@ -87,7 +87,7 @@ EXPORTS = [
     "ht2gpu_sam_slots", "ht2gpu_submit_sam", "ht2gpu_wait_sam", "ht2gpu_align_sam", "ht2gpu_run_reads",
     "ht2gpu_host_alloc", "ht2gpu_host_free", "ht2gpu_set_error", "ht2gpu_parse_reads", "ht2gpu_free_parsed",
     "ht2gpu_ctx_get", "ht2gpu_ctx_set", "ht2gpu_run_reads_multi", "ht2gpu_open_peer", "ht2gpu_sw_selftest", "ht2gpu_load_splicesites", "ht2gpu_collect_splicesites",
-    "ht2gpu_write_novel_splicesites",
+    "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry",
 ]
 
 
@@ -156,6 +156,7 @@ def load_library(path=None):
     lib.ht2gpu_load_splicesites.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.POINTER(C.c_uint32)]
     lib.ht2gpu_collect_splicesites.argtypes = [C.c_void_p, C.c_int]
     lib.ht2gpu_write_novel_splicesites.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.POINTER(C.c_uint64)]
+    lib.ht2gpu_launch_geometry.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
     if path is None:
         _lib = lib
     return lib
@@ -578,6 +579,12 @@ class Index(object):
 
     def is_graph(self):
         return bool(self._lib.ht2gpu_index_is_graph(self._h))
+
+    def geometry(self):
+        """ht2gpu_launch_geometry: (warps per block, read slots per lane, blocks per SM) of the alignment kernel."""
+        out = (C.c_int32 * 3)()
+        self._check(self._lib.ht2gpu_launch_geometry(self._h, out), "ht2gpu_launch_geometry")
+        return tuple(int(v) for v in out)
 
     def seed_search(self, batch, max_range=4):
         """ht2gpu_seed_search: partial-search chains + coordinates of small ranges."""

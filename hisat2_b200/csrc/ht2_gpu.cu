@@ -625,6 +625,7 @@ struct WorkPool {
     cudaEvent_t    evDone;        // recorded after the latest kernels of a batch (alignment + SAM)
     Ht2SwScratch*  dSw;           // --bowtie2-dp scratch per launched thread (allocated on first use)
     uint32_t*      dSwPool;
+    size_t         swThreads;     // launched threads dSw / dSwPool hold: geometries of equal nWork differ in grid size
     std::mutex     mu;            // [wait, launches, record] of one batch are one critical section
     int            refs;
 };
@@ -781,7 +782,7 @@ static int finishOpen(ht2gpu_handle* h)
         if (!wp) {
             wp = new WorkPool();
             wp->device = h->device; wp->nWork = h->nWork; wp->refs = 0;
-            wp->dWork = NULL; wp->dSw = NULL; wp->dSwPool = NULL;
+            wp->dWork = NULL; wp->dSw = NULL; wp->dSwPool = NULL; wp->swThreads = 0;
             CK(cudaMalloc(&wp->dWork, wp->nWork * sizeof(Ht2Work)));
             CK(cudaMemset(wp->dWork, 0, wp->nWork * sizeof(Ht2Work)));
             CK(cudaEventCreateWithFlags(&wp->evDone, cudaEventDisableTiming));
@@ -789,9 +790,17 @@ static int finishOpen(ht2gpu_handle* h)
             CK(cudaDeviceSynchronize());
             gPools.push_back(wp);
         }
-        if (h->P.bowtie2Dp && !wp->dSw) {   // dynamic-programming scratch (ht2_sw.h): per executing thread, not per read slot
+        if (h->P.bowtie2Dp && wp->swThreads < nThreads) {
+            // dynamic-programming scratch (ht2_sw.h): per executing thread, not per read slot.  Geometries with the same
+            // nWork share the pool but not the grid (8x4 and blocks_per_sm=2 x 2 slots: twice the threads), so the
+            // scratch grows to the largest grid once the pool's kernels are done.
+            std::lock_guard<std::mutex> lw(wp->mu);
+            CK(cudaEventSynchronize(wp->evDone));
+            cudaFree(wp->dSw); cudaFree(wp->dSwPool);
+            wp->dSw = NULL; wp->dSwPool = NULL; wp->swThreads = 0;
             CK(cudaMalloc(&wp->dSw, nThreads * sizeof(Ht2SwScratch)));
             CK(cudaMalloc(&wp->dSwPool, nThreads * (size_t)HT2_SW_POOL_WORDS * sizeof(uint32_t)));
+            wp->swThreads = nThreads;
         }
         wp->refs++;
         h->pool = wp;
@@ -931,6 +940,12 @@ extern "C" const void* ht2gpu_image_data(const ht2gpu_handle_t* h) { return h &&
 extern "C" size_t ht2gpu_image_bytes(const ht2gpu_handle_t* h) { return h ? h->blobBytes : 0; }
 extern "C" const void* ht2gpu_device_image(const ht2gpu_handle_t* h) { return h ? h->dBlob : NULL; }
 extern "C" const char* ht2gpu_last_error(const ht2gpu_handle_t* h) { return h ? h->err.c_str() : "null handle"; }
+extern "C" int ht2gpu_launch_geometry(const ht2gpu_handle_t* h, int32_t out[3])
+{
+    if (!h || !out || !h->pool) return HT2GPU_ERR_ARG;
+    out[0] = h->poolWarps; out[1] = h->rgK; out[2] = h->bpsm;
+    return HT2GPU_OK;
+}
 extern "C" uint32_t ht2gpu_num_refs(const ht2gpu_handle_t* h) { return h && h->img ? h->img->header()->nRefs : 0; }
 extern "C" const char* ht2gpu_ref_name(const ht2gpu_handle_t* h, uint32_t i) { return h->img->refName(i); }
 extern "C" uint32_t ht2gpu_ref_len(const ht2gpu_handle_t* h, uint32_t i) { return h->img->refPlen(i); }
@@ -1051,6 +1066,11 @@ static int ensureOut(ht2gpu_handle* h, SamSlot& S, uint32_t units, size_t alns, 
 static int launchAlign(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* b, uint32_t units, cudaEvent_t evStart = NULL)
 {
     WorkPool* wp = h->pool;
+    const uint32_t grid = (uint32_t)(h->nSM * h->bpsm);
+    if (h->P.bowtie2Dp && wp->swThreads < (size_t)grid * h->tpb) {   // every launched thread indexes its own DP scratch
+        h->err = "the workspace pool's DP scratch is smaller than the launch grid";
+        return HT2GPU_ERR_ARG;
+    }
     DevBatch db;
     db.seq = S.dSeq; db.qual = b->qual ? S.dQual : NULL; db.offs = S.dOffs; db.seeds = S.dSeeds;
     db.n_units = units; db.paired = b->paired; db.sw = h->P.bowtie2Dp ? wp->dSw : NULL; db.swPool = h->P.bowtie2Dp ? wp->dSwPool : NULL; db.minscTab = h->dMinsc;
@@ -1066,7 +1086,6 @@ static int launchAlign(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* 
     CK(cudaMemsetAsync(S.dCounters, 0, 8 * sizeof(unsigned int), S.stream));
     if (evStart) CK(cudaEventRecord(evStart, S.stream));   // kernel time is counted from here: after the waits for the previous kernels
     Ht2Work* work = wp->dWork;
-    const uint32_t grid = (uint32_t)(h->nSM * h->bpsm);
     const bool nospl = h->P.noSplicedAlignment != 0;   // the DNA-only instantiation has less code (DESIGN.md 4.1)
     if (h->graph) {
         if (nospl) ht2_align_pool_kernel<8, 4, true, true><<<grid, 256, 0, S.stream>>>(h->dBlob, h->P, db, o, work);

@@ -361,6 +361,10 @@ int ht2gpu_write_novel_splicesites(ht2gpu_handle_t** hs, int n, const char* path
  * problems (aligner_swsse_ee_u8.cpp:791-1163 restated twice, ht2_sw.h).  out[0] = mismatching cells / scores
  * (must be 0), out[1] = problems run, out[2] = cells compared per plane, out[3] = problems with a valid best. */
 int ht2gpu_sw_selftest(int device, uint32_t n, uint32_t seed, uint64_t out[4]);
+/* Diagnostics: the geometry of the handle's alignment kernel.  out[0] = warps per block, out[1] = read slots per
+ * lane, out[2] = blocks per SM.  The slots can differ from the options: a default handle on a device without room
+ * for the 4-slot workspace, or in a process that already holds the 2-slot one, runs with 2. */
+int ht2gpu_launch_geometry(const ht2gpu_handle_t* h, int32_t out[3]);
 
 const char* ht2gpu_last_error(const ht2gpu_handle_t* h);
 int ht2gpu_close(ht2gpu_handle_t* h);

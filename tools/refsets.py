@@ -3,6 +3,7 @@
 tiny.snp) by the seeded generators tools/simreads.py and tools/altreads.py, so that a checkout needs nothing else.
 
   python tools/refsets.py        # writes tests/golden/ref_sets.json: md5 of the unmodified reference's SAM per case
+  python tools/refsets.py --edge # only the edge/* cases (tools/edgereads.py); also writes tests/golden/edge_se.sam
 
 The expected values come from oracle/_ref/hisat2-align-s (oracle/Makefile).  Cases whose reads can hit a fixed device
 capacity list the flagged reads (`flagged`, from a GPU run of the library); their md5 excludes those reads' records."""
@@ -43,6 +44,39 @@ DP_CASES = [
 ]
 
 
+def _edge_cases():
+    """edge/<case>: the tools/edgereads.py corpus.  case -> (index, files, format flag, reference flags, library options,
+    front-end options of ht2gpu_reads_input_t).  Every case but `near` also runs as <case>_dp with --bowtie2-dp 2: on
+    near_A0_624 (a 250-base read with an insertion, overhanging the start of chrA) the reference under --bowtie2-dp 2
+    asks for a 32 GiB DP matrix and aborts."""
+    sys.path.insert(0, TOOLS)
+    import edgereads
+    cases = {
+        "se": ("tiny", ["se.fa"], "-f", [], {}, {}),
+        "near": ("tiny", ["near.fa"], "-f", [], {}, {}),
+        "pe": ("tiny", ["pe_1.fa", "pe_2.fa"], "-f", [], {}, {}),
+        "graph_se": ("tiny_snp", ["se.fa"], "-f", [], {}, {}),
+        "fq": ("tiny", ["q.fq"], "-q", [], {}, {}),
+        # --mp 42,2 makes a Q41+ mismatch cost more than a Q40 one unless the quality is clamped at 40
+        "fq_mp42": ("tiny", ["q.fq"], "-q", ["--mp", "42,2", "--score-min", "L,0,-1.5"],
+                    dict(mp_max=42, mp_min=2, score_min_type=ord("L"), score_min_const=0.0, score_min_coeff=-1.5), {}),
+        "fq64": ("tiny", ["q64.fq"], "-q", ["--phred64"], {}, dict(phred64=1)),
+        "fq_trim": ("tiny", ["q.fq"], "-q", ["-5", "3", "-3", "5"], {}, dict(trim5=3, trim3=5)),
+    }
+    for i, sm in enumerate(edgereads.SCORE_MIN):
+        flag = edgereads.score_min_flag(sm)
+        opts = {} if flag is None else dict(score_min_type=ord(sm[0]), score_min_const=sm[1], score_min_coeff=sm[2])
+        cases["sc%d" % i] = ("tiny", ["sc%d.fa" % i], "-f", [] if flag is None else ["--score-min", flag], opts, {})
+    for k in [k for k in cases if k != "near"]:
+        index, fs, fmt, flags, opts, front = cases[k]
+        cases[k + "_dp"] = (index, fs, fmt, flags + ["--bowtie2-dp", "2"], dict(opts, bowtie2_dp=2), front)
+    return cases
+
+
+EDGE_CASES = _edge_cases()
+EDGE_SEED = 11
+
+
 def load_expected():
     return json.load(open(OUT))
 
@@ -59,6 +93,19 @@ def generate(outdir, names=None):
     return outdir
 
 
+def generate_edge(outdir):
+    """The tools/edgereads.py corpus under outdir (edge_*); returns outdir."""
+    sys.path.insert(0, TOOLS)
+    import edgereads
+    if not os.path.exists(os.path.join(outdir, "edge_se.fa")):
+        edgereads.generate(os.path.join(GOLDEN, "tiny.fa"), os.path.join(outdir, "edge"), EDGE_SEED)
+    return outdir
+
+
+def edge_files(d, case):
+    return [os.path.join(d, "edge_" + f) for f in EDGE_CASES[case][1]]
+
+
 def sam_md5(sam, exclude=()):
     """md5 of the SAM lines without @PG (and without the records of the read names in `exclude`)."""
     if isinstance(sam, str):
@@ -73,18 +120,27 @@ def files(d, name, paired):
     return ["-1", f1, "-2", f2] if paired else ["-U", f1]
 
 
-def reference(d, index, name, paired, flags=(), fa=False):
+def reference(d, index, name, paired, flags=(), fa=False, fmt="-f"):
+    """SAM of the unmodified reference (--reorder).  fmt is -f or -q; flags may hold any of its alignment and input
+    options (--score-min, --phred64, -5 / -3, ...)."""
     out = os.path.join(d, "ref.sam")
-    subprocess.run([REFBIN, "-f", "-x", os.path.join(GOLDEN, index)] + list(flags or ["--no-spliced-alignment"]) +
+    subprocess.run([REFBIN, fmt, "-x", os.path.join(GOLDEN, index)] + list(flags or ["--no-spliced-alignment"]) +
                    (fa if fa else files(d, name, paired)) + ["-S", out, "-p", str(min(16, os.cpu_count() or 1)), "--reorder"],
                    check=True, stderr=subprocess.DEVNULL)
     return open(out, "rb").read()
 
 
-def main():
+def main(edge_only=False):
     old = json.load(open(OUT)) if os.path.exists(OUT) else {}
     flagged = old.get("flagged", {})
     md5 = {}
+    if edge_only:
+        md5 = {k: v for k, v in old.get("md5", {}).items() if not k.startswith("edge/")}
+        with tempfile.TemporaryDirectory() as d:
+            edge_reference(d, md5, flagged)
+        json.dump({"md5": md5, "flagged": flagged}, open(OUT, "w"), indent=1, sort_keys=True)
+        open(OUT, "a").write("\n")
+        return
     with tempfile.TemporaryDirectory() as d:
         generate(d)
         for name in ("sim10k", "hard20k", "len36", "len150", "len500", "sim200k"):
@@ -110,9 +166,23 @@ def main():
         k = 500000
         d1[:k * bench.RECSZ].tofile(f1); d2[:k * bench.RECSZ].tofile(f2)
         md5["full/pe500k"] = sam_md5(reference(d, "tiny", None, True, fa=["-1", f1, "-2", f2]))
+        edge_reference(d, md5, flagged)
     json.dump({"md5": md5, "flagged": flagged}, open(OUT, "w"), indent=1, sort_keys=True)
     open(OUT, "a").write("\n")
 
 
+def edge_reference(d, md5, flagged):
+    """edge/<case> md5s; the reference SAM of edge/se is also kept as tests/golden/edge_se.sam."""
+    generate_edge(d)
+    for case, (index, _, fmt, flags, _, _) in sorted(EDGE_CASES.items()):
+        fs = edge_files(d, case)
+        key = "edge/" + case
+        sam = reference(d, index, None, len(fs) == 2, ["--no-spliced-alignment"] + flags, fmt=fmt,
+                        fa=["-1", fs[0], "-2", fs[1]] if len(fs) == 2 else ["-U", fs[0]])
+        md5[key] = sam_md5(sam, flagged.get(key, ()))
+        if case == "se":
+            open(os.path.join(GOLDEN, "edge_se.sam"), "wb").write(b"".join(l for l in sam.splitlines(True) if not l.startswith(b"@PG")))
+
+
 if __name__ == "__main__":
-    main()
+    main(edge_only="--edge" in sys.argv[1:])
