@@ -739,8 +739,8 @@ static int finishOpen(ht2gpu_handle* h)
 #ifndef HT2_ENABLE_SPLICED
     if (!h->opt.no_spliced_alignment) { h->err = "spliced alignment is not implemented in this build; pass --no-spliced-alignment"; return HT2GPU_ERR_UNSUPPORTED; }
 #else
-    // experimental library build (HT2_SPLICED=1 python -m hisat2_b200.build): spliced mode == the reference's
-    // --no-temp-splicesite without known splice sites (empty splice-site DB); not yet run on a GPU
+    // spliced mode (the default build; HT2_NO_SPLICED=1 leaves it out) == the reference's --no-temp-splicesite: the
+    // splice-site DB holds only the sites loaded with ht2gpu_load_splicesites, never junctions of earlier reads
     if (!h->opt.no_spliced_alignment) {
         const Ht2SplTables& T = ht2_spl_tables();
         CK(cudaMalloc(&h->dSplT, sizeof(Ht2SplTables)));

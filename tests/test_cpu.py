@@ -1,4 +1,5 @@
 """CPU-side tests (no GPU): oracle vs golden vectors, host logic, C ABI."""
+import hashlib
 import os
 import re
 import subprocess
@@ -9,7 +10,16 @@ import pytest
 
 from conftest import GOLDEN, ROOT, sam_lines
 
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+import refsets  # noqa: E402
+
+REF_SETS = refsets.load_expected()
 KEEP = set(list(range(0, 100)) + list(range(250, 350)) + list(range(500, 600)))
+
+
+@pytest.fixture(scope="session")
+def spliced_dir(tmp_path_factory):
+    return refsets.generate_spliced(str(tmp_path_factory.mktemp("spliced")))
 
 
 def test_oracle_matches_reference_dump(oracle_bin):
@@ -134,8 +144,8 @@ def test_spliced_alignment_host_build_matches_golden_reference_sam(hostsim_splic
     edits, the spliced branch of combineWith (motif classes, intron-length rules, probability model),
     calculateScore for splice edits, N / XS:A / fragment lengths in SAM -- against golden SAM of the
     unmodified reference: 400 RNA-like reads over one or two introns (340 spliced alignments), the DNA
-    fixtures SE / PE FASTQ, and ALT-allele pairs on the graph index.  The CUDA library still refuses
-    spliced mode (these pieces are not on the device yet)."""
+    fixtures SE / PE FASTQ, and ALT-allele pairs on the graph index.  The CUDA library compiles the same
+    pieces into its kernels (tests/test_gpu.py and tests/test_geometry_edges.py run them on the device)."""
     env = dict(os.environ, HT2_OPTS="spliced=1")
     for idx, args, gold in (("tiny", ["tiny_rna.fa"], "tiny_spliced_rna.sam"), ("tiny", ["tiny_se.fa"], "tiny_spliced_se.sam"),
                             ("tiny", ["tiny_pe_1.fq", "tiny_pe_2.fq"], "tiny_spliced_pe_fq.sam"),
@@ -204,6 +214,45 @@ def test_populated_splice_site_db_host_build_matches_golden_reference_sam(hostsi
     open(bad, "w").write("chrA\t100\n")
     r = subprocess.run([hostsim_spliced_bin, "tiny", "tiny_rna.fa", str(tmp_path / "o5.sam")], cwd=GOLDEN, stderr=subprocess.PIPE, env=dict(env, HT2_SS=bad))
     assert r.returncode != 0 and b"truncated splice-site record" in r.stderr
+
+
+@pytest.mark.parametrize("case", sorted(refsets.SPLICED_CASES))
+def test_spliced_corpus_host_build_matches_reference(hostsim_spliced_bin, spliced_dir, tmp_path, case):
+    """The spliced corpus (tools/splicereads.py: every motif, anchors of 1-30 bases, intron lengths at every rule
+    boundary, several junctions per read, sequence ends and the N gap) and its simulated bulk through the host build
+    of the spliced aligner: the md5 of the reference's SAM (--no-temp-splicesite) for every spliced/* case, and of its
+    --novel-splicesite-outfile where recorded.  The reads the library flags for a device capacity are the recorded
+    ones (the host build has the device's capacities) and are left out of the md5, as on the GPU."""
+    index, _, _, _, opts, _ = refsets.SPLICED_CASES[case]
+    fs, ss = refsets.spliced_files(spliced_dir, case)
+    out, novel = str(tmp_path / "o.sam"), str(tmp_path / "novel.txt")
+    env = dict(os.environ, HT2_OPTS=",".join(["spliced=1"] + ["%s=%s" % kv for kv in sorted(opts.items())]))
+    if ss:
+        env["HT2_SS"] = ss
+    if case in refsets.SPLICED_NOVEL:
+        env["HT2_SS_OUT"] = novel
+    r = subprocess.run([hostsim_spliced_bin, index, fs[0], out] + fs[1:], cwd=GOLDEN, check=True, stderr=subprocess.PIPE, env=env)
+    key = "spliced/" + case
+    bad = sorted(set(re.findall(r"(?:read|pair) \d+ \(([^)/]*)[^)]*\): err=", r.stderr.decode())))
+    assert bad == REF_SETS["flagged"].get(key, [])
+    sam = open(out, "rb").read()
+    assert refsets.sam_md5(sam, bad) == REF_SETS["md5"][key]
+    assert sum(1 for l in sam_lines(sam) if not l.startswith(b"@") and b"N" in l.split(b"\t")[5]) > 250
+    if case in refsets.SPLICED_NOVEL:
+        assert hashlib.md5(open(novel, "rb").read()).hexdigest() == REF_SETS["md5"]["spliced_novel/" + case]
+
+
+def test_spliced_corpus_is_deterministic(tmp_path):
+    """tools/splicereads.py writes the same bytes for the same seed, and the recorded md5s belong to those bytes."""
+    import splicereads
+    a, b = str(tmp_path / "a"), str(tmp_path / "b")
+    splicereads.generate(os.path.join(GOLDEN, "tiny.fa"), a, refsets.SPLICE_SEED)
+    splicereads.generate(os.path.join(GOLDEN, "tiny.fa"), b, refsets.SPLICE_SEED)
+    for suffix in ("_se.fa", "_q.fq", "_pe_1.fa", "_pe_2.fa", "_ss.txt", "_sim.fa", "_sim_1.fa", "_sim_2.fa", "_sim_ss.txt"):
+        assert open(a + suffix, "rb").read() == open(b + suffix, "rb").read(), suffix
+    names = [l[1:].split("_")[0] for l in open(a + "_se.fa").read().split() if l.startswith(">")]
+    assert 1800 < len(names) < 4000
+    assert {"motif", "anchor", "len", "multi", "sense", "redge", "gap", "join"} <= set(names)
 
 
 def test_striped_dp_fill_and_backtrace_against_plain_scalar_dp(hostsim_bin):

@@ -1,13 +1,15 @@
-"""The edge-read corpus (tools/edgereads.py) under every launch geometry of the alignment kernel, and a plain restatement
-of the alignment score.
+"""The edge-read corpus (tools/edgereads.py) and the spliced corpus (tools/splicereads.py) under every launch geometry
+of the alignment kernel, and a plain restatement of the alignment score, splices included.
 
 The pool kernel has four linear-index instantiations (8 warps x 4 read slots, the DNA-only 8 x 2 that a default handle
 falls back to when the device lacks room for the 4-slot workspace, 4 x 8, and any of them with several blocks per SM).
 Every one must write the reference's SAM, so every case runs under each and asserts which kernel ran
 (Index.geometry()).  score_record() recomputes AS:i, XM, XO, XG, NM, YS:i and the --score-min test from each record's
-CIGAR, MD:Z, SEQ and QUAL with exact integers (numpy.float32 where the reference computes in float); it is pinned to the
-reference by the committed golden SAMs (CPU) and applied to every GPU run."""
+CIGAR, MD:Z, SEQ and QUAL with exact integers (numpy.float32 where the reference computes in float), and the splice
+penalties from the reference sequence at each intron; it is pinned to the reference by the committed golden SAMs (CPU)
+and applied to every GPU run."""
 import glob
+import math
 import os
 import sys
 
@@ -25,8 +27,24 @@ REF_SETS = refsets.load_expected()
 # ---------------------------------------------------------------------------------------------------------------------
 # score_record: the reference's end-to-end scoring (Scoring::mm / n / sc / readGap / refGap, SimpleFunc::f) restated
 # ---------------------------------------------------------------------------------------------------------------------
+# Splice motifs by the intron's first and last two reference bases (hi_aligner.h: GT-AG and its reverse complement
+# CT-AC are canonical; GC-AG, AT-AC and their reverse complements CT-GC, GT-AT are semi-canonical; anything else is
+# non-canonical and has no sense).  '+' / '-' is the transcript strand of XS:A.
+MOTIFS = {("GT", "AG"): ("can", "+"), ("CT", "AC"): ("can", "-"), ("GC", "AG"): ("semi", "+"), ("AT", "AC"): ("semi", "+"),
+          ("CT", "GC"): ("semi", "-"), ("GT", "AT"): ("semi", "-")}
+
+
+def intron_pen(n):
+    """--pen-canintronlen / --pen-noncanintronlen G,-8,1: max(0, (int)(-8 + ln(n))) in double."""
+    return max(0, int(-8.0 + math.log(n)))
+
+
+# can_pen / noncan_pen: --pen-cansplice 0 / --pen-noncansplice 12 (semi-canonical motifs pay the non-canonical one)
 DEFAULT_SCORING = dict(mp_max=6, mp_min=2, sp_max=2, sp_min=1, np=1, rdg_const=5, rdg_linear=3, rfg_const=5, rfg_linear=3,
-                       ignore_quals=0, score_min=None)
+                       ignore_quals=0, score_min=None, can_pen=0, noncan_pen=12, intron_pen=intron_pen, motifs=MOTIFS)
+MIN_INTRON_LEN = 20          # --min-intronlen: a shorter reference skip is a deletion
+MIN_ANCHOR = 7               # minAnchorLen (canonical) / minAnchorLenNoncan (semi- and non-canonical)
+MIN_ANCHOR_NONCAN = 14
 F32 = np.float32
 
 
@@ -103,15 +121,70 @@ def known_alt_positions(zs):
     return pos
 
 
-def score_record(line, o=DEFAULT_SCORING):
+_TINY = []
+
+
+def tiny_contigs():
+    """{name: bases} of tests/golden/tiny.fa, the sequence of both committed indexes (tiny, tiny_snp)."""
+    if not _TINY:
+        _TINY.append({k: v.decode() for k, v in edgereads.load_contigs(os.path.join(GOLDEN, "tiny.fa")).items()})
+    return _TINY[0]
+
+
+def load_sites(*paths):
+    """{(chrom, last exon base, first base after the intron)} of splice-site files (0-based, the files' convention)."""
+    out = set()
+    for p in paths:
+        for l in open(p):
+            t = l.split()
+            if len(t) >= 3:
+                out.add((t[0], int(t[1]), int(t[2])))
+    return out
+
+
+def record_introns(f, o=DEFAULT_SCORING, ref=None, sites=frozenset()):
+    """The N operations of a split SAM record as dicts: length, motif class ('can', 'semi' or None), sense ('+', '-' or
+    None), whether the site list holds it, and the aligned bases (M) left and right of it in the read."""
+    ref = tiny_contigs() if ref is None else ref
+    chrom, rp = f[2], int(f[3]) - 1
+    cig = parse_cigar(f[5])
+    out = []
+    for k, (op, n) in enumerate(cig):
+        if op == "N":
+            motif = (ref[chrom][rp:rp + 2], ref[chrom][rp + n - 2:rp + n])
+            cls, sense = o["motifs"].get(motif, (None, None))
+            out.append(dict(len=n, cls=cls, sense=sense, known=(chrom, rp - 1, rp + n) in sites,
+                            left=sum(m for c, m in cig[:k] if c == "M"), right=sum(m for c, m in cig[k + 1:] if c == "M")))
+        if op in "MDN":
+            rp += n
+    return out
+
+
+def splice_penalty(introns, o=DEFAULT_SCORING):
+    """What the introns of one alignment cost (an intron of the site list costs nothing)."""
+    return sum(o["intron_pen"](i["len"]) + (o["can_pen"] if i["cls"] == "can" else o["noncan_pen"])
+               for i in introns if not i["known"])
+
+
+def score_record(line, o=DEFAULT_SCORING, ref=None, sites=frozenset()):
     """Recompute (AS, XM, XO, XG, NM) of an aligned SAM record from CIGAR, MD:Z, SEQ and QUAL, or None if unaligned.
     Phred qualities are SAM's (+33).  AS:i is read from the record only where reference Ns leave a choice: it must then
-    be the computed penalty plus 0..(number of reference Ns) N penalties."""
+    be the computed penalty plus 0..(number of reference Ns) N penalties.  A spliced record (N in its CIGAR) is scored
+    as the same record without its Ns, minus splice_penalty() of its introns: their motifs come from `ref` (tiny.fa by
+    default), and those in `sites` are free, or else all of them are charged."""
     f = line.split("\t")
     if int(f[1]) & 4:
         return None
     tags = parse_tags(f)
     cig = parse_cigar(f[5])
+    spl = alt_spl = 0
+    if any(op == "N" for op, _ in cig):
+        introns = record_introns(f, o, ref, sites)
+        spl = splice_penalty(introns, o)
+        # a listed intron costs nothing if the search path that found the alignment consulted the site list; the
+        # reference charges some listed introns as unlisted ones (secondary alignments, alignments through a graph ALT)
+        alt_spl = splice_penalty([dict(i, known=False) for i in introns], o)
+    cig = [c for c in cig if c[0] != "N"]
     seq, qual = f[9], [ord(c) - 33 for c in f[10]]
     md = parse_md(tags["MD"])
     alts = known_alt_positions(tags["Zs"]) if "Zs" in tags else set()
@@ -171,6 +244,9 @@ def score_record(line, o=DEFAULT_SCORING):
         else:
             raise AssertionError("CIGAR op %s: %s" % (op, line))
     assert rd == len(seq) and left == 0 and mi == len(md), line
+    if alt_spl != spl and int(tags["AS"]) == -(pen + alt_spl):
+        spl = alt_spl
+    pen += spl
     if ref_n:
         as_ = int(tags["AS"])
         if -pen - ref_n * o["np"] <= as_ <= -pen and (pen + as_) % o["np"] == 0:
@@ -178,9 +254,43 @@ def score_record(line, o=DEFAULT_SCORING):
     return -pen, xm, xo, xg, nm
 
 
-def check_records(sam, o=DEFAULT_SCORING):
-    """score_record against every aligned record without an N (splice) in its CIGAR; YS:i against the mate's AS:i.
-    Returns the number of records checked."""
+def max_intron_len(cls, anchor):
+    """The longest unknown intron an alignment may have when its shorter anchor is `anchor` bases and it has no other
+    edit (MaxIntronLen): 2^clamp(2a - 4, 13, 30) canonical, 2^min(2a - 10, 30) otherwise; 0 below the minimum anchor."""
+    if cls == "can":
+        return 1 << min(max(2 * anchor - 4, 13), 30) if anchor >= MIN_ANCHOR else 0
+    return 1 << min(2 * max(anchor, 5) - 10, 30) if anchor >= MIN_ANCHOR_NONCAN else 0
+
+
+def check_splices(f, tags, o=DEFAULT_SCORING, ref=None, sites=frozenset()):
+    """The splice rules a split record must satisfy beyond its score: every N is an intron of at least --min-intronlen
+    bases; XS:A never contradicts the sense of an intron's motif, is absent when two canonical introns' senses
+    disagree, and is the sense of the motifs when every intron is canonical and they agree; an unknown intron of a
+    record with no other edit respects MaxIntronLen of its shorter anchor.  (XS:A is the direction the aligner recorded
+    with the splice, not a function of the final CIGAR: the reference gives some non-canonical introns the sense '-'
+    and some semi-canonical introns none, so only canonical introns pin it.)"""
+    introns = record_introns(f, o, ref, sites)
+    line = "\t".join(f)
+    assert all(i["len"] >= MIN_INTRON_LEN for i in introns), line
+    senses = set(i["sense"] for i in introns) - {None}
+    xs = tags.get("XS")
+    if len(set(i["sense"] for i in introns if i["cls"] == "can")) > 1:
+        assert xs is None, line
+    if senses:
+        assert xs in (None,) + tuple(senses), line
+        if all(i["cls"] == "can" for i in introns) and len(senses) == 1:
+            assert xs == senses.pop(), line
+    cig = parse_cigar(f[5])
+    if len(introns) == 1 and not introns[0]["known"] and int(tags["NM"]) == 0 and all(op in "MN" for op, _ in cig):
+        i = introns[0]
+        assert i["len"] <= max_intron_len(i["cls"], min(i["left"], i["right"])), line
+    return introns
+
+
+def check_records(sam, o=DEFAULT_SCORING, ref=None, sites=frozenset(), stats=None):
+    """score_record against every aligned record, spliced ones with check_splices as well; YS:i against the mate's AS:i.
+    Returns the number of records checked; `stats`, a dict, collects the spliced records checked ('spliced') and the
+    lengths of their introns ('intron_lens')."""
     recs = [l for l in (sam.decode() if isinstance(sam, bytes) else sam).splitlines() if l and not l.startswith("@")]
     primary_as = {}
     for l in recs:
@@ -195,25 +305,42 @@ def check_records(sam, o=DEFAULT_SCORING):
         if flag & 1 and not flag & 0x108 and "YS" in tags:
             mate = primary_as.get((f[0], (flag & 0xC0) ^ 0xC0))
             assert mate is not None and int(tags["YS"]) == mate, l
-        if flag & 4 or "N" in f[5]:
+        if flag & 4:
             continue
-        got = score_record(l, o)
+        got = score_record(l, o, ref, sites)
         want = tuple(int(tags[k]) for k in ("AS", "XM", "XO", "XG", "NM"))
         assert got == want, "%s\nrecomputed AS/XM/XO/XG/NM %s" % (l, got)
         assert got[0] >= min_score(o, len(f[9])), l
+        if "N" in f[5]:
+            introns = check_splices(f, tags, o, ref, sites)
+            if stats is not None:
+                stats["spliced"] = stats.get("spliced", 0) + 1
+                stats.setdefault("intron_lens", set()).update(i["len"] for i in introns)
         n += 1
     return n
 
 
+def golden_sites(path):
+    """The splice-site list a golden SAM was made with (empty for the runs without --known-splicesite-infile)."""
+    name = os.path.basename(path)
+    if name == "tiny_ss_rna_pe_known_novel.sam":
+        return load_sites(os.path.join(GOLDEN, "tiny_ss_known.txt"), os.path.join(GOLDEN, "tiny_ss_novel.txt"))
+    if "_ss_rna_" in name:
+        return load_sites(os.path.join(GOLDEN, "tiny_ss_rna_ss.txt"))
+    return frozenset()
+
+
 def test_score_restatement_matches_every_golden_sam():
     """Every aligned record of every committed golden SAM of the reference (default scoring; FASTA and FASTQ, SE and PE,
-    linear and graph indexes, spliced mode without the spliced records, the edge corpus): AS:i, XM, XO, XG, NM and YS:i
-    equal score_record's, and AS >= minsc(len)."""
-    total, files = 0, 0
+    linear and graph indexes, spliced mode with and without a splice-site list, the edge corpora): AS:i, XM, XO, XG, NM
+    and YS:i equal score_record's, AS >= minsc(len), and spliced records keep the splice rules of check_splices.  The
+    spliced edge corpus holds introns on both sides of the first two intron-length penalty steps."""
+    total, files, stats = 0, 0, {}
     for path in sorted(glob.glob(os.path.join(GOLDEN, "*.sam"))):
-        total += check_records(open(path, "rb").read())
+        total += check_records(open(path, "rb").read(), sites=golden_sites(path), stats=stats)
         files += 1
-    assert files >= 19 and total > 9000
+    assert files >= 20 and total > 9000 and stats["spliced"] > 1500
+    assert {8103, 8104, 22026, 22027} <= stats["intron_lens"]
 
 
 def test_score_restatement_detects_changed_penalties():
@@ -229,6 +356,21 @@ def test_score_restatement_detects_changed_penalties():
     assert clipped
     off = dict(DEFAULT_SCORING, sp_max=3)
     assert any(score_record(l, off) != score_record(l) for l in clipped)
+    # the splice terms: the first intron-length step at 8105 instead of 8104, --pen-noncansplice 11, or the two
+    # semi-canonical classes' senses swapped each disagree with a golden spliced record
+    assert [intron_pen(n) for n in (8103, 8104, 22026, 22027)] == [0, 1, 1, 2]
+    swapped = {m: (c, {"+": "-", "-": "+"}[s] if c == "semi" else s) for m, (c, s) in MOTIFS.items()}
+    for o in (dict(DEFAULT_SCORING, intron_pen=lambda n: intron_pen(n - 1)), dict(DEFAULT_SCORING, noncan_pen=11),
+              dict(DEFAULT_SCORING, motifs=swapped)):
+        assert any(golden_disagrees(path, o) for path in sorted(glob.glob(os.path.join(GOLDEN, "*.sam"))))
+
+
+def golden_disagrees(path, o):
+    try:
+        check_records(open(path, "rb").read(), o, sites=golden_sites(path))
+    except AssertionError:
+        return True
+    return False
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -302,9 +444,9 @@ def scoring_of(opts):
     return o
 
 
-def run_case(idx, batch, paired, opts):
-    """Align; device SAM == host formatter's for every read no capacity flagged; the restatement holds on every record.
-    Returns (header + host SAM, sorted flagged read names)."""
+def run_case(idx, batch, paired, opts, sites=frozenset()):
+    """Align; device SAM == host formatter's for every read no capacity flagged; the restatement holds on every record
+    (`sites`: the splice sites loaded into the handle).  Returns (header + host SAM, sorted flagged read names)."""
     res = idx.align(batch)
     errs = np.nonzero(res.reads["err"])[0]
     bad = sorted(set(batch.names[int(u) * (2 if paired else 1)].split(b"/")[0].decode() for u in errs))
@@ -313,7 +455,7 @@ def run_case(idx, batch, paired, opts):
     assert st["n_err_reads"] == len(errs)
     keep = lambda s: [l for l in s.splitlines() if l.split(b"\t")[0].decode() not in bad]
     assert keep(dev) == keep(host), "device SAM differs from the host formatter's"
-    check_records(b"\n".join(keep(host)), scoring_of(opts))
+    check_records(b"\n".join(keep(host)), scoring_of(opts), sites=sites)
     return idx.sam_header() + host, bad
 
 
@@ -323,9 +465,10 @@ def edge_batch(h2, d, case):
     return h2.ReadBatch.parse(path1=fs[0], path2=fs[1] if len(fs) == 2 else None, fastq=fmt == "-q", **front), len(fs) == 2
 
 
-# Graph-index cases run last (test_graph_index_cases_match_reference): opening a graph index raises the context's
-# per-thread stack limit for its recursive aligner, which takes ~11 GB of device memory for the rest of the process,
-# and the 8 x 4 workspace with its --bowtie2-dp scratch only fits an 80 GB card before that.
+# Graph-index cases run last (test_graph_index_cases_match_reference), after the linear edge, simulated and spliced
+# cases: opening a graph index raises the context's per-thread stack limit for its recursive aligner, which takes
+# ~11 GB of device memory for the rest of the process, and the 8 x 4 workspace with its --bowtie2-dp scratch only fits
+# an 80 GB card before that.
 EDGE_IDS = sorted(c for c in refsets.EDGE_CASES if refsets.EDGE_CASES[c][0] != "tiny_snp")
 
 
@@ -381,6 +524,61 @@ def check_sim_case(h2, sets, geometry, case):
         idx.close()
     assert bad == REF_SETS["flagged"].get(key, [])
     assert refsets.sam_md5(sam, bad) == REF_SETS["md5"][key]
+
+
+@pytest.fixture(scope="session")
+def spliced_dir(tmp_path_factory):
+    return refsets.generate_spliced(str(tmp_path_factory.mktemp("spliced")))
+
+
+SPLICED_IDS = sorted(c for c in refsets.SPLICED_CASES if refsets.SPLICED_CASES[c][0] != "tiny_snp")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", SPLICED_IDS)
+@pytest.mark.parametrize("geometry", list(GEOMETRIES))
+def test_spliced_corpus_matches_reference_under_every_geometry(h2, spliced_dir, geometry, case):
+    """Spliced mode (the reference's --no-temp-splicesite) on the spliced corpus (every motif, anchors of 1-30 bases
+    with and without an edit, intron lengths at every rule boundary, 2-4 junctions per read, sequence ends, the N gap,
+    pairs across junctions) and its simulated bulk, with and without a splice-site list and with --bowtie2-dp 2:
+    SAM equal to the reference's under each kernel geometry, the splice score and rules of check_records on every
+    record, and the --novel-splicesite-outfile equal to the reference's."""
+    check_spliced_case(h2, spliced_dir, geometry, case)
+
+
+def check_spliced_case(h2, d, geometry, case):
+    index, _, fmt, _, opts, _ = refsets.SPLICED_CASES[case]
+    fs, ss = refsets.spliced_files(d, case)
+    idx = open_geometry(h2, index, geometry, no_spliced_alignment=0, **opts)
+    try:
+        sites = frozenset()
+        if ss:
+            assert idx.load_splicesites(ss) > 200
+            sites = load_sites(ss)
+        batch = h2.ReadBatch.parse(path1=fs[0], path2=fs[1] if len(fs) == 2 else None, fastq=fmt == "-q")
+        sam, bad = run_case(idx, batch, len(fs) == 2, opts, sites)
+        novel = None
+        if case in refsets.SPLICED_NOVEL:
+            # the junctions of the printed alignments, collected by the SAM kernel over several batches
+            idx.collect_splicesites(True)
+            idx.run_reads(path1=fs[0], path2=fs[1] if len(fs) == 2 else None, fastq=fmt == "-q", batch_reads=4096, collect=False)
+            path = os.path.join(d, "novel_%s_%s.txt" % (case, geometry))
+            assert idx.write_novel_splicesites(path) > 100
+            novel = open(path, "rb").read()
+    finally:
+        idx.close()
+    key = "spliced/" + case
+    assert bad == REF_SETS["flagged"].get(key, [])
+    assert refsets.sam_md5(sam, bad) == REF_SETS["md5"][key]
+    assert sum(1 for l in sam_lines(sam) if not l.startswith(b"@") and b"N" in l.split(b"\t")[5]) > 250
+    if novel is not None:
+        import hashlib
+        assert hashlib.md5(novel).hexdigest() == REF_SETS["md5"]["spliced_novel/" + case]
+    if case == "edge_se":
+        got = [l.rstrip(b"\n") for l in refsets.spliced_golden_lines(sam)]
+        want = sam_lines(open(os.path.join(GOLDEN, "edge_spliced_se.sam"), "rb").read())
+        first = next((i for i, (a, b) in enumerate(zip(got, want)) if a != b), None)
+        assert first is None and len(got) == len(want), (got[first], want[first]) if first is not None else len(got)
 
 
 @pytest.mark.gpu
@@ -461,10 +659,14 @@ def test_dp_scratch_covers_every_grid_sharing_a_pool(h2, edge_dir, first, second
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", ["edge/" + c for c in sorted(refsets.EDGE_CASES) if refsets.EDGE_CASES[c][0] == "tiny_snp"] +
-                         [c[0] for c in SIM_CASES if c[1] == "tiny_snp"])
-def test_graph_index_cases_match_reference(h2, edge_dir, sets, case):
-    """The graph-index (tiny_snp) cases: graph indexes have one geometry, 8 x 4 (asserted by open_geometry)."""
+                         [c[0] for c in SIM_CASES if c[1] == "tiny_snp"] +
+                         ["spliced/" + c for c in sorted(refsets.SPLICED_CASES) if refsets.SPLICED_CASES[c][0] == "tiny_snp"])
+def test_graph_index_cases_match_reference(h2, edge_dir, sets, spliced_dir, case):
+    """The graph-index (tiny_snp) cases, spliced ones included: graph indexes have one geometry, 8 x 4 (asserted by
+    open_geometry)."""
     if case.startswith("edge/"):
         check_edge_case(h2, edge_dir, "8x4", case[5:])
+    elif case.startswith("spliced/"):
+        check_spliced_case(h2, spliced_dir, "8x4", case[8:])
     else:
         check_sim_case(h2, sets, "8x4", case)

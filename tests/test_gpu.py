@@ -325,15 +325,15 @@ def test_dynamic_programming_extension_matches_reference_binary_run_here(h2, set
 
 
 def test_spliced_alignment_when_compiled_in(h2, tmp_path):
-    """Spliced mode (== hisat2 --no-temp-splicesite: empty splice-site DB, reads independent).  The default
-    library refuses it (no CPU or approximate path); a library built with HT2_SPLICED=1 must reproduce the
+    """Spliced mode (== hisat2 --no-temp-splicesite: empty splice-site DB, reads independent), compiled into the
+    default library (a build with HT2_NO_SPLICED=1 refuses it loudly, with no CPU or approximate path): the
     committed golden SAM of the reference on the RNA-like fixture (340 spliced alignments) and the DNA
     fixtures, and, when oracle/_ref is on the box, the reference run in place on 20k chr22 pairs."""
     try:
         idx = h2.Index(os.path.join(GOLDEN, "tiny"), no_spliced_alignment=0)
     except h2.Ht2GpuError as e:
         assert "spliced" in str(e)
-        pytest.skip("library built without HT2_SPLICED=1: spliced mode is refused loudly")
+        pytest.skip("library built with HT2_NO_SPLICED=1: spliced mode is refused loudly")
     for args, gold, rd in ((("tiny_rna.fa",), "tiny_spliced_rna.sam", h2.ReadBatch.from_fasta), (("tiny_se.fa",), "tiny_spliced_se.sam", h2.ReadBatch.from_fasta),
                            (("tiny_pe_1.fq", "tiny_pe_2.fq"), "tiny_spliced_pe_fq.sam", h2.ReadBatch.from_fastq)):
         batch = rd(os.path.join(GOLDEN, args[0]), path2=os.path.join(GOLDEN, args[1]) if len(args) > 1 else None)

@@ -4,6 +4,8 @@ tiny.snp) by the seeded generators tools/simreads.py and tools/altreads.py, so t
 
   python tools/refsets.py        # writes tests/golden/ref_sets.json: md5 of the unmodified reference's SAM per case
   python tools/refsets.py --edge # only the edge/* cases (tools/edgereads.py); also writes tests/golden/edge_se.sam
+  python tools/refsets.py --spliced  # only the spliced/* and spliced_novel/* cases (tools/splicereads.py); also
+                                     # writes tests/golden/edge_spliced_se.sam (SPLICED_GOLDEN)
 
 The expected values come from oracle/_ref/hisat2-align-s (oracle/Makefile).  Cases whose reads can hit a fixed device
 capacity list the flagged reads (`flagged`, from a GPU run of the library); their md5 excludes those reads' records."""
@@ -76,6 +78,34 @@ def _edge_cases():
 EDGE_CASES = _edge_cases()
 EDGE_SEED = 11
 
+# spliced/<case>: the tools/splicereads.py corpus (splice_*) and its tools/sim_rna.py bulk (splice_sim*), aligned in
+# spliced mode as the reference's --no-temp-splicesite (splice sites are not carried from read to read, so every read
+# aligns on its own, as the library does).  case -> (index, files, format flag, reference flags, library options,
+# known-splice-site file or None).
+SPLICED_CASES = {
+    "edge_se": ("tiny", ["se.fa"], "-f", [], {}, None),
+    "edge_pe": ("tiny", ["pe_1.fa", "pe_2.fa"], "-f", [], {}, None),
+    "edge_fq": ("tiny", ["q.fq"], "-q", [], {}, None),
+    "sim_se": ("tiny", ["sim.fa"], "-f", [], {}, None),
+    "sim_pe": ("tiny", ["sim_1.fa", "sim_2.fa"], "-f", [], {}, None),
+    "ss_edge_se": ("tiny", ["se.fa"], "-f", [], {}, "ss.txt"),
+    "ss_sim_pe": ("tiny", ["sim_1.fa", "sim_2.fa"], "-f", [], {}, "sim_ss.txt"),
+    "edge_se_dp": ("tiny", ["se.fa"], "-f", ["--bowtie2-dp", "2"], dict(bowtie2_dp=2), None),
+    "graph_edge_se": ("tiny_snp", ["se.fa"], "-f", [], {}, None),
+    "graph_ss_sim_pe": ("tiny_snp", ["sim_1.fa", "sim_2.fa"], "-f", [], {}, "sim_ss.txt"),
+}
+# cases whose --novel-splicesite-outfile is recorded too, as spliced_novel/<case>
+SPLICED_NOVEL = ("sim_pe", "edge_se")
+SPLICE_SEED = 17
+# the reads of spliced/edge_se whose reference records are committed as tests/golden/edge_spliced_se.sam: the intron
+# lengths at the rule boundaries and the junctions of opposite sense (the md5 covers the rest of the corpus)
+SPLICED_GOLDEN = (b"len_", b"sense_")
+
+
+def spliced_golden_lines(sam):
+    """The SAM lines (headers without @PG, records of the SPLICED_GOLDEN reads) kept as edge_spliced_se.sam."""
+    return [l for l in sam.splitlines(True) if (l.startswith(b"@") and not l.startswith(b"@PG")) or l.startswith(SPLICED_GOLDEN)]
+
 
 def load_expected():
     return json.load(open(OUT))
@@ -106,6 +136,21 @@ def edge_files(d, case):
     return [os.path.join(d, "edge_" + f) for f in EDGE_CASES[case][1]]
 
 
+def generate_spliced(outdir):
+    """The tools/splicereads.py corpus under outdir (splice_*); returns outdir."""
+    sys.path.insert(0, TOOLS)
+    import splicereads
+    if not os.path.exists(os.path.join(outdir, "splice_se.fa")):
+        splicereads.generate(os.path.join(GOLDEN, "tiny.fa"), os.path.join(outdir, "splice"), SPLICE_SEED)
+    return outdir
+
+
+def spliced_files(d, case):
+    """(read files, known-splice-site file or None) of spliced/<case> under d."""
+    c = SPLICED_CASES[case]
+    return [os.path.join(d, "splice_" + f) for f in c[1]], (os.path.join(d, "splice_" + c[5]) if c[5] else None)
+
+
 def sam_md5(sam, exclude=()):
     """md5 of the SAM lines without @PG (and without the records of the read names in `exclude`)."""
     if isinstance(sam, str):
@@ -130,10 +175,17 @@ def reference(d, index, name, paired, flags=(), fa=False, fmt="-f"):
     return open(out, "rb").read()
 
 
-def main(edge_only=False):
+def main(edge_only=False, spliced_only=False):
     old = json.load(open(OUT)) if os.path.exists(OUT) else {}
     flagged = old.get("flagged", {})
     md5 = {}
+    if spliced_only:
+        md5 = {k: v for k, v in old.get("md5", {}).items() if not k.startswith(("spliced/", "spliced_novel/"))}
+        with tempfile.TemporaryDirectory() as d:
+            spliced_reference(d, md5, flagged)
+        json.dump({"md5": md5, "flagged": flagged}, open(OUT, "w"), indent=1, sort_keys=True)
+        open(OUT, "a").write("\n")
+        return
     if edge_only:
         md5 = {k: v for k, v in old.get("md5", {}).items() if not k.startswith("edge/")}
         with tempfile.TemporaryDirectory() as d:
@@ -167,8 +219,28 @@ def main(edge_only=False):
         d1[:k * bench.RECSZ].tofile(f1); d2[:k * bench.RECSZ].tofile(f2)
         md5["full/pe500k"] = sam_md5(reference(d, "tiny", None, True, fa=["-1", f1, "-2", f2]))
         edge_reference(d, md5, flagged)
+        spliced_reference(d, md5, flagged)
     json.dump({"md5": md5, "flagged": flagged}, open(OUT, "w"), indent=1, sort_keys=True)
     open(OUT, "a").write("\n")
+
+
+def spliced_reference(d, md5, flagged):
+    """spliced/<case> md5s (reference run with --no-temp-splicesite) and spliced_novel/<case>, the md5 of its
+    --novel-splicesite-outfile; the reference records of the SPLICED_GOLDEN reads of spliced/edge_se are also kept as
+    tests/golden/edge_spliced_se.sam."""
+    generate_spliced(d)
+    for case, (index, _, fmt, flags, _, _) in sorted(SPLICED_CASES.items()):
+        fs, ss = spliced_files(d, case)
+        key = "spliced/" + case
+        novel = os.path.join(d, "novel.txt")
+        extra = (["--known-splicesite-infile", ss] if ss else []) + (["--novel-splicesite-outfile", novel] if case in SPLICED_NOVEL else [])
+        sam = reference(d, index, None, len(fs) == 2, ["--no-temp-splicesite"] + flags + extra, fmt=fmt,
+                        fa=["-1", fs[0], "-2", fs[1]] if len(fs) == 2 else ["-U", fs[0]])
+        md5[key] = sam_md5(sam, flagged.get(key, ()))
+        if case in SPLICED_NOVEL:
+            md5["spliced_novel/" + case] = hashlib.md5(open(novel, "rb").read()).hexdigest()
+        if case == "edge_se":
+            open(os.path.join(GOLDEN, "edge_spliced_se.sam"), "wb").write(b"".join(spliced_golden_lines(sam)))
 
 
 def edge_reference(d, md5, flagged):
@@ -185,4 +257,4 @@ def edge_reference(d, md5, flagged):
 
 
 if __name__ == "__main__":
-    main(edge_only="--edge" in sys.argv[1:])
+    main(edge_only="--edge" in sys.argv[1:], spliced_only="--spliced" in sys.argv[1:])
