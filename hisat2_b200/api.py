@@ -78,6 +78,20 @@ class CParsedReads(C.Structure):
 SINK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
 
 
+class CSamOutput(C.Structure):
+    _fields_ = [("no_unal", C.c_int32), ("omit_sec_seq", C.c_int32), ("no_sq", C.c_int32), ("rg_id", C.c_char_p),
+                ("rg", C.POINTER(C.c_char_p)), ("n_rg", C.c_int32)]
+
+
+# ReportingMetrics of ht2gpu_align_counts_t, in its field order
+ALIGN_COUNTS = ("nread", "npaired", "nunpaired", "nconcord_0", "nconcord_uni1", "nconcord_uni2", "ndiscord",
+                "nunp_0_0", "nunp_0_uni1", "nunp_0_uni2", "nunp_0", "nunp_uni1", "nunp_uni2")
+
+
+class CAlignCounts(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ALIGN_COUNTS]
+
+
 EXPORTS = [
     "ht2gpu_default_options", "ht2gpu_open", "ht2gpu_open_image", "ht2gpu_open_device_image", "ht2gpu_build_image",
     "ht2gpu_free_image", "ht2gpu_image_data", "ht2gpu_image_bytes", "ht2gpu_device_image", "ht2gpu_align_batch",
@@ -87,7 +101,8 @@ EXPORTS = [
     "ht2gpu_sam_slots", "ht2gpu_submit_sam", "ht2gpu_wait_sam", "ht2gpu_align_sam", "ht2gpu_run_reads",
     "ht2gpu_host_alloc", "ht2gpu_host_free", "ht2gpu_set_error", "ht2gpu_parse_reads", "ht2gpu_free_parsed",
     "ht2gpu_ctx_get", "ht2gpu_ctx_set", "ht2gpu_run_reads_multi", "ht2gpu_open_peer", "ht2gpu_sw_selftest", "ht2gpu_load_splicesites", "ht2gpu_collect_splicesites",
-    "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry",
+    "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry", "ht2gpu_set_sam_output", "ht2gpu_align_counts",
+    "ht2gpu_format_align_summary",
 ]
 
 
@@ -157,6 +172,10 @@ def load_library(path=None):
     lib.ht2gpu_collect_splicesites.argtypes = [C.c_void_p, C.c_int]
     lib.ht2gpu_write_novel_splicesites.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.POINTER(C.c_uint64)]
     lib.ht2gpu_launch_geometry.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
+    lib.ht2gpu_set_sam_output.argtypes = [C.c_void_p, C.POINTER(CSamOutput)]
+    lib.ht2gpu_align_counts.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(CAlignCounts)]
+    lib.ht2gpu_format_align_summary.argtypes = [C.POINTER(CAlignCounts), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                                C.POINTER(C.c_size_t)]
     if path is None:
         _lib = lib
     return lib
@@ -169,6 +188,21 @@ def sw_selftest(n=2000, seed=1, device=0):
     if rc != 0:
         raise Ht2GpuError("ht2gpu_sw_selftest failed (%d)" % rc)
     return {"mismatches": int(out[0]), "problems": int(out[1]), "cells": int(out[2]), "valid": int(out[3])}
+
+
+def format_align_summary(counts, new_style=False, discordant=True, mixed=True):
+    """ht2gpu_format_align_summary: the alignment summary hisat2 prints at the end of a run (AlnSink::printAlSumm),
+    from a dict of ALIGN_COUNTS (Index.align_counts).  discordant / mixed = False under --no-discordant / --no-mixed.
+    Host only."""
+    lib = load_library()
+    c = CAlignCounts(*[int(counts.get(k, 0)) for k in ALIGN_COUNTS])
+    p, n = C.c_void_p(), C.c_size_t()
+    rc = lib.ht2gpu_format_align_summary(C.byref(c), int(bool(new_style)), int(bool(discordant)), int(bool(mixed)), C.byref(p), C.byref(n))
+    if rc != 0:
+        raise Ht2GpuError("ht2gpu_format_align_summary rc=%d" % rc)
+    s = C.string_at(p.value, n.value).decode()
+    lib.ht2gpu_free_text(p)
+    return s
 
 
 _ASC2DNA = np.zeros(256, dtype=np.uint8)
@@ -521,6 +555,24 @@ class Index(object):
         self._check(self._lib.ht2gpu_write_novel_splicesites(hs, 1 + len(peers), path.encode(), C.byref(n)), "ht2gpu_write_novel_splicesites")
         return int(n.value)
 
+    def set_sam_output(self, no_unal=False, omit_sec_seq=False, no_sq=False, rg_id=None, rg=()):
+        """ht2gpu_set_sam_output: --no-unal, --omit-sec-seq, --no-sq, --rg-id and the extra --rg fields of the @RG
+        line (printed only with an rg_id).  Applies to the batches that follow and to sam_header()."""
+        rg = [r.encode() if isinstance(r, str) else bytes(r) for r in rg]
+        arr = (C.c_char_p * max(1, len(rg)))(*rg)
+        cfg = CSamOutput(int(bool(no_unal)), int(bool(omit_sec_seq)), int(bool(no_sq)),
+                         (rg_id.encode() if isinstance(rg_id, str) else rg_id) if rg_id else None, arr, len(rg))
+        self._check(self._lib.ht2gpu_set_sam_output(self._h, C.byref(cfg)), "ht2gpu_set_sam_output")
+        self._sam_output = dict(no_unal=no_unal, omit_sec_seq=omit_sec_seq, no_sq=no_sq, rg_id=rg_id, rg=tuple(rg))
+
+    def align_counts(self, peers=(), reset=False):
+        """ht2gpu_align_counts: the per-read outcome counts (ReportingMetrics) of every batch formatted on the device
+        through this handle (+ peers) since open or the last reset, as a dict of ALIGN_COUNTS."""
+        hs = (C.c_void_p * (1 + len(peers)))(self._h, *[p._h for p in peers])
+        c = CAlignCounts()
+        self._check(self._lib.ht2gpu_align_counts(hs, 1 + len(peers), int(bool(reset)), C.byref(c)), "ht2gpu_align_counts")
+        return {k: int(getattr(c, k)) for k in ALIGN_COUNTS}
+
     def peer(self, device):
         """ht2gpu_open_peer: a replica of this index on another device of this process (device-to-device copy)."""
         o = Options()
@@ -539,6 +591,8 @@ class Index(object):
             raise Ht2GpuError("ht2gpu_open_peer rc=%d: %s" % (rc, msg))
         if getattr(self, "_ss", None):
             other.load_splicesites(*self._ss)
+        if getattr(self, "_sam_output", None):
+            other.set_sam_output(**self._sam_output)
         return other
 
     def run_reads(self, path1=None, path2=None, data1=None, data2=None, fastq=False, collect=True, peers=(), sink=None, **kw):

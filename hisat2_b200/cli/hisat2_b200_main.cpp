@@ -15,7 +15,9 @@ static void usage() {
                     "            [-I N] [-X N] [--no-mixed] [--no-discordant] [--seed N] [--batch N] [--device N] [--gpus N] [-p N]\n"
                     "            [-5 N] [-3 N] [-s N] [-u N] [--phred33|--phred64] [--no-temp-splicesite]\n"
                     "            [--known-splicesite-infile F] [--novel-splicesite-infile F] [--novel-splicesite-outfile F]\n"
-                    "            [--bowtie2-dp 0|1|2] [--score-min F,C,L] [--gbar N] [--sensitive] [--very-sensitive] [--fast]\n");
+                    "            [--bowtie2-dp 0|1|2] [--score-min F,C,L] [--gbar N] [--sensitive] [--very-sensitive] [--fast]\n"
+                    "            [--no-unal] [--omit-sec-seq] [--no-hd] [--no-sq] [--rg-id ID] [--rg TEXT]...\n"
+                    "            [--summary-file F] [--new-summary] [--quiet]\n");
 }
 static void two(const char* a, int32_t& x, int32_t& y) { sscanf(a, "%d,%d", &x, &y); }
 
@@ -28,6 +30,12 @@ int main(int argc, char** argv)
     int trim5 = 0, trim3 = 0, threads = 0, gpus = 1; bool phred64 = false; uint64_t skip = 0, upto = 0;
     bool sensitive = false, verySensitive = false, fast = false, noTempSpliceSite = false;
     const char *knownSs = NULL, *novelSs = NULL, *novelOut = NULL;   // --known-splicesite-infile / --novel-splicesite-infile (hisat2.cpp:1689-1691)
+    // SAM output (hisat2.cpp:601-623, 1342-1343, 1389-1407): --no-hd prints no header at all (no @PG either,
+    // hisat2.cpp:4127-4131); --rg ID:<x> sets the read-group id like --rg-id <x>, any other --rg text is an @RG field
+    bool noHd = false, newSummary = false, quiet = false;
+    int32_t noUnal = 0, omitSecSeq = 0, noSq = 0;
+    std::string rgId; std::vector<std::string> rgFields;
+    const char* summaryFile = NULL;
     bool mpGiven = false;   // "--mp a,b" becomes MMP=Q,a,b, which switches the cost model back to quality-aware even
                             // under --ignore-quals (aligner_seed_policy.cpp:396-418)
     for (int i = 1; i < argc; i++) {
@@ -64,7 +72,18 @@ int main(int argc, char** argv)
         else if (a == "-5" || a == "--trim5") trim5 = atoi(next()); else if (a == "-3" || a == "--trim3") trim3 = atoi(next());
         else if (a == "-s" || a == "--skip") skip = (uint64_t)atoll(next()); else if (a == "-u" || a == "--upto" || a == "--qupto") upto = (uint64_t)atoll(next());
         else if (a == "--phred64" || a == "--phred64-quals" || a == "--solexa1.3-quals") phred64 = true; else if (a == "--phred33" || a == "--phred33-quals") phred64 = false;
-        else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--fr" || a == "--quiet" || a == "--no-unal-ignored") {}
+        else if (a == "--no-unal") noUnal = 1;
+        else if (a == "--omit-sec-seq" || a == "--sam-omit-sec-seq") omitSecSeq = 1;
+        else if (a == "--no-hd" || a == "--no-head" || a == "--no-HD" || a == "--sam-no-hd" || a == "--sam-no-head" || a == "--sam-nohead" || a == "--sam-noHD") noHd = true;
+        else if (a == "--no-sq" || a == "--no-SQ" || a == "--sam-no-sq" || a == "--sam-nosq" || a == "--sam-noSQ") noSq = 1;
+        else if (a == "--rg-id" || a == "--sam-rg-id") rgId = next();
+        else if (a == "--rg" || a == "--RG" || a == "--sam-rg" || a == "--sam-RG") {
+            std::string v = next();
+            if (v.compare(0, 3, "ID:") == 0) rgId = v.substr(3); else rgFields.push_back(v);
+        }
+        else if (a == "--summary-file") summaryFile = next(); else if (a == "--new-summary") newSummary = true;
+        else if (a == "--quiet") quiet = true;   // no alignment summary (hisat2.cpp:4165)
+        else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--fr" || a == "--no-unal-ignored") {}
         else if (a == "-h" || a == "--help") { usage(); return 0; }
         else { fprintf(stderr, "Error: option %s is not supported by hisat2-b200\n", a.c_str()); return 1; }
     }
@@ -90,8 +109,16 @@ int main(int argc, char** argv)
     const bool paired = m1 != NULL;
     FILE* fo = out ? fopen(out, "wb") : stdout;
     if (!fo) { fprintf(stderr, "Error: cannot write %s\n", out); return 1; }
-    { char* hd; size_t hl; ht2gpu_sam_header(h, &hd, &hl); fwrite(hd, 1, hl, fo); ht2gpu_free_text(hd);
-      fprintf(fo, "@PG\tID:hisat2\tPN:hisat2-b200\tVN:0.2\n"); }
+    std::vector<const char*> rgPtrs;
+    for (const std::string& f : rgFields) rgPtrs.push_back(f.c_str());
+    ht2gpu_sam_output_t so; memset(&so, 0, sizeof(so));
+    so.no_unal = noUnal; so.omit_sec_seq = omitSecSeq; so.no_sq = noSq;
+    so.rg_id = rgId.empty() ? NULL : rgId.c_str(); so.rg = rgPtrs.data(); so.n_rg = (int32_t)rgPtrs.size();
+    if (ht2gpu_set_sam_output(h, &so) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
+    if (!noHd) {
+        char* hd; size_t hl; ht2gpu_sam_header(h, &hd, &hl); fwrite(hd, 1, hl, fo); ht2gpu_free_text(hd);
+        fprintf(fo, "@PG\tID:hisat2\tPN:hisat2-b200\tVN:0.2\n");
+    }
     ht2gpu_reads_input_t in; memset(&in, 0, sizeof(in));
     in.path1 = paired ? m1 : u; in.path2 = paired ? m2 : NULL;
     in.format = fastq ? 1 : 0; in.trim5 = trim5; in.trim3 = trim3; in.phred64 = phred64 ? 1 : 0; in.seed = gseed;
@@ -104,6 +131,7 @@ int main(int argc, char** argv)
         ht2gpu_handle_t* hg = NULL;
         if (ht2gpu_open_peer(h, &og, &hg) != HT2GPU_OK) { fprintf(stderr, "Error: device %d: %s\n", og.device, ht2gpu_last_error(hg)); return 1; }
         hs.push_back(hg);
+        if (ht2gpu_set_sam_output(hg, &so) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(hg)); return 1; }
     }
     if (knownSs || novelSs) {
         uint32_t ns = 0;
@@ -118,10 +146,24 @@ int main(int argc, char** argv)
         uint64_t nw = 0;
         if (ht2gpu_write_novel_splicesites(hs.data(), (int)hs.size(), novelOut, &nw) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
     }
-    for (size_t g = 1; g < hs.size(); g++) ht2gpu_close(hs[g]);
     if (st.n_err_reads)
         fprintf(stderr, "Warning: %llu read(s) exceeded a device-side capacity; their records may differ from hisat2's\n", (unsigned long long)st.n_err_reads);
     if (fo != stdout) fclose(fo);
+    if (!quiet) {   // the alignment summary over every device (AlnSink::finish, hisat2.cpp:4165-4185)
+        ht2gpu_align_counts_t c;
+        char* txt = NULL; size_t tl = 0;
+        if (ht2gpu_align_counts(hs.data(), (int)hs.size(), 0, &c) != HT2GPU_OK ||
+            ht2gpu_format_align_summary(&c, newSummary ? 1 : 0, o.no_discordant ? 0 : 1, o.no_mixed ? 0 : 1, &txt, &tl) != HT2GPU_OK) {
+            fprintf(stderr, "Error: cannot format the alignment summary\n"); return 1;
+        }
+        fwrite(txt, 1, tl, stderr);
+        if (summaryFile) {
+            FILE* fs = fopen(summaryFile, "wb");
+            if (fs) { fwrite(txt, 1, tl, fs); fclose(fs); }
+        }
+        ht2gpu_free_text(txt);
+    }
+    for (size_t g = 1; g < hs.size(); g++) ht2gpu_close(hs[g]);
     ht2gpu_close(h);
     return 0;
 }

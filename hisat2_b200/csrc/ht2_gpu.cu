@@ -531,21 +531,37 @@ ht2_seed_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatch b, u
 template <bool WRITE>
 __global__ void __launch_bounds__(HT2_SAM_TPB)
 ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigned long long* __restrict__ blk, char* __restrict__ out,
-               unsigned long long cap, unsigned int* counters)
+               unsigned long long cap, unsigned int* counters, unsigned long long* __restrict__ tally)
 {
     __shared__ unsigned long long sWarp[HT2_SAM_TPB / 32];
+    __shared__ uint32_t sTally[HT2_SAM_TPB / 32][HT2_T_N];
     const uint32_t u = blockIdx.x * HT2_SAM_TPB + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     Ht2SamFmt F;
     F.bind(&in);
     unsigned long long mine = 0;
     if (!WRITE) {
+        Ht2SamTally t;
+#pragma unroll
+        for (int k = 0; k < HT2_T_N; k++) t.c[k] = 0;
         if (u < units) {
             Ht2SamOut<false> o; o.p = NULL; o.n = 0;
-            F.unit(o, u);
+            F.unit(o, u, &t);
             mine = o.n;
             lens[u] = (uint32_t)o.n;
             if (in.reads[u].err) atomicAdd(&counters[4], 1u);
+        }
+        // ReportingMetrics of the block: warp sums, then one 64-bit atomic per counter per block
+#pragma unroll
+        for (int k = 0; k < HT2_T_N; k++) {
+            const uint32_t s = __reduce_add_sync(0xffffffffu, t.c[k]);
+            if (lane == 0) sTally[wib][k] = s;
+        }
+        __syncthreads();
+        if (threadIdx.x < HT2_T_N) {
+            unsigned long long s = 0;
+            for (int w = 0; w < HT2_SAM_TPB / 32; w++) s += sTally[w][threadIdx.x];
+            if (s) atomicAdd(&tally[threadIdx.x], s);
         }
     } else mine = u < units ? lens[u] : 0;
     // inclusive warp scan, then across the block's warps
@@ -591,6 +607,7 @@ ht2_sam_scan_kernel(unsigned long long* blk, uint32_t nBlk)
 // the D2H copy of batch i-1 overlap the kernels of batch i.  The alignment workspaces (dWork) are shared by all
 // slots: kernels of different slots are chained through the device's WorkPool.
 #define HT2GPU_N_SLOTS 3
+#define HT2_META_TALLY 16
 // device memory a handle leaves free beside its workspace pool: slot buffers of 4 M-read batches, the per-thread
 // stack of the pool kernel, and headroom for other work on the device
 #define HT2_MEM_RESERVE ((size_t)10 << 30)
@@ -606,8 +623,10 @@ struct SamSlot {
     unsigned long long* dBlk; size_t capBlk;      // per-block sums, then exclusive block offsets; [nBlk] = total
     char* dSam; size_t capSam;
     Ht2SsRec* dColRecs; size_t capCol;            // --novel-splicesite-outfile: junction records of the batch (count in dCounters[6])
+    unsigned long long* dTally;                   // ReportingMetrics of the batch (HT2_T_N counters, ht2_sam.h), zeroed per SAM pass
     char* hSam; size_t capHSam;                   // pinned
-    unsigned long long* hMeta;                    // pinned: [0] total SAM bytes, [1..4] result counters, [5] reads with errors
+    unsigned long long* hMeta;                    // pinned: [0] total SAM bytes, [1..4] result counters, [5] reads with errors,
+                                                  //         [HT2_META_TALLY ..] the batch's ReportingMetrics
     // the submitted batch (for a re-run after a pool overflow)
     ht2gpu_read_batch_t batch; uint32_t units; size_t namesBytes; uint64_t h2dBytes; uint32_t nLaunch;
     bool pending;
@@ -653,6 +672,10 @@ struct ht2gpu_handle {
     Ht2NovelSites  novel;     // ... aggregated here (ht2gpu_wait_sam), written by ht2gpu_write_novel_splicesites
     std::mutex     novelMu;
     std::vector<uint8_t> ssBlob;   // ... and its host copy (host formatter)
+    Ht2SamOutput   samOut;    // SAM output settings (ht2gpu_set_sam_output)
+    char*          dRgTag;    // ... its "RG:Z:<id>" on the device, or NULL
+    ht2gpu_align_counts_t counts;   // ReportingMetrics of every batch ht2gpu_wait_sam returned (ht2gpu_align_counts)
+    std::mutex     countMu;
     size_t         nWork;
     cudaStream_t   stream;
     cudaEvent_t    ev[4];
@@ -970,6 +993,7 @@ extern "C" int ht2gpu_close(ht2gpu_handle_t* h)
     if (h->dMinsc) cudaFree(h->dMinsc);
     if (h->dSplT) cudaFree(h->dSplT);
     if (h->dSsT) cudaFree(h->dSsT);
+    if (h->dRgTag) cudaFree(h->dRgTag);
     cudaFree(h->dStats);
     for (int k = 0; k < HT2GPU_N_SLOTS; k++) {
         SamSlot& S = h->slots[k];
@@ -977,7 +1001,7 @@ extern "C" int ht2gpu_close(ht2gpu_handle_t* h)
         cudaStreamSynchronize(S.stream);
         cudaFree(S.dSeq); cudaFree(S.dQual); cudaFree(S.dOffs); cudaFree(S.dSeeds); cudaFree(S.dNames); cudaFree(S.dNameOffs);
         cudaFree(S.dReads); cudaFree(S.dAlns); cudaFree(S.dEdits); cudaFree(S.dPairs); cudaFree(S.dCounters);
-        cudaFree(S.dSamLen); cudaFree(S.dBlk); cudaFree(S.dSam); cudaFree(S.dColRecs);
+        cudaFree(S.dSamLen); cudaFree(S.dBlk); cudaFree(S.dSam); cudaFree(S.dColRecs); cudaFree(S.dTally);
         if (S.hSam) cudaFreeHost(S.hSam);
         if (S.hMeta) cudaFreeHost(S.hMeta);
         cudaStreamDestroy(S.stream);
@@ -1016,7 +1040,8 @@ static int slotInit(ht2gpu_handle* h, SamSlot& S)
     CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
     for (int i = 0; i < 6; i++) CK(cudaEventCreate(&S.ev[i]));
     CK(cudaMalloc(&S.dCounters, 8 * sizeof(unsigned int)));
-    CK(cudaHostAlloc(&S.hMeta, 16 * sizeof(unsigned long long), cudaHostAllocPortable));
+    CK(cudaMalloc(&S.dTally, HT2_T_N * sizeof(unsigned long long)));
+    CK(cudaHostAlloc(&S.hMeta, (HT2_META_TALLY + HT2_T_N) * sizeof(unsigned long long), cudaHostAllocPortable));
     S.init = true;
     return HT2GPU_OK;
 }
@@ -1257,6 +1282,7 @@ static Ht2SamIn samIn(const ht2gpu_handle* h, const SamSlot& S)
     in.reads = S.dReads; in.alns = S.dAlns; in.edits = S.dEdits; in.pairs = S.dPairs;
     in.khits = h->P.khits; in.secondary = h->P.secondary; in.mixed = h->P.mixed; in.discord = h->P.discord; in.ssT = h->dSsT;
     in.colCount = h->collectSs ? S.dCounters + 6 : NULL; in.colRecs = S.dColRecs; in.colCap = (uint32_t)S.capCol;
+    in.noUnal = h->samOut.noUnal; in.omitSecSeq = h->samOut.omitSecSeq; in.rgTag = h->dRgTag;
     return in;
 }
 
@@ -1275,10 +1301,12 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
     else CK(cudaEventRecord(S.ev[2], S.stream));
     CK(cudaEventRecord(S.ev[3], S.stream));
     if (h->collectSs) CK(cudaMemsetAsync(S.dCounters + 6, 0, sizeof(unsigned int), S.stream));
+    // the counting pass tallies the batch's ReportingMetrics; a re-run (ht2gpu_wait_sam) must not count it twice
+    CK(cudaMemsetAsync(S.dTally, 0, HT2_T_N * sizeof(unsigned long long), S.stream));
     const Ht2SamIn in = samIn(h, S);
-    ht2_sam_kernel<false><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, NULL, 0, S.dCounters);
+    ht2_sam_kernel<false><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, NULL, 0, S.dCounters, S.dTally);
     ht2_sam_scan_kernel<<<1, 1024, 0, S.stream>>>(S.dBlk, nBlk);
-    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.capSam, S.dCounters);
+    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.capSam, S.dCounters, S.dTally);
     CK(cudaGetLastError());
     S.nLaunch += 3;
     CK(cudaEventRecord(S.ev[4], S.stream));
@@ -1286,6 +1314,7 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
     // meta: total SAM bytes, result counters, reads with errors
     CK(cudaMemcpyAsync(&S.hMeta[0], S.dBlk + nBlk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
     CK(cudaMemcpyAsync(&S.hMeta[1], S.dCounters, 8 * sizeof(unsigned int), cudaMemcpyDeviceToHost, S.stream));
+    CK(cudaMemcpyAsync(&S.hMeta[HT2_META_TALLY], S.dTally, HT2_T_N * sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
     return HT2GPU_OK;
 }
 
@@ -1317,7 +1346,9 @@ extern "C" int ht2gpu_submit_sam(ht2gpu_handle_t* h, int slot, const ht2gpu_read
     rc = ensureOut(h, S, S.units, (size_t)b->n_reads * 2 + 1024, (size_t)b->n_reads * 4 + 4096, (size_t)S.units * 2 + 1024);
     if (rc) return rc;
     // SAM text: ~2.2 bytes per base + ~170 per record at one record per read; grown from the measured size if short
-    const size_t est = (size_t)((double)b->offs[b->n_reads] * 2.6) + (size_t)b->n_reads * 260 + names_bytes + 4096;
+    // (+ "\tRG:Z:<id>" per record with a read group)
+    const size_t rgBytes = h->samOut.rgId.empty() ? 0 : h->samOut.rgTag().size() + 1;
+    const size_t est = (size_t)((double)b->offs[b->n_reads] * 2.6) + (size_t)b->n_reads * (260 + rgBytes) + names_bytes + 4096;
     if (est > S.capSam) CK(growBuf(S.dSam, S.capSam, est, 1, 1));
     return enqueueKernels(h, S, true);
 }
@@ -1364,6 +1395,11 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
         if (nrec) CK(cudaMemcpy(recs.data(), S.dColRecs, (size_t)nrec * sizeof(Ht2SsRec), cudaMemcpyDeviceToHost));
         std::lock_guard<std::mutex> lk(h->novelMu);
         h->novel.add(recs.data(), recs.size());
+    }
+    {
+        std::lock_guard<std::mutex> lk(h->countMu);
+        uint64_t* tot = (uint64_t*)&h->counts;
+        for (int k = 0; k < HT2_T_N; k++) tot[k] += S.hMeta[HT2_META_TALLY + k];
     }
     if (h->dStats) dumpStats(h);
     const unsigned int* c = (const unsigned int*)&S.hMeta[1];
@@ -1596,8 +1632,9 @@ extern "C" void ht2gpu_free_seed_results(ht2gpu_seed_result_t* res)
 // ---------------------------------------------------------------------------
 extern "C" int ht2gpu_sam_header(ht2gpu_handle_t* h, char** out, size_t* out_len)
 {
+    if (!h || !out) return HT2GPU_ERR_ARG;
     std::string s;
-    ht2_sam_header(s, *h->img);
+    ht2_sam_header(s, *h->img, &h->samOut);
     char* p = (char*)malloc(s.size() + 1);
     memcpy(p, s.data(), s.size()); p[s.size()] = 0;
     *out = p; if (out_len) *out_len = s.size();
@@ -1663,5 +1700,47 @@ extern "C" int ht2gpu_format_sam(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* 
     if (!h || !b || !res || !names || !out) return HT2GPU_ERR_ARG;
     unsigned nth = std::thread::hardware_concurrency();
     if (const char* e = getenv("HT2GPU_THREADS")) nth = (unsigned)atoi(e);
-    return ht2_format_batch(*h->img, h->P, b, names, res, out, out_len, nth, h->ssBlob.empty() ? NULL : h->ssBlob.data()) ? HT2GPU_OK : HT2GPU_ERR_ARG;
+    return ht2_format_batch(*h->img, h->P, b, names, res, out, out_len, nth, h->ssBlob.empty() ? NULL : h->ssBlob.data(),
+                            NULL, NULL, 0, &h->samOut) ? HT2GPU_OK : HT2GPU_ERR_ARG;
+}
+
+// SAM output settings (--no-unal, --omit-sec-seq, --no-sq, --rg-id / --rg).  The read group's "RG:Z:<id>" is uploaded
+// once here; the SAM kernels print it from device memory.
+extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output_t* cfg)
+{
+    if (!h || !cfg || cfg->n_rg < 0 || (cfg->n_rg > 0 && !cfg->rg)) return HT2GPU_ERR_ARG;
+    for (int k = 0; k < HT2GPU_N_SLOTS; k++)
+        if (h->slots[k].pending) { h->err = "ht2gpu_set_sam_output: a batch is in flight (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
+    Ht2SamOutput so;
+    so.noUnal = cfg->no_unal != 0; so.omitSecSeq = cfg->omit_sec_seq != 0; so.noSq = cfg->no_sq != 0;
+    if (cfg->rg_id) so.rgId = cfg->rg_id;
+    for (int i = 0; i < cfg->n_rg; i++) { if (!cfg->rg[i]) return HT2GPU_ERR_ARG; so.rg.push_back(cfg->rg[i]); }
+    CK(cudaSetDevice(h->device));
+    for (int k = 0; k < HT2GPU_N_SLOTS; k++) if (h->slots[k].init) CK(cudaStreamSynchronize(h->slots[k].stream));
+    if (h->dRgTag) { CK(cudaFree(h->dRgTag)); h->dRgTag = NULL; }
+    const std::string tag = so.rgTag();
+    if (!tag.empty()) {
+        CK(cudaMalloc(&h->dRgTag, tag.size() + 1));
+        CK(cudaMemcpy(h->dRgTag, tag.c_str(), tag.size() + 1, cudaMemcpyHostToDevice));
+    }
+    h->samOut = so;
+    return HT2GPU_OK;
+}
+
+// The output settings of two handles are the same (ht2gpu_run_reads_multi: one run prints one kind of record)
+bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b) { return a->samOut == b->samOut; }
+
+extern "C" int ht2gpu_align_counts(ht2gpu_handle_t** hs, int n, int reset, ht2gpu_align_counts_t* out)
+{
+    if (!hs || n < 1 || !out) return HT2GPU_ERR_ARG;
+    for (int i = 0; i < n; i++) if (!hs[i]) return HT2GPU_ERR_ARG;
+    memset(out, 0, sizeof(*out));
+    uint64_t* o = (uint64_t*)out;
+    for (int i = 0; i < n; i++) {
+        std::lock_guard<std::mutex> lk(hs[i]->countMu);
+        const uint64_t* c = (const uint64_t*)&hs[i]->counts;
+        for (int k = 0; k < HT2_T_N; k++) o[k] += c[k];
+        if (reset) memset(&hs[i]->counts, 0, sizeof(hs[i]->counts));
+    }
+    return HT2GPU_OK;
 }

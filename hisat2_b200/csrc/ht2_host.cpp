@@ -261,11 +261,12 @@ bool ht2_read_reads(const char* path, std::vector<Ht2HostRead>& out, int mate, s
 // ---------------------------------------------------------------------------
 // SAM back end
 // ---------------------------------------------------------------------------
-void ht2_sam_header(std::string& o, const Ht2Image& img)
+// SamConfig::printHeader (sam.h:446-463) without @PG: @HD, @SQ unless --no-sq, @RG when a read-group id is set
+void ht2_sam_header(std::string& o, const Ht2Image& img, const Ht2SamOutput* so)
 {
     o += "@HD\tVN:1.0\tSO:unsorted\n";
     const Ht2ImageHeader* H = img.header();
-    for (uint32_t i = 0; i < H->nRefs; i++) {
+    for (uint32_t i = 0; !(so && so->noSq) && i < H->nRefs; i++) {
         o += "@SQ\tSN:";
         const char* nm = img.refName(i);
         for (const char* c = nm; *c && !isspace((unsigned char)*c); c++) o.push_back(*c);
@@ -273,14 +274,104 @@ void ht2_sam_header(std::string& o, const Ht2Image& img)
         appendInt(o, img.refPlen(i));
         o += "\n";
     }
+    if (so && !so->rgId.empty()) {
+        o += "@RG\tID:";
+        o += so->rgId;
+        for (const std::string& f : so->rg) { o += "\t"; o += f; }
+        o += "\n";
+    }
+}
+
+// printPct (aln_sink.h:1613-1622): fixed, two decimals, 0.00% for a zero denominator
+static void appendPct(std::string& o, uint64_t num, uint64_t denom)
+{
+    double pct = 0.0f;
+    if (denom != 0) pct = 100.0 * (double)num / (double)denom;
+    char buf[64];
+    snprintf(buf, sizeof(buf), "%.2f%%", pct);
+    o += buf;
+}
+
+void ht2_format_align_summary(std::string& o, const ht2gpu_align_counts_t& m, bool newStyle, bool discord, bool mixed)
+{
+    auto num = [&](uint64_t v) { appendInt(o, (int64_t)v); };
+    // "<n> (<pct>)" as most lines of the summary print it
+    auto np = [&](uint64_t v, uint64_t denom) { num(v); o += " ("; appendPct(o, v, denom); o += ")"; };
+    const uint64_t totread = m.nread, totpair = m.npaired, totunpair = m.nunpaired;
+    const uint64_t tot_al_cand = totunpair + totpair * 2;
+    const uint64_t tot_al = (m.nconcord_uni1 + m.nconcord_uni2) * 2 + m.ndiscord * 2 + m.nunp_0_uni1 + m.nunp_0_uni2 + m.nunp_uni1 + m.nunp_uni2;
+    const uint64_t ncondiscord_0 = m.nconcord_0 - m.ndiscord;
+    if (newStyle) {
+        o += "HISAT2 summary stats:\n";
+        if (totpair > 0) {
+            o += "\tTotal pairs: "; num(totpair); o += "\n";
+            o += "\t\tAligned concordantly or discordantly 0 time: "; np(ncondiscord_0, m.npaired); o += "\n";
+            o += "\t\tAligned concordantly 1 time: "; np(m.nconcord_uni1, m.npaired); o += "\n";
+            o += "\t\tAligned concordantly >1 times: "; np(m.nconcord_uni2, m.npaired); o += "\n";
+            o += "\t\tAligned discordantly 1 time: "; np(m.ndiscord, m.npaired); o += "\n";
+            o += "\tTotal unpaired reads: "; num(ncondiscord_0 * 2); o += "\n";
+            o += "\t\tAligned 0 time: "; np(m.nunp_0_0, ncondiscord_0 * 2); o += "\n";
+            o += "\t\tAligned 1 time: "; np(m.nunp_0_uni1, ncondiscord_0 * 2); o += "\n";
+            o += "\t\tAligned >1 times: "; np(m.nunp_0_uni2, ncondiscord_0 * 2); o += "\n";
+        } else {
+            o += "\tTotal reads: "; num(totread); o += "\n";
+            o += "\t\tAligned 0 time: "; np(m.nunp_0, m.nunpaired); o += "\n";
+            o += "\t\tAligned 1 time: "; np(m.nunp_uni1, m.nunpaired); o += "\n";
+            o += "\t\tAligned >1 times: "; np(m.nunp_uni2, m.nunpaired); o += "\n";
+        }
+        o += "\tOverall alignment rate: "; appendPct(o, tot_al, tot_al_cand); o += "\n";
+        return;
+    }
+    num(totread); o += totread > 0 ? " reads; of these:\n" : " reads\n";
+    if (totpair > 0) {
+        o += "  "; np(totpair, totread); o += " were paired; of these:\n";
+        o += "    "; np(m.nconcord_0, m.npaired); o += " aligned concordantly 0 times\n";
+        o += "    "; np(m.nconcord_uni1, m.npaired); o += " aligned concordantly exactly 1 time\n";
+        o += "    "; np(m.nconcord_uni2, m.npaired); o += " aligned concordantly >1 times\n";
+        if (discord) {
+            o += "    ----\n";
+            o += "    "; num(m.nconcord_0); o += " pairs aligned concordantly 0 times; of these:\n";
+            o += "      "; np(m.ndiscord, m.nconcord_0); o += " aligned discordantly 1 time\n";
+        }
+        if (mixed) {
+            o += "    ----\n";
+            o += "    "; num(ncondiscord_0); o += " pairs aligned 0 times concordantly or discordantly; of these:\n";
+            o += "      "; num(ncondiscord_0 * 2); o += " mates make up the pairs; of these:\n";
+            o += "        "; np(m.nunp_0_0, ncondiscord_0 * 2); o += " aligned 0 times\n";
+            o += "        "; np(m.nunp_0_uni1, ncondiscord_0 * 2); o += " aligned exactly 1 time\n";
+            o += "        "; np(m.nunp_0_uni2, ncondiscord_0 * 2); o += " aligned >1 times\n";
+        }
+    }
+    if (totunpair > 0) {
+        o += "  "; np(totunpair, totread); o += " were unpaired; of these:\n";
+        o += "    "; np(m.nunp_0, m.nunpaired); o += " aligned 0 times\n";
+        o += "    "; np(m.nunp_uni1, m.nunpaired); o += " aligned exactly 1 time\n";
+        o += "    "; np(m.nunp_uni2, m.nunpaired); o += " aligned >1 times\n";
+    }
+    appendPct(o, tot_al, tot_al_cand); o += " overall alignment rate\n";
+}
+
+extern "C" int ht2gpu_format_align_summary(const ht2gpu_align_counts_t* c, int new_style, int discordant, int mixed,
+                                           char** out, size_t* out_len)
+{
+    if (!c || !out) return HT2GPU_ERR_ARG;
+    std::string s;
+    ht2_format_align_summary(s, *c, new_style != 0, discordant != 0, mixed != 0);
+    char* p = (char*)malloc(s.size() + 1);
+    if (!p) return HT2GPU_ERR_ARG;
+    memcpy(p, s.data(), s.size()); p[s.size()] = 0;
+    *out = p; if (out_len) *out_len = s.size();
+    return HT2GPU_OK;
 }
 
 // The SAM back end of one batch (ht2gpu_format_sam) on the host: the formatter of ht2_sam.h -- the same
 // source the device kernel runs -- on host threads over contiguous unit ranges: a counting pass, a prefix
 // over the ranges, a writing pass straight into the output (records in read order = --reorder).
 bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read_batch_t* b, const char* names,
-                      const ht2gpu_result_batch_t* res, char** out, size_t* out_len, unsigned nth, const uint8_t* ssT, uint32_t* colCount, Ht2SsRec* colRecs, uint32_t colCap)
+                      const ht2gpu_result_batch_t* res, char** out, size_t* out_len, unsigned nth, const uint8_t* ssT, uint32_t* colCount, Ht2SsRec* colRecs, uint32_t colCap,
+                      const Ht2SamOutput* so, ht2gpu_align_counts_t* counts)
 {
+    const std::string rgTag = so ? so->rgTag() : std::string();
     const uint32_t units = b->paired ? b->n_reads / 2 : b->n_reads;
     std::vector<uint32_t> nameOffs((size_t)b->n_reads + 1);
     {
@@ -294,10 +385,12 @@ bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read
     in.n_reads = b->n_reads; in.paired = b->paired;
     in.reads = res->reads; in.alns = res->alns; in.edits = res->edits; in.pairs = res->pairs;
     in.khits = P.khits; in.secondary = P.secondary; in.mixed = P.mixed; in.discord = P.discord; in.ssT = ssT; in.colCount = colCount; in.colRecs = colRecs; in.colCap = colCap;
+    in.noUnal = so && so->noUnal; in.omitSecSeq = so && so->omitSecSeq; in.rgTag = rgTag.empty() ? NULL : rgTag.c_str();
     Ht2SamFmt F; F.bind(&in);
     if (nth > 64) nth = 64;
     if (nth < 1 || units < 4096) nth = 1;
     std::vector<uint64_t> bytes(nth, 0), at(nth + 1, 0);
+    std::vector<Ht2SamTally> tally(nth);
     auto range = [&](unsigned t, uint32_t& u0, uint32_t& u1) { u0 = (uint32_t)((uint64_t)units * t / nth); u1 = (uint32_t)((uint64_t)units * (t + 1) / nth); };
     auto forThreads = [&](const std::function<void(unsigned)>& fn) {
         if (nth == 1) { fn(0); return; }
@@ -308,10 +401,15 @@ bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read
     forThreads([&](unsigned t) {
         uint32_t u0, u1; range(t, u0, u1);
         Ht2SamOut<false> o; o.p = NULL; o.n = 0;
-        for (uint32_t u = u0; u < u1; u++) F.unit(o, u);
+        memset(&tally[t], 0, sizeof(Ht2SamTally));
+        for (uint32_t u = u0; u < u1; u++) F.unit(o, u, &tally[t]);
         bytes[t] = o.n;
     });
     for (unsigned t = 0; t < nth; t++) at[t + 1] = at[t] + bytes[t];
+    if (counts) {
+        uint64_t* c = (uint64_t*)counts;   // ht2gpu_align_counts_t: HT2_T_N uint64_t in the order of the tally
+        for (unsigned t = 0; t < nth; t++) for (int k = 0; k < HT2_T_N; k++) c[k] += tally[t].c[k];
+    }
     const size_t total = (size_t)at[nth];
     char* p = (char*)malloc(total + 1);
     if (!p) return false;

@@ -44,11 +44,26 @@ bool ht2_read_fasta(const char* path, std::vector<Ht2HostRead>& out, int mate, s
 bool ht2_read_fastq(const char* path, std::vector<Ht2HostRead>& out, int mate, std::string& err);
 bool ht2_read_reads(const char* path, std::vector<Ht2HostRead>& out, int mate, std::string& err);  // by first character
 
+// SAM output settings of a handle (ht2gpu_set_sam_output): --no-unal, --omit-sec-seq, --no-sq, --rg-id, --rg
+struct Ht2SamOutput {
+    bool noUnal = false, omitSecSeq = false, noSq = false;
+    std::string rgId;                 // empty = no read group
+    std::vector<std::string> rg;      // extra @RG fields, in the given order
+    std::string rgTag() const { return rgId.empty() ? std::string() : "RG:Z:" + rgId; }
+    bool operator==(const Ht2SamOutput& o) const {
+        return noUnal == o.noUnal && omitSecSeq == o.omitSecSeq && noSq == o.noSq && rgId == o.rgId && rg == o.rg;
+    }
+};
+
 // SAM
-void ht2_sam_header(std::string& o, const Ht2Image& img);
-// ht2gpu_format_sam's body: host-only, shared with the test build
+void ht2_sam_header(std::string& o, const Ht2Image& img, const Ht2SamOutput* so = NULL);
+// ht2gpu_format_sam's body: host-only, shared with the test build.  counts != NULL: the units' outcomes are added
+// to it (ReportingMetrics, the counting pass of ht2_sam.h)
 bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read_batch_t* b, const char* names,
                       const ht2gpu_result_batch_t* res, char** out, size_t* out_len, unsigned nthreads, const uint8_t* ssT = NULL,
-                      uint32_t* colCount = NULL, struct Ht2SsRec* colRecs = NULL, uint32_t colCap = 0);
+                      uint32_t* colCount = NULL, struct Ht2SsRec* colRecs = NULL, uint32_t colCap = 0,
+                      const Ht2SamOutput* so = NULL, ht2gpu_align_counts_t* counts = NULL);
+// AlnSink::printAlSumm (aln_sink.h:1613-1816) with canRep = false (mhits is always 0, hisat2.cpp:1882-1884)
+void ht2_format_align_summary(std::string& o, const ht2gpu_align_counts_t& c, bool newStyle, bool discord, bool mixed);
 
 #endif

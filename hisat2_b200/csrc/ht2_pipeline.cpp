@@ -19,6 +19,8 @@
 #include "../../include/ht2gpu.h"
 #include "ht2_reads.h"
 
+bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b);   // ht2_gpu.cu
+
 namespace {
 double nowS() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 void* pinAlloc(size_t n) { return ht2gpu_host_alloc(n); }
@@ -63,6 +65,8 @@ extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2g
     if (!hs || nDev < 1 || !in) return HT2GPU_ERR_ARG;
     for (int i = 0; i < nDev; i++) if (!hs[i]) return HT2GPU_ERR_ARG;
     ht2gpu_handle_t* h = hs[0];
+    for (int i = 1; i < nDev; i++)
+        if (!ht2_same_sam_output(h, hs[i])) { ht2gpu_set_error(h, "ht2gpu_run_reads_multi: the handles' SAM output settings differ"); return HT2GPU_ERR_ARG; }
     ht2gpu_run_stats_t S; memset(&S, 0, sizeof(S));
     const double t0 = nowS();
     unsigned nth = in->threads > 0 ? (unsigned)in->threads : std::thread::hardware_concurrency();

@@ -43,7 +43,20 @@ struct Ht2SamIn {
     uint32_t*       colCount;    // --novel-splicesite-outfile: junctions of the printed alignments (write pass only), or NULL
     Ht2SsRec*       colRecs;
     uint32_t        colCap;
+    // SAM output settings (ht2gpu_set_sam_output)
+    uint32_t        noUnal;      // --no-unal: appendMate prints nothing for rs == NULL (aln_sink.h:3040)
+    uint32_t        omitSecSeq;  // --omit-sec-seq: SEQ / QUAL '*' in non-primary records (aln_sink.h:3190-3215)
+    const char*     rgTag;       // "RG:Z:<id>" or NULL (sam.h:780, 1102)
 };
+
+// ReportingMetrics (aln_sink.h:2007-2346) of the units a formatter pass went through, in the field order of
+// ht2gpu_align_counts_t.  The *_rep counters need -M: hisat2.cpp:1882-1884 sets mhits to 0 whatever the options
+// (line 1883), so pairMax / unpair1Max / unpair2Max are never set and nconcord_rep, nunp_0_rep and nunp_rep stay 0;
+// they are not kept.
+enum { HT2_T_NREAD, HT2_T_NPAIRED, HT2_T_NUNPAIRED, HT2_T_NCONCORD_0, HT2_T_NCONCORD_UNI1, HT2_T_NCONCORD_UNI2, HT2_T_NDISCORD,
+       HT2_T_NUNP_0_0, HT2_T_NUNP_0_UNI1, HT2_T_NUNP_0_UNI2, HT2_T_NUNP_0, HT2_T_NUNP_UNI1, HT2_T_NUNP_UNI2, HT2_T_N };
+struct Ht2SamTally { uint32_t c[HT2_T_N]; };
+static_assert(sizeof(ht2gpu_align_counts_t) == HT2_T_N * sizeof(uint64_t), "ht2gpu_align_counts_t follows the tally's order");
 
 template <bool WRITE>
 struct Ht2SamOut {
@@ -358,6 +371,10 @@ struct Ht2SamFmt {
         else if (!rd.nfilt) o.s("\tYF:Z:NS");
         else if (!rd.scfilt) o.s("\tYF:Z:SC");
     }
+    // the read group follows YT:Z / YF:Z and precedes XS:A / NH:i (sam.h:780, 1102)
+    template <bool W> HT2_HD void putRG(Ht2SamOut<W>& o) const {
+        if (in->rgTag) { o.c('\t'); o.s(in->rgTag); }
+    }
 
     // SpliceSiteDB::addSpliceSite (splice_site.cpp:190-350) for one printed alignment: every junction whose anchors
     // are long enough (15 bases + 2 per mismatch / gap on its side, + 6 without a canonical motif) is recorded with the
@@ -430,6 +447,7 @@ struct Ht2SamFmt {
     template <bool W>
     HT2_NI void appendMate(Ht2SamOut<W>& o, const Ht2SamRead& rd, uint32_t ordlen, const ht2gpu_aln_t* rs, const ht2gpu_aln_t* rso,
                            const Ht2SamSumm& summ, const Ht2SamFlags& fl, bool fraglenSet, int64_t fraglen, bool haveOscore) const {
+        if (rs == NULL && in->noUnal) return;
         putName(o, rd.name, fl.partOfPair());
         o.c('\t');
         int flag = 0;
@@ -452,6 +470,7 @@ struct Ht2SamFmt {
             putSeqQual(o, rd, true);
             o.s("\tYT:Z:"); o.s(ytz);
             putYF(o, rd);
+            putRG(o);
             o.c('\n');
             return;
         }
@@ -556,7 +575,8 @@ struct Ht2SamFmt {
         } else o.s("*\t0\t");
         o.i64(fraglenSet ? fraglen : 0);
         o.c('\t');
-        putSeqQual(o, rd, rs->fw != 0);
+        if (!fl.primary && in->omitSecSeq) o.s("*\t*");
+        else putSeqQual(o, rd, rs->fw != 0);
         // optional flags (sam.h:525-1010)
         o.s("\tAS:i:"); o.i64(rs->score);
         const Ht2SamKey& sb = summ.secbest[rd.mate < 2 ? 0 : 1];
@@ -621,6 +641,7 @@ struct Ht2SamFmt {
         if (summ.paired && haveOscore && rso) { o.s("\tYS:i:"); o.i64(rso->score); }
         o.s("\tYT:Z:"); o.s(ytz);
         putYF(o, rd);
+        putRG(o);
 #ifdef HT2_ENABLE_SPLICED
         {   // XS:A: AlnRes::spliced_whichsense_transcript (aligner_result.h:1288-1318, sam.h:925-937)
             uint32_t whichsense = HT2_SPL_UNKNOWN; bool any = false;
@@ -683,7 +704,7 @@ struct Ht2SamFmt {
     }
 
     // finishRead for an unpaired read (aln_sink.h:2213-2557, unpaired branches)
-    template <bool W> HT2_HD void finishUnpaired(Ht2SamOut<W>& o, uint32_t u) const {
+    template <bool W> HT2_HD void finishUnpaired(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t) const {
         const ht2gpu_read_result_t& rr = in->reads[u];
         Ht2SamRead rd; mkRead(u, 0, rd);
         Ht2Rng rnd; rnd.last = rr.rng_state;
@@ -692,21 +713,27 @@ struct Ht2SamFmt {
         const uint64_t nunpair1 = n < in->khits ? n : in->khits;   // ReportingState::getReport
         Ht2SamSumm summ; summ.reset();
         Ht2SamFlags fl = {HT2_PAIR_UNPAIRED, true, false};
+        if (t) { t->c[HT2_T_NREAD]++; t->c[HT2_T_NUNPAIRED]++; }
         if (nunpair1 > 0) {
             addUnp(summ, 0, rs, n, rd.len);
             uint16_t sel[HT2_SAM_MAXSEL];
             const uint32_t nsel = selectByScore(rs, n, rd.len, NULL, 0, NULL, 0, false, nunpair1, sel, rnd);
             summ.numAlns[0] = nsel;
+            if (t) { t->c[HT2_T_NUNP_UNI1] += (uint32_t)(nsel == 1); t->c[HT2_T_NUNP_UNI2] += (uint32_t)(nsel != 1); }   // aln_sink.h:2290-2299
             for (uint32_t i = 0; i < nsel; i++) {
                 fl.primary = (i == 0);
                 appendMate(o, rd, 0, &rs[sel[i]], NULL, summ, fl, false, 0, false);
             }
-        } else appendMate(o, rd, 0, NULL, NULL, summ, fl, false, 0, false);
+        } else {
+            if (t) t->c[HT2_T_NUNP_0]++;
+            appendMate(o, rd, 0, NULL, NULL, summ, fl, false, 0, false);
+        }
     }
 
     // AlnSinkWrap::finishRead for a pair (aln_sink.h:1939-2557)
-    template <bool W> HT2_HD void finishPaired(Ht2SamOut<W>& o, uint32_t u) const {
+    template <bool W> HT2_HD void finishPaired(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t) const {
         const ht2gpu_read_result_t& rr = in->reads[u];
+        if (t) { t->c[HT2_T_NREAD]++; t->c[HT2_T_NPAIRED]++; }
         Ht2SamRead rd1, rd2; mkRead(2 * u, 1, rd1); mkRead(2 * u + 1, 2, rd2);
         Ht2Rng rnd; rnd.last = rr.rng_state;
         const ht2gpu_aln_t* rs1u = in->alns + rr.aln_off;
@@ -738,6 +765,7 @@ struct Ht2SamFmt {
             addUnp(summ, 0, rs1u, n1, rd1.len); addUnp(summ, 1, rs2u, n2, rd2.len);
             const uint32_t nsel = selectByScore(rs1u, n1, rd1.len, rs2u, rd2.len, pairs, np, true, nconcord, sel, rnd);
             summ.numAlnsPaired = nsel;
+            if (t) { t->c[HT2_T_NCONCORD_UNI1] += (uint32_t)(nsel == 1); t->c[HT2_T_NCONCORD_UNI2] += (uint32_t)(nsel != 1); }   // select1_.size(), aln_sink.h:2100-2110
             Ht2SamFlags fl1 = {HT2_PAIR_CONCORD_MATE1, true, true}, fl2 = {HT2_PAIR_CONCORD_MATE2, true, true};
             for (uint32_t i = 0; i < nsel; i++) {
                 const ht2gpu_aln_t& a = rs1u[pairs[2 * sel[i]]]; const ht2gpu_aln_t& b = rs2u[pairs[2 * sel[i] + 1]];
@@ -747,6 +775,7 @@ struct Ht2SamFmt {
             }
             return;
         } else if (discordant) {
+            if (t) { t->c[HT2_T_NCONCORD_0]++; t->c[HT2_T_NDISCORD]++; }   // aln_sink.h:2191-2192
             Ht2SamSumm summ; summ.reset();
             summ.paired = true;
             const ht2gpu_aln_t& a = rs1u[0]; const ht2gpu_aln_t& b = rs2u[0];
@@ -786,6 +815,12 @@ struct Ht2SamFmt {
         // numAlns1/2 setters are applied to both summaries (aln_sink.h:2238-2239, 2263-2264)
         if (rep1) { summ1.numAlns[0] = nsel1; summ2.numAlns[0] = nsel1; }
         if (rep2) { summ1.numAlns[1] = nsel2; summ2.numAlns[1] = nsel2; }
+        if (t) {   // aln_sink.h:2271-2346 (constant indexes: the device tally stays in registers)
+            t->c[HT2_T_NCONCORD_0]++;
+            t->c[HT2_T_NUNP_0_0] += (uint32_t)!rep1 + (uint32_t)!rep2;
+            t->c[HT2_T_NUNP_0_UNI1] += (uint32_t)(rep1 && nsel1 == 1) + (uint32_t)(rep2 && nsel2 == 1);
+            t->c[HT2_T_NUNP_0_UNI2] += (uint32_t)(rep1 && nsel1 != 1) + (uint32_t)(rep2 && nsel2 != 1);
+        }
         Ht2SamFlags fl1 = {HT2_PAIR_UNPAIRED_MATE1, true, repRs2 != NULL}, fl2 = {HT2_PAIR_UNPAIRED_MATE2, true, repRs1 != NULL};
         int64_t refid = -1, refoff = -1;
         if (rep1) {
@@ -829,8 +864,9 @@ struct Ht2SamFmt {
         }
     }
 
-    template <bool W> HT2_HD void unit(Ht2SamOut<W>& o, uint32_t u) const {
-        if (in->paired) finishPaired(o, u); else finishUnpaired(o, u);
+    // t != NULL: also tally the unit's outcome (the counting pass)
+    template <bool W> HT2_HD void unit(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t = NULL) const {
+        if (in->paired) finishPaired(o, u, t); else finishUnpaired(o, u, t);
     }
 };
 

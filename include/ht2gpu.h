@@ -244,7 +244,8 @@ typedef struct {
 int ht2gpu_run_reads(ht2gpu_handle_t* h, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx, ht2gpu_run_stats_t* stats);
 /* The same over several devices of ONE process (hisat2 -p N + --reorder, hisat2.cpp:3657-3696, outq.cpp:51-99, with
  * GPUs in place of threads): batch i runs on hs[i % n], the sink receives the batches in input order.  Every handle
- * holds a replica of the same index (ht2gpu_open_peer); reads are the only thing that is sharded. */
+ * holds a replica of the same index (ht2gpu_open_peer); reads are the only thing that is sharded.  Handles whose
+ * SAM output settings (ht2gpu_set_sam_output) differ are refused with HT2GPU_ERR_ARG. */
 int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int n, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
                            ht2gpu_run_stats_t* stats);
 /* Replicate an open index onto another device of this process: the packed image is copied device to device
@@ -325,8 +326,43 @@ int ht2gpu_index_is_graph(const ht2gpu_handle_t* h);
  * buffer is malloc'ed; free with ht2gpu_free_text. */
 int ht2gpu_format_sam(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* batch, const char* names,
                       const ht2gpu_result_batch_t* res, char** out, size_t* out_len);
+/* @HD, @SQ (unless no_sq) and @RG (when a read-group id is set) of ht2gpu_set_sam_output: SamConfig::printHeader
+ * (sam.h:446-463) without @PG. */
 int ht2gpu_sam_header(ht2gpu_handle_t* h, char** out, size_t* out_len);
 void ht2gpu_free_text(char* p);
+
+/* ---- SAM output settings and the alignment summary ------------------------------
+ * SAM output settings of a handle (AlnSinkSam::appendMate aln_sink.h:3040, 3190-3215; sam.h:446-463, 780, 1102):
+ *   no_unal       --no-unal: no record for a read (mate) without an alignment; its aligned mate keeps its record
+ *   omit_sec_seq  --omit-sec-seq: SEQ and QUAL are '*' in non-primary records
+ *   no_sq         --no-sq: ht2gpu_sam_header prints no @SQ lines
+ *   rg_id         --rg-id: "@RG\tID:<rg_id>" (+ "\t<rg[i]>" for every --rg field) in the header, "RG:Z:<rg_id>" in
+ *                 every record; NULL or "" = no read group (the rg fields are then not printed either)
+ * All off by default.  Set between batches, like ht2gpu_load_splicesites (refused while a batch is in flight). */
+typedef struct {
+    int32_t no_unal, omit_sec_seq, no_sq;
+    const char* rg_id;
+    const char* const* rg;
+    int32_t n_rg;
+} ht2gpu_sam_output_t;
+int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output_t* cfg);
+
+/* Per-read outcome counts of ReportingMetrics (aln_sink.h:2007-2012, 2100-2110, 2191-2192, 2271-2346), tallied by the
+ * SAM kernels for every read (pair) formatted through ht2gpu_wait_sam (ht2gpu_align_sam, ht2gpu_run_reads(_multi)).
+ * Reads that fail the length / N / score filters count as unaligned; reads skipped by -s / -u are not counted. */
+typedef struct {
+    uint64_t nread, npaired, nunpaired;
+    uint64_t nconcord_0, nconcord_uni1, nconcord_uni2, ndiscord;
+    uint64_t nunp_0_0, nunp_0_uni1, nunp_0_uni2;   /* mates of pairs without a concordant / discordant alignment */
+    uint64_t nunp_0, nunp_uni1, nunp_uni2;         /* unpaired reads */
+} ht2gpu_align_counts_t;
+/* The sum over hs[0..n) of the counts since open (or since the last reset); reset != 0 zeroes them afterwards. */
+int ht2gpu_align_counts(ht2gpu_handle_t** hs, int n, int reset, ht2gpu_align_counts_t* out);
+/* Host only (no device): the alignment summary hisat2 prints at the end of a run, AlnSink::printAlSumm
+ * (aln_sink.h:1613-1816).  new_style = --new-summary; discordant / mixed = 0 under --no-discordant / --no-mixed
+ * (the classic format then leaves out that section).  Free *out with ht2gpu_free_text. */
+int ht2gpu_format_align_summary(const ht2gpu_align_counts_t* c, int new_style, int discordant, int mixed,
+                                char** out, size_t* out_len);
 
 /* Reference-sequence names and lengths (ht2_index_getrefnames, ht2.h:108). */
 uint32_t ht2gpu_num_refs(const ht2gpu_handle_t* h);

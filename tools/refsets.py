@@ -6,12 +6,15 @@ tiny.snp) by the seeded generators tools/simreads.py and tools/altreads.py, so t
   python tools/refsets.py --edge # only the edge/* cases (tools/edgereads.py); also writes tests/golden/edge_se.sam
   python tools/refsets.py --spliced  # only the spliced/* and spliced_novel/* cases (tools/splicereads.py); also
                                      # writes tests/golden/edge_spliced_se.sam (SPLICED_GOLDEN)
+  python tools/refsets.py --output   # only tests/golden/output_sets.json: the output/* cases (SAM output options) and
+                                     # the alignment summaries summary/* and summary_new/* (verbatim, under "summary")
 
 The expected values come from oracle/_ref/hisat2-align-s (oracle/Makefile).  Cases whose reads can hit a fixed device
 capacity list the flagged reads (`flagged`, from a GPU run of the library); their md5 excludes those reads' records."""
 import hashlib
 import json
 import os
+import re
 import subprocess
 import sys
 import tempfile
@@ -21,6 +24,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 TOOLS = os.path.join(ROOT, "tools")
 REFBIN = os.path.join(ROOT, "oracle", "_ref", "hisat2-align-s")
 OUT = os.path.join(GOLDEN, "ref_sets.json")
+OUTPUT_OUT = os.path.join(GOLDEN, "output_sets.json")   # --output: SAM output options and alignment summaries
 
 # name -> generator arguments (every set is written as <name>_1.fa / <name>_2.fa)
 SETS = {
@@ -102,6 +106,159 @@ SPLICE_SEED = 17
 SPLICED_GOLDEN = (b"len_", b"sense_")
 
 
+# output/<case>: SAM output options (--no-unal, --rg-id / --rg, --omit-sec-seq, --no-sq) on the sets above.
+# case -> (input, reference flags, library options, SAM output settings of Index.set_sam_output).  An input is
+# ("se" | "paired" | "graph_se" | "graph_pe", <set>), ("edge", <EDGE_CASES key>), ("spliced", <SPLICED_CASES key>) or
+# ("dp", <DP_CASES index>).  Only inputs without flagged reads.
+RG = ["--rg-id", "g1", "--rg", "SM:s1", "--rg", "PL:ILLUMINA"]
+RG_OUT = dict(rg_id="g1", rg=("SM:s1", "PL:ILLUMINA"))
+OUTPUT_CASES = {
+    "no_unal_se_hard20k": (("se", "hard20k"), ["--no-unal"], {}, dict(no_unal=1)),
+    "no_unal_pe_hard20k": (("paired", "hard20k"), ["--no-unal"], {}, dict(no_unal=1)),
+    "no_unal_pe_hard20k_no_mixed": (("paired", "hard20k"), ["--no-unal", "--no-mixed"], dict(no_mixed=1), dict(no_unal=1)),
+    "no_unal_edge_se": (("edge", "se"), ["--no-unal"], {}, dict(no_unal=1)),
+    "no_unal_spliced_edge_pe": (("spliced", "edge_pe"), ["--no-unal"], {}, dict(no_unal=1)),
+    "rg_graph_pe_alt20k": (("graph_pe", "alt20k"), RG, {}, RG_OUT),
+    "rg_spliced_ss_edge_se": (("spliced", "ss_edge_se"), RG, {}, RG_OUT),
+    "rg_id_from_rg_se_reads": (("se", "reads"), ["--rg", "ID:g2", "--rg", "LB:x"], {}, dict(rg_id="g2", rg=("LB:x",))),
+    "rg_without_id_se_reads": (("se", "reads"), ["--rg", "SM:only"], {}, dict(rg=("SM:only",))),
+    "omit_sec_seq_k30_se_reads": (("se", "reads"), ["--omit-sec-seq", "-k", "30", "--secondary"], dict(khits=30, secondary=1), dict(omit_sec_seq=1)),
+    "omit_sec_seq_k5_se_reads": (("se", "reads"), ["--omit-sec-seq", "-k", "5"], dict(khits=5), dict(omit_sec_seq=1)),
+    "omit_sec_seq_k30_pe_sim10k": (("paired", "sim10k"), ["--omit-sec-seq", "-k", "30", "--secondary"], dict(khits=30, secondary=1), dict(omit_sec_seq=1)),
+    "omit_sec_seq_k5_pe_sim10k": (("paired", "sim10k"), ["--omit-sec-seq", "-k", "5"], dict(khits=5), dict(omit_sec_seq=1)),
+    "no_sq_se_reads": (("se", "reads"), ["--no-sq"], {}, dict(no_sq=1)),
+}
+# summary/<case> and summary_new/<case>: the reference's alignment summary (stderr), classic and --new-summary.
+# case -> (input, reference flags, library options, read front-end options of ht2gpu_reads_input_t)
+SUMMARY_CASES = {
+    "se_reads": (("se", "reads"), [], {}, {}),
+    "se_hard20k": (("se", "hard20k"), [], {}, {}),
+    "pe_sim10k": (("paired", "sim10k"), [], {}, {}),
+    "pe_hard20k": (("paired", "hard20k"), [], {}, {}),
+    "graph_se_alt20k": (("graph_se", "alt20k"), [], {}, {}),
+    "graph_pe_alt20k": (("graph_pe", "alt20k"), [], {}, {}),
+    "edge_se": (("edge", "se"), [], {}, {}),
+    "edge_pe": (("edge", "pe"), [], {}, {}),
+    "spliced_sim_pe": (("spliced", "sim_pe"), [], {}, {}),
+    "spliced_edge_se": (("spliced", "edge_se"), [], {}, {}),
+    "pe_hard20k_no_mixed": (("paired", "hard20k"), ["--no-mixed"], dict(no_mixed=1), {}),
+    "pe_hard20k_no_discordant": (("paired", "hard20k"), ["--no-discordant"], dict(no_discordant=1), {}),
+    "pe_hard20k_no_mixed_no_discordant": (("paired", "hard20k"), ["--no-mixed", "--no-discordant"], dict(no_mixed=1, no_discordant=1), {}),
+    "pe_hard20k_k1": (("paired", "hard20k"), ["-k", "1"], dict(khits=1), {}),
+    "se_reads_skip100_upto300": (("se", "reads"), ["-s", "100", "-u", "300"], {}, dict(skip=100, upto=300)),
+    "dp1_sensitive": (("dp", 1), [], {}, {}),
+}
+SUMMARY_SETS = ("reads", "sim10k", "hard20k", "alt20k")
+# rep_1.fa (generate_repeats): 100-base reads of the segments tiny.fa holds twice.  Under -k 30 --secondary every read
+# prints two records, more SAM text than the device's first estimate per read, so the SAM kernels run again
+SUMMARY_CASES["rep_k30_secondary"] = (("se", "rep"), ["-k", "30", "--secondary"], dict(khits=30, secondary=1), {})
+
+
+def generate_repeats(outdir, rdlen=100, n=1000):
+    """rep_1.fa under outdir: every fifth of the rdlen-base windows of tiny.fa whose sequence (or reverse complement)
+    occurs exactly twice, at most n reads, in reference order.  Deterministic; returns outdir."""
+    path = os.path.join(outdir, "rep_1.fa")
+    if os.path.exists(path):
+        return outdir
+    seqs, cur = {}, None
+    for l in open(os.path.join(GOLDEN, "tiny.fa")):
+        l = l.strip()
+        if l.startswith(">"):
+            cur = l[1:].split()[0]
+            seqs[cur] = []
+        elif cur is not None:
+            seqs[cur].append(l.upper())
+    comp = str.maketrans("ACGT", "TGCA")
+    count, order = {}, []
+    for name, parts in seqs.items():
+        s = "".join(parts)
+        for i in range(len(s) - rdlen + 1):
+            w = s[i:i + rdlen]
+            if "N" in w:
+                continue
+            key = min(w, w.translate(comp)[::-1])
+            count[key] = count.get(key, 0) + 1
+            order.append((name, i, w, key))
+    reads = [(name, i, w) for name, i, w, key in order if count[key] == 2][::5][:n]
+    with open(path, "w") as f:
+        for name, i, w in reads:
+            f.write(">rep_%s_%d\n%s\n" % (name, i, w))
+    return outdir
+
+
+def generate_output_sets(d):
+    """Every read set the OUTPUT_CASES and SUMMARY_CASES use, under d; returns d."""
+    generate(d, SUMMARY_SETS)
+    generate_repeats(d)
+    generate_edge(d)
+    generate_spliced(d)
+    return d
+
+
+def output_input(d, src):
+    """(index, read files, format flag, reference flags, library options, known-splice-site file or None) of an
+    OUTPUT_CASES / SUMMARY_CASES input under d (generate(d, SUMMARY_SETS), generate_edge(d) and generate_spliced(d))."""
+    kind, name = src
+    if kind in ("se", "paired", "graph_se", "graph_pe"):
+        paired = kind in ("paired", "graph_pe")
+        fs = [os.path.join(d, name + "_1.fa")] + ([os.path.join(d, name + "_2.fa")] if paired else [])
+        return ("tiny_snp" if kind.startswith("graph") else "tiny"), fs, "-f", ["--no-spliced-alignment"], {}, None
+    if kind == "edge":
+        index, _, fmt, flags, opts, _ = EDGE_CASES[name]
+        return index, edge_files(d, name), fmt, ["--no-spliced-alignment"] + flags, dict(opts), None
+    if kind == "spliced":
+        index, _, fmt, flags, opts, _ = SPLICED_CASES[name]
+        fs, ss = spliced_files(d, name)
+        return index, fs, fmt, ["--no-temp-splicesite"] + flags + (["--known-splicesite-infile", ss] if ss else []), \
+            dict(opts, no_spliced_alignment=0), ss
+    index, setname, paired, flags, opts = DP_CASES[name]
+    fs = [os.path.join(d, setname + "_1.fa")] + ([os.path.join(d, setname + "_2.fa")] if paired else [])
+    return index, fs, "-f", ["--no-spliced-alignment"] + flags, dict(opts), None
+
+
+def summary_text(stderr):
+    """The alignment summary at the end of the reference's stderr (warnings come earlier)."""
+    lines = stderr.decode().splitlines(True)
+    for i, l in enumerate(lines):
+        if re.match(r"^\d+ reads", l) or l.startswith("HISAT2 summary stats:"):
+            return "".join(lines[i:])
+    raise ValueError("no alignment summary in the reference's stderr")
+
+
+def reference_run(d, src, flags):
+    """(SAM, stderr) of the unmodified reference on an OUTPUT_CASES / SUMMARY_CASES input (--reorder)."""
+    index, fs, fmt, base, _, _ = output_input(d, src)
+    out = os.path.join(d, "ref.sam")
+    reads = ["-1", fs[0], "-2", fs[1]] if len(fs) == 2 else ["-U", fs[0]]
+    r = subprocess.run([REFBIN, fmt, "-x", os.path.join(GOLDEN, index)] + base + list(flags) + reads +
+                       ["-S", out, "-p", str(min(16, os.cpu_count() or 1)), "--reorder"], check=True, stderr=subprocess.PIPE)
+    return open(out, "rb").read(), r.stderr
+
+
+def load_output_expected():
+    return json.load(open(OUTPUT_OUT))
+
+
+def output_main():
+    """Writes OUTPUT_OUT: {"md5": output/<case> md5s, "summary": summary/<case>, summary_new/<case> texts}."""
+    md5, summary = {}, {}
+    with tempfile.TemporaryDirectory() as d:
+        output_reference(d, md5, summary)
+    json.dump({"md5": md5, "summary": summary}, open(OUTPUT_OUT, "w"), indent=1, sort_keys=True)
+    open(OUTPUT_OUT, "a").write("\n")
+
+
+def output_reference(d, md5, summary):
+    """output/<case> md5s and summary/<case>, summary_new/<case> texts."""
+    generate_output_sets(d)
+    for case, (src, flags, _, _) in sorted(OUTPUT_CASES.items()):
+        sam, _ = reference_run(d, src, flags)
+        md5["output/" + case] = sam_md5(sam)
+    for case, (src, flags, _, _) in sorted(SUMMARY_CASES.items()):
+        summary["summary/" + case] = summary_text(reference_run(d, src, flags)[1])
+        summary["summary_new/" + case] = summary_text(reference_run(d, src, flags + ["--new-summary"])[1])
+
+
 def spliced_golden_lines(sam):
     """The SAM lines (headers without @PG, records of the SPLICED_GOLDEN reads) kept as edge_spliced_se.sam."""
     return [l for l in sam.splitlines(True) if (l.startswith(b"@") and not l.startswith(b"@PG")) or l.startswith(SPLICED_GOLDEN)]
@@ -175,7 +332,10 @@ def reference(d, index, name, paired, flags=(), fa=False, fmt="-f"):
     return open(out, "rb").read()
 
 
-def main(edge_only=False, spliced_only=False):
+def main(edge_only=False, spliced_only=False, output_only=False):
+    if output_only:
+        output_main()
+        return
     old = json.load(open(OUT)) if os.path.exists(OUT) else {}
     flagged = old.get("flagged", {})
     md5 = {}
@@ -222,6 +382,7 @@ def main(edge_only=False, spliced_only=False):
         spliced_reference(d, md5, flagged)
     json.dump({"md5": md5, "flagged": flagged}, open(OUT, "w"), indent=1, sort_keys=True)
     open(OUT, "a").write("\n")
+    output_main()
 
 
 def spliced_reference(d, md5, flagged):
@@ -257,4 +418,4 @@ def edge_reference(d, md5, flagged):
 
 
 if __name__ == "__main__":
-    main(edge_only="--edge" in sys.argv[1:], spliced_only="--spliced" in sys.argv[1:])
+    main(edge_only="--edge" in sys.argv[1:], spliced_only="--spliced" in sys.argv[1:], output_only="--output" in sys.argv[1:])
