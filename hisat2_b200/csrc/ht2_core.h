@@ -280,7 +280,8 @@ struct alignas(128) Ht2Work {
     uint32_t    hybIter, hybHj, mateI, mateJ, mateSize[2];
     // partialSearch continuation (time slicing, HT2_PS_SLICE): a search that has not finished after a slice of LF
     // steps parks its loop state here and the slot stays in TS_PS, so that a round never lasts longer than one slice
-    // while most lanes of the group have long finished (a partial search is ~12 steps on average, ~90 at most)
+    // while most lanes of the group have long finished (a partial search of a 101-bp read is ~12 steps on average,
+    // ~90 at most; the searches of 1 000-base reads run to hundreds)
     uint32_t    psCont, psTop, psBot, psNtop, psNbot, psDep, psSame, psSimilar;
     uint8_t     psPseudo, psAnchor, psPad[2];
     // ---- arrays
@@ -892,8 +893,12 @@ struct Ht2AlignerT {
     // HI_Aligner::partialSearch (hi_aligner.h:6361-6600).  Returns stop
     // flags through pseudogeneStop/anchorStop like the reference.  Returns false when the search was parked after a
     // slice of LF steps (W->psCont): the caller calls again, with the same arguments, to continue it.
+// 128 steps: short-read searches finish in the round that starts them.  Parking costs a round of its own -- a
+// re-claim of the slot and a cold workspace -- so shorter slices cost more than the long lanes they cut: on an H100
+// (400 W), the pool kernel of a 2 M-pair bench-shaped batch takes 156.5 ms at 8 steps, 149.5 ms at 16, 148.3 ms at
+// 32, 146.9 ms at 64, and 143.5 +- 0.4 ms at 128, 256 and 1024 (DESIGN.md 4.1).
 #ifndef HT2_PS_SLICE
-#define HT2_PS_SLICE 16
+#define HT2_PS_SLICE 128
 #endif
     HT2_NI bool partialSearch(uint32_t rdi, bool fw, bool& pseudogeneStop, bool& anchorStop) {
         if (GRAPH) return partialSearchGraph(rdi, fw, pseudogeneStop, anchorStop);
