@@ -525,14 +525,22 @@ ht2_seed_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatch b, u
 //   ht2_sam_scan_kernel   : exclusive scan of the block sums (one block), blk[nBlk] = total
 //   ht2_sam_kernel<true>  : writing pass -- unit offset = block offset + in-block exclusive scan of lens
 // Records land in read order (= --reorder), exactly the bytes AlnSinkWrap::finishRead prints.
+//
+// The block's units fill one contiguous byte range of the output, [blk[b], blk[b+1]).  The writing pass formats
+// them into shared memory at their in-block offsets and then copies the range out with aligned 16-byte stores:
+// one thread's text is a few hundred bytes long, so byte stores straight to global memory would have every store
+// instruction touch 32 different sectors.  A block whose text does not fit the staging buffer (many multi-mapping
+// records, long reads) formats straight into global memory; the bytes are the same either way.
 // ---------------------------------------------------------------------------
 #define HT2_SAM_TPB 128
+#define HT2_SAM_STAGE_BLOCKS 2     // writing-pass blocks per SM the staging buffer leaves room for
 
 template <bool WRITE>
 __global__ void __launch_bounds__(HT2_SAM_TPB)
 ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigned long long* __restrict__ blk, char* __restrict__ out,
-               unsigned long long cap, unsigned int* counters, unsigned long long* __restrict__ tally)
+               unsigned long long cap, unsigned int* counters, unsigned long long* __restrict__ tally, uint32_t stageBytes)
 {
+    extern __shared__ uint4 sStage[];   // writing pass: stageBytes of dynamic shared memory
     __shared__ unsigned long long sWarp[HT2_SAM_TPB / 32];
     __shared__ uint32_t sTally[HT2_SAM_TPB / 32][HT2_T_N];
     const uint32_t u = blockIdx.x * HT2_SAM_TPB + threadIdx.x;
@@ -573,12 +581,26 @@ ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigne
     for (uint32_t w = 0; w < wib; w++) base += sWarp[w];
     if (!WRITE) {
         if (threadIdx.x == HT2_SAM_TPB - 1) blk[blockIdx.x] = base + incl;
-    } else if (u < units) {
-        const unsigned long long at = blk[blockIdx.x] + base + incl - mine;
-        if (at + mine <= cap) {
-            Ht2SamOut<true> o; o.p = out + at; o.n = 0;
-            F.unit(o, u);
-        }
+        return;
+    }
+    // the staging buffer starts at the 16-byte boundary at or below the block's first output byte
+    const unsigned long long b0 = blk[blockIdx.x], b1 = blk[blockIdx.x + 1];
+    const uint32_t head = (uint32_t)(b0 & 15);
+    const bool staged = b1 <= cap && b1 - b0 + head <= stageBytes;   // the same for the whole block
+    char* const stage = (char*)sStage;
+    if (u < units) {
+        const unsigned long long at = base + incl - mine;   // in the block
+        Ht2SamOut<true> o; o.n = 0;
+        if (staged) { o.p = stage + head + at; F.unit(o, u); }
+        else if (b0 + at + mine <= cap) { o.p = out + b0 + at; F.unit(o, u); }
+    }
+    if (!staged) return;
+    __syncthreads();
+    char* const dst = out + (b0 - head);   // out is 16-byte aligned (cudaMalloc)
+    const uint32_t end = head + (uint32_t)(b1 - b0);
+    for (uint32_t lo = threadIdx.x * 16; lo < end; lo += HT2_SAM_TPB * 16) {
+        if (lo >= head && lo + 16 <= end) *(uint4*)(dst + lo) = sStage[lo / 16];
+        else for (uint32_t i = lo < head ? head : lo; i < end && i < lo + 16; i++) dst[i] = stage[i];
     }
 }
 
@@ -615,6 +637,7 @@ struct SamSlot {
     bool         init;
     cudaStream_t stream;
     cudaEvent_t  ev[6];            // start, h2d done, kernel start, align done, sam done, d2h done
+    cudaEvent_t  evSplit[3];       // HT2GPU_SAM_SPLIT=1: before the counting pass, after it, after the block scan
     uint8_t *dSeq, *dQual; uint64_t* dOffs; uint32_t* dSeeds; char* dNames; uint32_t* dNameOffs;
     size_t capSeq, capQual, capOffs, capSeeds, capNames, capNameOffs;
     ht2gpu_read_result_t* dReads; ht2gpu_aln_t* dAlns; ht2gpu_edit_t* dEdits; uint16_t* dPairs; unsigned int* dCounters;
@@ -662,6 +685,7 @@ struct ht2gpu_handle {
     int            device;
     int            nSM;
     int            tpb, bpsm;
+    uint32_t       samStage;  // bytes of the SAM writing pass's staging buffer (dynamic shared memory per block)
     bool           graph;
     int            poolWarps;
     int            rgK;
@@ -837,6 +861,15 @@ static int finishOpen(ht2gpu_handle* h)
         else { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, false, false>)); need = fa.localSizeBytes + 4 * 1024; }
         CK(cudaFuncGetAttributes(&fa, ht2_sam_kernel<true>));
         if (fa.localSizeBytes + 2048 > need) need = fa.localSizeBytes + 2048;
+        // the writing pass's staging buffer: what leaves room for HT2_SAM_STAGE_BLOCKS blocks per SM (1 KB of every
+        // block's shared memory is reserved by the system)
+        int smemSM = 0, smemBlk = 0;
+        CK(cudaDeviceGetAttribute(&smemSM, cudaDevAttrMaxSharedMemoryPerMultiprocessor, h->device));
+        CK(cudaDeviceGetAttribute(&smemBlk, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+        size_t stage = (size_t)smemSM / HT2_SAM_STAGE_BLOCKS - 1024 - fa.sharedSizeBytes;
+        if (stage > (size_t)smemBlk - fa.sharedSizeBytes) stage = (size_t)smemBlk - fa.sharedSizeBytes;
+        h->samStage = (uint32_t)(stage & ~(size_t)15);
+        CK(cudaFuncSetAttribute(ht2_sam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->samStage));
         size_t cur = 0;
         CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
         if (cur < need) CK(cudaDeviceSetLimit(cudaLimitStackSize, need));
@@ -1006,6 +1039,7 @@ extern "C" int ht2gpu_close(ht2gpu_handle_t* h)
         if (S.hMeta) cudaFreeHost(S.hMeta);
         cudaStreamDestroy(S.stream);
         for (int i = 0; i < 6; i++) cudaEventDestroy(S.ev[i]);
+        for (int i = 0; i < 3; i++) if (S.evSplit[i]) cudaEventDestroy(S.evSplit[i]);
     }
     if (h->stream) { cudaStreamDestroy(h->stream); for (int i = 0; i < 4; i++) cudaEventDestroy(h->ev[i]); }
     delete h->img;
@@ -1039,6 +1073,7 @@ static int slotInit(ht2gpu_handle* h, SamSlot& S)
     if (S.init) return HT2GPU_OK;
     CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
     for (int i = 0; i < 6; i++) CK(cudaEventCreate(&S.ev[i]));
+    if (getenv("HT2GPU_SAM_SPLIT")) for (int i = 0; i < 3; i++) CK(cudaEventCreate(&S.evSplit[i]));
     CK(cudaMalloc(&S.dCounters, 8 * sizeof(unsigned int)));
     CK(cudaMalloc(&S.dTally, HT2_T_N * sizeof(unsigned long long)));
     CK(cudaHostAlloc(&S.hMeta, (HT2_META_TALLY + HT2_T_N) * sizeof(unsigned long long), cudaHostAllocPortable));
@@ -1304,9 +1339,13 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
     // the counting pass tallies the batch's ReportingMetrics; a re-run (ht2gpu_wait_sam) must not count it twice
     CK(cudaMemsetAsync(S.dTally, 0, HT2_T_N * sizeof(unsigned long long), S.stream));
     const Ht2SamIn in = samIn(h, S);
-    ht2_sam_kernel<false><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, NULL, 0, S.dCounters, S.dTally);
+    if (S.evSplit[0]) CK(cudaEventRecord(S.evSplit[0], S.stream));
+    ht2_sam_kernel<false><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, NULL, 0, S.dCounters, S.dTally, 0);
+    if (S.evSplit[1]) CK(cudaEventRecord(S.evSplit[1], S.stream));
     ht2_sam_scan_kernel<<<1, 1024, 0, S.stream>>>(S.dBlk, nBlk);
-    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.capSam, S.dCounters, S.dTally);
+    if (S.evSplit[2]) CK(cudaEventRecord(S.evSplit[2], S.stream));
+    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, h->samStage, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.capSam, S.dCounters,
+                                                                        S.dTally, h->samStage);
     CK(cudaGetLastError());
     S.nLaunch += 3;
     CK(cudaEventRecord(S.ev[4], S.stream));
@@ -1402,6 +1441,15 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
         for (int k = 0; k < HT2_T_N; k++) tot[k] += S.hMeta[HT2_META_TALLY + k];
     }
     if (h->dStats) dumpStats(h);
+    if (S.evSplit[0]) {   // HT2GPU_SAM_SPLIT=1: the three SAM kernels of the batch's last SAM pass (investigation aid)
+        float ms[3];
+        CK(cudaEventElapsedTime(&ms[0], S.evSplit[0], S.evSplit[1]));
+        CK(cudaEventElapsedTime(&ms[1], S.evSplit[1], S.evSplit[2]));
+        CK(cudaEventElapsedTime(&ms[2], S.evSplit[2], S.ev[4]));
+        fprintf(stderr, "sam kernels: count %.3f ms  scan %.3f ms  write %.3f ms  total %.3f ms  |  %zu bytes of SAM, %u units  |  "
+                "%.1f GB/s over the three, %.1f GB/s over the writing pass\n", ms[0], ms[1], ms[2], ms[0] + ms[1] + ms[2], total, S.units,
+                total / ((ms[0] + ms[1] + ms[2]) * 1e6), total / (ms[2] * 1e6));
+    }
     const unsigned int* c = (const unsigned int*)&S.hMeta[1];
     out->sam = S.hSam; out->sam_len = total;
     out->n_alns = c[0]; out->n_err_reads = c[4];

@@ -65,11 +65,30 @@ struct Ht2SamOut {
     HT2_HD void c(char ch) { if (WRITE) p[n] = ch; n++; }
     HT2_HD void s(const char* lit) { while (*lit) { c(*lit); lit++; } }
     HT2_HD void i64(int64_t v) {
-        char buf[24]; int k = 0;
         uint64_t u = v < 0 ? (uint64_t)0 - (uint64_t)v : (uint64_t)v;
+        if (!WRITE) {   // the counting pass: the number of digits only
+            uint32_t k = 1;
+            for (uint64_t p = 10; k < 20 && u >= p; p *= 10) k++;
+            n += k + (v < 0);
+            return;
+        }
+        char buf[24]; int k = 0;
         do { buf[k++] = (char)('0' + u % 10); u /= 10; } while (u);
         if (v < 0) c('-');
         while (k) c(buf[--k]);
+    }
+    // cnt bytes, byte i = byteAt(i), 4 to a store once the destination is 4-byte aligned (SEQ / QUAL)
+    template <typename F> HT2_HD void run(uint32_t cnt, F byteAt) {
+        if (WRITE) {
+            char* d = p + n;
+            uint32_t i = 0;
+            for (; i < cnt && ((uintptr_t)(d + i) & 3); i++) d[i] = byteAt(i);
+            for (; i + 4 <= cnt; i += 4)
+                *(uint32_t*)(d + i) = (uint32_t)(uint8_t)byteAt(i) | ((uint32_t)(uint8_t)byteAt(i + 1) << 8) |
+                                      ((uint32_t)(uint8_t)byteAt(i + 2) << 16) | ((uint32_t)(uint8_t)byteAt(i + 3) << 24);
+            for (; i < cnt; i++) d[i] = byteAt(i);
+        }
+        n += cnt;
     }
 };
 
@@ -354,17 +373,13 @@ struct Ht2SamFmt {
     template <bool W> HT2_HD void putSeqQual(Ht2SamOut<W>& o, const Ht2SamRead& rd, bool fw) const {
         const uint32_t n = rd.len;
         if (n == 0) { o.s("*\t*"); return; }   // aln_sink.h:3194, 3210
-        if (W) {
-            char* d = o.p + o.n;
-            if (fw) for (uint32_t i = 0; i < n; i++) d[i] = "ACGTN"[rd.seq[i]];
-            else for (uint32_t i = 0; i < n; i++) { const uint8_t c = rd.seq[n - i - 1]; d[i] = "TGCAN"[c < 4 ? c : 4]; }
-            d[n] = '\t';
-            d += n + 1;
-            if (!rd.qual) for (uint32_t i = 0; i < n; i++) d[i] = 'I';
-            else if (fw) for (uint32_t i = 0; i < n; i++) d[i] = (char)rd.qual[i];
-            else for (uint32_t i = 0; i < n; i++) d[i] = (char)rd.qual[n - i - 1];
-        }
-        o.n += 2 * (uint64_t)n + 1;
+        const uint8_t* sq = rd.seq; const uint8_t* ql = rd.qual;
+        if (fw) o.run(n, [&](uint32_t i) { return "ACGTN"[sq[i]]; });
+        else o.run(n, [&](uint32_t i) { const uint8_t c = sq[n - i - 1]; return "TGCAN"[c < 4 ? c : 4]; });
+        o.c('\t');
+        if (!ql) o.run(n, [&](uint32_t) { return 'I'; });
+        else if (fw) o.run(n, [&](uint32_t i) { return (char)ql[i]; });
+        else o.run(n, [&](uint32_t i) { return (char)ql[n - i - 1]; });
     }
     template <bool W> HT2_HD void putYF(Ht2SamOut<W>& o, const Ht2SamRead& rd) const {
         if (!rd.lenfilt) o.s("\tYF:Z:LN");
