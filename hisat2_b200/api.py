@@ -35,6 +35,11 @@ class CReadBatch(C.Structure):
 
 
 EDIT_DTYPE = np.dtype([("pos", "<u4"), ("chr", "u1"), ("qchr", "u1"), ("type", "u1"), ("pad", "u1"), ("snp_id", "<u4")])
+SW_MAX_EDITS = 128   # HT2GPU_SW_MAX_EDITS
+SW_JOB_DTYPE = np.dtype([("fw", "<u4"), ("tidx", "<u4"), ("toff", "<u4"), ("rdoff", "<u4"), ("len", "<u4"), ("seed", "<u4"),
+                         ("minsc", "<i8"), ("read_off", "<u8"), ("read_len", "<u4"), ("pad", "<u4")])
+SW_RESULT_DTYPE = np.dtype([("found", "<u4"), ("err", "<u4"), ("toff", "<u4"), ("n_edits", "<u4"), ("score", "<i8"),
+                            ("best", "<i8"), ("rnd_next", "<u4"), ("pad", "<u4")])
 ALN_DTYPE = np.dtype([("tidx", "<u4"), ("toff", "<u4"), ("score", "<i4"), ("fw", "u1"), ("mate", "u1"),
                       ("n_edits", "<u2"), ("trim5", "<u2"), ("trim3", "<u2"), ("ref_extent", "<u4"), ("edit_off", "<u4")])
 READ_DTYPE = np.dtype([("aln_off", "<u4"), ("n_aln", "<u2", (2,)), ("pair_off", "<u4"), ("n_pairs", "<u4"),
@@ -102,7 +107,7 @@ EXPORTS = [
     "ht2gpu_host_alloc", "ht2gpu_host_free", "ht2gpu_set_error", "ht2gpu_parse_reads", "ht2gpu_free_parsed",
     "ht2gpu_ctx_get", "ht2gpu_ctx_set", "ht2gpu_run_reads_multi", "ht2gpu_open_peer", "ht2gpu_sw_selftest", "ht2gpu_load_splicesites", "ht2gpu_collect_splicesites",
     "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry", "ht2gpu_set_sam_output", "ht2gpu_align_counts",
-    "ht2gpu_format_align_summary",
+    "ht2gpu_format_align_summary", "ht2gpu_sw_extend",
 ]
 
 
@@ -168,6 +173,7 @@ def load_library(path=None):
     lib.ht2gpu_parse_reads.argtypes = [C.POINTER(CReadsInput), C.POINTER(CParsedReads), C.c_char_p, C.c_size_t]
     lib.ht2gpu_free_parsed.argtypes = [C.POINTER(CParsedReads)]
     lib.ht2gpu_sw_selftest.argtypes = [C.c_int, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64)]
+    lib.ht2gpu_sw_extend.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     lib.ht2gpu_load_splicesites.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.POINTER(C.c_uint32)]
     lib.ht2gpu_collect_splicesites.argtypes = [C.c_void_p, C.c_int]
     lib.ht2gpu_write_novel_splicesites.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.POINTER(C.c_uint64)]
@@ -639,6 +645,28 @@ class Index(object):
         out = (C.c_int32 * 3)()
         self._check(self._lib.ht2gpu_launch_geometry(self._h, out), "ht2gpu_launch_geometry")
         return tuple(int(v) for v in out)
+
+    def sw_extend(self, jobs, warp_fill=True):
+        """ht2gpu_sw_extend: the --bowtie2-dp seed extension on its own, one job per lane, with this handle's options.
+        jobs: dicts with fw, tidx, toff, rdoff, len, minsc, seed, read (str of ACGTN) and qual (Phred+33 str).
+        warp_fill: the pool kernel's DP round (True) or the lane fill.  Returns (SW_RESULT_DTYPE array, list of
+        edit arrays in the reference's convention)."""
+        n = len(jobs)
+        cj = np.zeros(n, dtype=SW_JOB_DTYPE)
+        seqs, quals, off = [], [], 0
+        for i, j in enumerate(jobs):
+            rd, qu = j["read"].encode(), j["qual"].encode()
+            cj[i] = (j["fw"], j["tidx"], j["toff"], j["rdoff"], j["len"], j["seed"], j["minsc"], off, len(rd), 0)
+            seqs.append(_ASC2DNA[np.frombuffer(rd, dtype=np.uint8)]); quals.append(np.frombuffer(qu, dtype=np.uint8))
+            off += len(rd)
+        seq = np.ascontiguousarray(np.concatenate(seqs) if seqs else np.zeros(1, np.uint8), dtype=np.uint8)
+        qual = np.ascontiguousarray(np.concatenate(quals) if quals else np.zeros(1, np.uint8), dtype=np.uint8)
+        res = np.zeros(n, dtype=SW_RESULT_DTYPE)
+        ed = np.zeros(n * SW_MAX_EDITS, dtype=EDIT_DTYPE)
+        self._check(self._lib.ht2gpu_sw_extend(self._h, n, cj.ctypes.data, seq.ctypes.data, qual.ctypes.data, 1 if warp_fill else 0,
+                                               res.ctypes.data, ed.ctypes.data), "ht2gpu_sw_extend")
+        edits = [ed[i * SW_MAX_EDITS:i * SW_MAX_EDITS + min(int(res["n_edits"][i]), SW_MAX_EDITS)] for i in range(n)]
+        return res, edits
 
     def seed_search(self, batch, max_range=4):
         """ht2gpu_seed_search: partial-search chains + coordinates of small ranges."""

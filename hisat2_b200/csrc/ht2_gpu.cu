@@ -257,6 +257,33 @@ __device__ __forceinline__ uint32_t rg_code(const Ht2Work* W)
     return RG_TOP + W->st;
 }
 
+// A round of DP problems (--bowtie2-dp): every lane with a slot (my >= 0: base + my) frames its own rectangle, then the WARP
+// fills the score planes of one problem after the other (ht2_sw.h swFillCoop: a 64-row vector per column instead of
+// a lone lane's 2), and the lanes go back to their own candidates / backtraces (swExtendAnchor -> swFinish).  Run by
+// the pool kernel and by ht2gpu_sw_extend's harness; all 32 lanes must call it.
+template <bool GRAPH, bool NOSPL>
+__device__ __forceinline__ void ht2_dp_round(Ht2AlignerT<GRAPH, NOSPL>& A, Ht2Work* base, int my, uint32_t lane)
+{
+    bool fill = false;
+    if (my >= 0) {
+        Ht2Work* W = base + my;
+        A.attach(W);
+        bool ret;
+        fill = A.swPrepare(W->curRdi, W->genomeHits[W->hybHj], ret);
+        A.swStage = fill ? 1u : 2u; A.swRetv = ret;
+    }
+    __syncwarp();
+    uint32_t m = __ballot_sync(0xffffffffu, fill);
+    while (m) {
+        const int k = __ffs((int)m) - 1;
+        m &= m - 1;
+        Ht2SwScratch* Sk = (Ht2SwScratch*)__shfl_sync(0xffffffffu, (unsigned long long)A.sw, k);
+        uint32_t* pk = (uint32_t*)__shfl_sync(0xffffffffu, (unsigned long long)A.swPl, k);
+        A.swFillCoop(Sk, pk, lane);
+    }
+    __syncwarp();
+}
+
 // ---------------------------------------------------------------------------
 // ht2_align_pool_kernel: block-shared slot pool, warp-independent rounds, lock-free claims.
 //
@@ -366,29 +393,7 @@ ht2_align_pool_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatc
         __threadfence_block();   // acquire: the previous owner's workspace writes
         const long long t0 = o.stats ? clock64() : 0;
 #ifndef HT2_NO_DP
-        if (T == RG_TOP + TS_HYB_DP) {
-            // A round of DP problems (--bowtie2-dp): every lane frames its own rectangle, then the WARP fills the
-            // score planes of one problem after the other (ht2_sw.h swFillCoop: a 64-row vector per column instead
-            // of a lone lane's 2), and the lanes go back to their own candidates / backtraces below.
-            bool fill = false;
-            if (my >= 0) {
-                Ht2Work* W = base + my;
-                A.attach(W);
-                bool ret;
-                fill = A.swPrepare(W->curRdi, W->genomeHits[W->hybHj], ret);
-                A.swStage = fill ? 1u : 2u; A.swRetv = ret;
-            }
-            __syncwarp();
-            uint32_t m = __ballot_sync(0xffffffffu, fill);
-            while (m) {
-                const int k = __ffs((int)m) - 1;
-                m &= m - 1;
-                Ht2SwScratch* Sk = (Ht2SwScratch*)__shfl_sync(0xffffffffu, (unsigned long long)A.sw, k);
-                uint32_t* pk = (uint32_t*)__shfl_sync(0xffffffffu, (unsigned long long)A.swPl, k);
-                A.swFillCoop(Sk, pk, lane);
-            }
-            __syncwarp();
-        }
+        if (T == RG_TOP + TS_HYB_DP) ht2_dp_round(A, base, my, lane);
 #endif
         if (my >= 0) {
             Ht2Work* W = base + my;
@@ -1547,10 +1552,14 @@ extern "C" int ht2gpu_sw_selftest(int device, uint32_t n, uint32_t seed, uint64_
         q.mmpMax = 2 + rnd(6); q.mmpMin = 1 + rnd(q.mmpMax); q.npen = 1 + rnd(2); q.mmcostConstant = rnd(4) == 0;
         q.rdGapConst = 1 + rnd(8); q.rdGapLinear = 1 + rnd(4); q.rfGapConst = 1 + rnd(8); q.rfGapLinear = 1 + rnd(4);
         q.gapbar = 1 + rnd(12);
-        q.nrow = 20 + rnd(HT2_SW_MAX_RDLEN - 20); q.ncol = q.nrow + 40;
+        // rows 1..256: the first problems take 256 and every 32k +- 1 (the warp fill's row blocks), the rest any length;
+        // a quarter of the rectangles are narrowed by up to 20 columns, as frameSeedExtensionRect trims at a contig end
+        static const uint32_t edgeRows[] = {256, 1, 31, 33, 63, 65, 95, 97, 127, 129, 159, 161, 191, 193, 223, 225, 255};
+        q.nrow = it < sizeof(edgeRows) / sizeof(edgeRows[0]) ? edgeRows[it] : 1 + rnd(HT2_SW_MAX_RDLEN);
+        q.ncol = q.nrow + 40 - (rnd(4) == 0 ? rnd(21) : 0);
         for (uint32_t j = 0; j < q.ncol + 8; j++) q.rf[j] = rnd(50) == 0 ? 4 : rnd(4);
         uint32_t k = 0;
-        for (uint32_t j = 20; k < q.nrow && j < q.ncol;) {       // the read: the window with substitutions and small indels
+        for (uint32_t j = q.ncol - q.nrow > 20 ? 20 : q.ncol - q.nrow; k < q.nrow && j < q.ncol;) {   // the read: the window with substitutions and small indels
             const uint32_t r = rnd(100);
             if (r < 3) q.rd[k++] = (uint8_t)rnd(4);
             else if (r < 6) j++;
@@ -1581,11 +1590,105 @@ extern "C" int ht2gpu_sw_selftest(int device, uint32_t n, uint32_t seed, uint64_
 }
 
 namespace {
-struct DevTmp {   // temporaries of one ht2gpu_seed_search call: freed on every return path
+struct DevTmp {   // temporaries of one ht2gpu_seed_search / ht2gpu_sw_extend call: freed on every return path
     std::vector<void*> ptrs;
     template <typename T> cudaError_t alloc(T*& p, size_t bytes) { void* q = NULL; cudaError_t e = cudaMalloc(&q, bytes); if (e == cudaSuccess) ptrs.push_back(q); p = (T*)q; return e; }
     ~DevTmp() { for (void* q : ptrs) cudaFree(q); }
 };
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// ht2gpu_sw_extend: the --bowtie2-dp seed extension on its own, one job per lane, through the production code:
+// warp fill = ht2_dp_round (the pool kernel's DP round) then swExtendAnchor -> swFinish; lane fill = swExtendAnchor
+// (swPrepare + swFill + swFinish).  A warp holds whatever jobs it is given -- ones that fill, ones whose anchor
+// already spans the read, ones refused -- as a round of the pool kernel does.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(32)
+ht2_sw_extend_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, const ht2gpu_sw_job_t* jobs, const uint8_t* seq,
+                     const uint8_t* qual, uint32_t n, Ht2Work* work, Ht2SwScratch* scr, uint32_t* pools, int warpFill,
+                     ht2gpu_sw_result_t* res, ht2gpu_edit_t* edits)
+{
+    const uint32_t lane = threadIdx.x, j = blockIdx.x * 32 + lane;
+    Ht2AlignerT<false, true> A;
+    A.bind(blob, &P, NULL);
+    A.sw = scr + j; A.swPl = pools + (size_t)j * HT2_SW_POOL_WORDS; A.swStride = 1;
+    Ht2Work* W = NULL;
+    if (j < n) {
+        const ht2gpu_sw_job_t& q = jobs[j];
+        W = work + j;                                           // zeroed by the host
+        Ht2Read& R = W->rd[0];
+        const uint32_t len = q.read_len < HT2_MAX_RDLEN ? q.read_len : HT2_MAX_RDLEN;
+        R.len = len;
+        for (uint32_t i = 0; i < len; i++) {
+            const uint8_t c = seq[q.read_off + i], rc = seq[q.read_off + len - 1 - i];
+            R.seq[0][i] = c; R.qual[0][i] = qual[q.read_off + i];
+            R.seq[1][i] = rc < 4 ? (uint8_t)(rc ^ 3) : (uint8_t)4; R.qual[1][i] = qual[q.read_off + len - 1 - i];
+        }
+        W->cfgMinsc[0] = q.minsc; W->cfgMinsc[1] = HT2_IDX_MAX32;
+        W->curRdi = 0; W->hybHj = 0;
+        W->rnd.init(q.seed);
+        A.initHit(W->genomeHits[0], q.fw != 0, q.rdoff, q.len, 0, 0, q.tidx, q.toff, q.toff);
+        A.sw->jbest = HT2_MIN_I64;                              // stays so unless swPrepare frames the problem
+    }
+    bool found = false;
+    if (warpFill) {
+        ht2_dp_round(A, work + (size_t)blockIdx.x * 32, j < n ? (int)lane : -1, lane);
+        if (W) found = A.swExtendAnchor(0, W->genomeHits[0]);
+    } else if (W) {
+        A.attach(W);
+        found = A.swExtendAnchor(0, W->genomeHits[0]);
+    }
+    if (!W) return;
+    const Ht2Hit& gh = W->genomeHits[0];
+    ht2gpu_sw_result_t& r = res[j];
+    r.found = found ? 1u : 0u; r.err = W->err; r.toff = gh.toff; r.n_edits = gh.nedits;
+    r.score = gh.score; r.best = A.sw->jbest;
+    r.rnd_next = W->rnd.nextU32();
+    // the edits are already in the reference's convention: it inverts a reverse-strand list twice (nextAlignment, hybridSearch)
+    const uint32_t ne = gh.nedits < HT2GPU_SW_MAX_EDITS ? gh.nedits : HT2GPU_SW_MAX_EDITS;
+    for (uint32_t k = 0; k < ne; k++) {
+        const Ht2Edit& e = gh.edits[k];
+        ht2gpu_edit_t& d = edits[(size_t)j * HT2GPU_SW_MAX_EDITS + k];
+        d.pos = e.pos; d.chr = e.chr; d.qchr = e.qchr; d.type = e.type; d.pad = e.pad; d.snp_id = e.snpID;
+    }
+}
+
+extern "C" int ht2gpu_sw_extend(ht2gpu_handle_t* h, uint32_t n, const ht2gpu_sw_job_t* jobs, const uint8_t* seq, const uint8_t* qual,
+                                int warp_fill, ht2gpu_sw_result_t* res, ht2gpu_edit_t* edits)
+{
+    if (!h || (n && (!jobs || !seq || !qual || !res || !edits))) return HT2GPU_ERR_ARG;
+    if (h->graph) { h->err = "ht2gpu_sw_extend: linear indexes only"; return HT2GPU_ERR_UNSUPPORTED; }
+    if (n == 0) return HT2GPU_OK;
+    size_t bases = 0;
+    for (uint32_t i = 0; i < n; i++) { const size_t e = (size_t)jobs[i].read_off + jobs[i].read_len; if (e > bases) bases = e; }
+    CK(cudaSetDevice(h->device));
+    const uint32_t nt = (n + 31) / 32 * 32;                  // every lane of a launched warp indexes its own scratch
+    DevTmp tmp;
+    ht2gpu_sw_job_t* dJobs = NULL; uint8_t *dSeq = NULL, *dQual = NULL; Ht2Work* dWork = NULL; Ht2SwScratch* dScr = NULL;
+    uint32_t* dPool = NULL; ht2gpu_sw_result_t* dRes = NULL; ht2gpu_edit_t* dEd = NULL;
+    CK(tmp.alloc(dJobs, sizeof(ht2gpu_sw_job_t) * n));
+    CK(tmp.alloc(dSeq, bases + 1));
+    CK(tmp.alloc(dQual, bases + 1));
+    CK(tmp.alloc(dWork, sizeof(Ht2Work) * n));
+    CK(tmp.alloc(dScr, sizeof(Ht2SwScratch) * nt));
+    CK(tmp.alloc(dPool, sizeof(uint32_t) * (size_t)HT2_SW_POOL_WORDS * nt));
+    CK(tmp.alloc(dRes, sizeof(ht2gpu_sw_result_t) * n));
+    CK(tmp.alloc(dEd, sizeof(ht2gpu_edit_t) * (size_t)HT2GPU_SW_MAX_EDITS * n));
+    CK(cudaMemcpy(dJobs, jobs, sizeof(ht2gpu_sw_job_t) * n, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dSeq, seq, bases, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dQual, qual, bases, cudaMemcpyHostToDevice));
+    CK(cudaMemset(dWork, 0, sizeof(Ht2Work) * n));
+    CK(cudaMemset(dScr, 0, sizeof(Ht2SwScratch) * nt));
+    CK(cudaMemset(dEd, 0, sizeof(ht2gpu_edit_t) * (size_t)HT2GPU_SW_MAX_EDITS * n));
+    size_t lim = 0;
+    CK(cudaDeviceGetLimit(&lim, cudaLimitStackSize));
+    if (lim < 8192) CK(cudaDeviceSetLimit(cudaLimitStackSize, 8192));
+    ht2_sw_extend_kernel<<<nt / 32, 32>>>(h->dBlob, h->P, dJobs, dSeq, dQual, n, dWork, dScr, dPool, warp_fill, dRes, dEd);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(res, dRes, sizeof(ht2gpu_sw_result_t) * n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(edits, dEd, sizeof(ht2gpu_edit_t) * (size_t)HT2GPU_SW_MAX_EDITS * n, cudaMemcpyDeviceToHost));
+    return HT2GPU_OK;
 }
 
 extern "C" int ht2gpu_seed_search(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* b, uint32_t maxRange, ht2gpu_seed_result_t* res)

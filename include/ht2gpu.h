@@ -397,6 +397,29 @@ int ht2gpu_write_novel_splicesites(ht2gpu_handle_t** hs, int n, const char* path
  * problems (aligner_swsse_ee_u8.cpp:791-1163 restated twice, ht2_sw.h).  out[0] = mismatching cells / scores
  * (must be 0), out[1] = problems run, out[2] = cells compared per plane, out[3] = problems with a valid best. */
 int ht2gpu_sw_selftest(int device, uint32_t n, uint32_t seed, uint64_t out[4]);
+/* Diagnostics: the --bowtie2-dp seed extension (the dp block of SplicedAligner::hybridSearch) on n jobs, one per
+ * lane, with the handle's options and (linear) index.  Job i aligns the read at seq / qual[read_off, + read_len)
+ * (codes 0..4, Phred+33) on strand fw, framed by the anchor (tidx, toff, rdoff, len), with minsc and a
+ * RandomSource seeded with seed.  warp_fill != 0 runs the pool kernel's DP round (the warp fills the planes of
+ * one problem after the other), 0 the lane fill.  res[i]: found, the per-read error bits, the hit's toff and
+ * score, the best last-row score (INT64_MIN when the DP did not run or nothing reached minsc), n_edits and the
+ * first draw of the RandomSource afterwards; its edits (the reference's convention) are at
+ * edits[i * HT2GPU_SW_MAX_EDITS].  Device temporaries are sized for the n jobs and freed before returning. */
+#define HT2GPU_SW_MAX_EDITS 128
+typedef struct {
+    uint32_t fw, tidx, toff, rdoff, len;
+    uint32_t seed;
+    int64_t  minsc;
+    uint64_t read_off;
+    uint32_t read_len, pad;
+} ht2gpu_sw_job_t;
+typedef struct {
+    uint32_t found, err, toff, n_edits;
+    int64_t  score, best;
+    uint32_t rnd_next, pad;
+} ht2gpu_sw_result_t;
+int ht2gpu_sw_extend(ht2gpu_handle_t* h, uint32_t n, const ht2gpu_sw_job_t* jobs, const uint8_t* seq, const uint8_t* qual,
+                     int warp_fill, ht2gpu_sw_result_t* res, ht2gpu_edit_t* edits);
 /* Diagnostics: the geometry of the handle's alignment kernel.  out[0] = warps per block, out[1] = read slots per
  * lane, out[2] = blocks per SM.  The slots can differ from the options: a default handle on a device without room
  * for the 4-slot workspace, or in a process that already holds the 2-slot one, runs with 2. */

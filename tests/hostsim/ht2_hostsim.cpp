@@ -4,6 +4,7 @@
 // debugged on machines without a GPU.  Not part of the product: the shipped
 // library (libht2gpu.so) has no CPU path and fails loudly without CUDA.
 // usage: ht2_hostsim <index_base> <reads.fa> <out.sam> [--spliced]
+//        ht2_hostsim --sw-extend <index_base> <jobs.txt> [<golden>]   (tools/swjobs.py jobs; see swExtend below)
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
@@ -224,10 +225,14 @@ static int swSelfTest(int n, unsigned seed) {
         P.mmpMax = 2 + rnd(6); P.mmpMin = 1 + rnd(P.mmpMax); P.npen = 1 + rnd(2); P.mmcostConstant = rnd(4) == 0;
         P.rdGapConst = 1 + rnd(8); P.rdGapLinear = 1 + rnd(4); P.rfGapConst = 1 + rnd(8); P.rfGapLinear = 1 + rnd(4);
         P.gapbar = 1 + rnd(12);
-        const uint32_t nrow = 20 + rnd(HT2_SW_MAX_RDLEN - 20), ncol = nrow + 40;
+        // rows 1..256: the first problems take 256 and every 32k +- 1 (the warp fill's row blocks), the rest any length;
+        // a quarter of the rectangles are narrowed by up to 20 columns, as frameSeedExtensionRect trims at a contig end
+        static const uint32_t edgeRows[] = {256, 1, 31, 33, 63, 65, 95, 97, 127, 129, 159, 161, 191, 193, 223, 225, 255};
+        const uint32_t nrow = it < (int)(sizeof(edgeRows) / sizeof(edgeRows[0])) ? edgeRows[it] : 1 + rnd(HT2_SW_MAX_RDLEN);
+        const uint32_t ncol = nrow + 40 - (rnd(4) == 0 ? rnd(21) : 0);
         std::vector<uint8_t> ref(ncol + 8), rd, qu;
         for (auto& c : ref) c = rnd(50) == 0 ? 4 : rnd(4);
-        for (uint32_t j = 20; rd.size() < nrow && j < ncol;) {   // the read: the window with substitutions and small indels
+        for (uint32_t j = ncol - nrow > 20 ? 20 : ncol - nrow; rd.size() < nrow && j < ncol;) {   // the read: the window with substitutions and small indels
             uint32_t r = rnd(100);
             if (r < 3) { rd.push_back((uint8_t)rnd(4)); }                        // insertion in the read
             else if (r < 6) { j++; }                                               // deletion
@@ -289,8 +294,106 @@ static int swSelfTest(int n, unsigned seed) {
     return bad ? 1 : 0;
 }
 
+// --sw-extend INDEX JOBS [GOLDEN]: the --bowtie2-dp seed extension (swExtendAnchor = swPrepare + swFill + swFinish)
+// on the jobs of tools/swjobs.py, one result line per job in the format of oracle/ref_sw plus the error bits:
+//   <id> <found> <off|-> <score|-> <best|-> <rnd.nextU32() after> <edits|-> <err>
+// With GOLDEN (tests/golden/sw_extend_ref.txt), every job's first seven fields must equal the reference's (its best
+// only where it reaches minsc), except for the jobs the device refuses by design: reads over 256 bases and minsc
+// below -15000 (HT2_ERR_SW), alignments of more than HT2_MAX_EDITS edits, and jobs the reference finds nothing for
+// whose rejected candidates ran past the backtrace's HT2_SW_MAX_EDITS edits (HT2_ERR_EDITS).  Prints a summary line; exit 1 on a mismatch.
+static int swExtend(const char* index, const char* jobsPath, const char* goldenPath) {
+    std::string err;
+    Ht2Image* img = ht2_image_load(index, err);
+    if (!img) { fprintf(stderr, "%s\n", err.c_str()); return 1; }
+    FILE* fj = fopen(jobsPath, "r");
+    if (!fj) { fprintf(stderr, "cannot open %s\n", jobsPath); return 1; }
+    std::vector<std::string> golden;
+    if (goldenPath) {
+        FILE* fg = fopen(goldenPath, "r");
+        if (!fg) { fprintf(stderr, "cannot open %s\n", goldenPath); return 1; }
+        char* gl = NULL; size_t gcap = 0;
+        while (getline(&gl, &gcap, fg) > 0) { std::string s(gl); while (!s.empty() && (s.back() == '\n' || s.back() == '\r')) s.pop_back(); golden.push_back(s); }
+        free(gl); fclose(fg);
+        if (!golden.empty()) golden.erase(golden.begin());   // the job stream's sha1
+    }
+    Ht2Params P;
+    ht2_default_params(P, *img, true);
+    P.bowtie2Dp = 2;
+    Ht2Work* W = new Ht2Work();
+    Ht2SwScratch* S = new Ht2SwScratch();
+    uint32_t* pool = new uint32_t[HT2_SW_POOL_WORDS];
+    Ht2AlignerT<false> A;
+    char* line = NULL; size_t cap = 0;
+    size_t n = 0, bad = 0, flagged = 0;
+    std::vector<char> rd(4096), qu(4096);
+    while (getline(&line, &cap, fj) > 0) {
+        long long id, mpMax, mpMin, ignq, np, rdc, rdl, rfc, rfl, gbar, fw, tidx, toff, rdoff, len, minsc; unsigned long long seed;
+        if (sscanf(line, "%lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %lld %llu %4095s %4095s", &id, &mpMax, &mpMin,
+                   &ignq, &np, &rdc, &rdl, &rfc, &rfl, &gbar, &fw, &tidx, &toff, &rdoff, &len, &minsc, &seed, rd.data(), qu.data()) != 19) {
+            fprintf(stderr, "malformed job line: %s", line); return 1;
+        }
+        P.mmpMax = (int)mpMax; P.mmpMin = (int)mpMin; P.mmcostConstant = ignq != 0; P.npen = (int)np;
+        P.rdGapConst = (int)rdc; P.rdGapLinear = (int)rdl; P.rfGapConst = (int)rfc; P.rfGapLinear = (int)rfl; P.gapbar = (int)gbar;
+        Ht2HostRead hr;
+        for (const char* c = rd.data(); *c; c++) hr.seq.push_back((uint8_t)ht2_asc2code((uint8_t)*c));
+        for (const char* c = qu.data(); *c; c++) hr.qual.push_back((uint8_t)*c);
+        memset(W, 0, sizeof(Ht2Work));
+        A.bind(img->blob.data(), &P, W); A.sw = S; A.swPl = pool; A.swStride = 1;
+        A.minsc[0] = minsc; A.minsc[1] = HT2_IDX_MAX32;
+        ht2_fill_read(W->rd[0], hr);
+        W->rnd.init((uint32_t)seed);
+        Ht2Hit gh; memset(&gh, 0, sizeof(gh));
+        Ht2AlignerT<false>::initHit(gh, fw != 0, (uint32_t)rdoff, (uint32_t)len, 0, 0, (uint32_t)tidx, (uint32_t)toff, (uint32_t)toff);
+        const bool found = A.swExtendAnchor(0, gh);
+        const bool dp = (uint32_t)len < W->rd[0].len;
+        char out[8192]; int o = 0;
+        o += snprintf(out + o, sizeof(out) - o, "%lld %d ", id, found ? 1 : 0);
+        if (found && dp) o += snprintf(out + o, sizeof(out) - o, "%u %lld ", gh.toff, (long long)gh.score);
+        else o += snprintf(out + o, sizeof(out) - o, "- - ");
+        if (dp && S->jbest != HT2_MIN_I64 && !W->err) o += snprintf(out + o, sizeof(out) - o, "%lld ", (long long)S->jbest);
+        else o += snprintf(out + o, sizeof(out) - o, "- ");
+        o += snprintf(out + o, sizeof(out) - o, "%u ", W->rnd.nextU32());
+        if (found && dp) {   // the reference inverts a reverse-strand edit list twice (nextAlignment, hybridSearch)
+            for (uint32_t k = 0; k < gh.nedits; k++)
+                o += snprintf(out + o, sizeof(out) - o, "%s%u:%u:%c:%c", k ? "," : "", gh.edits[k].pos, gh.edits[k].type, gh.edits[k].chr, gh.edits[k].qchr);
+        }
+        if (!found || !dp || gh.nedits == 0) o += snprintf(out + o, sizeof(out) - o, "-");
+        snprintf(out + o, sizeof(out) - o, " %u", W->err);
+        printf("%s\n", out);
+        if (W->err) flagged++;
+        if (goldenPath) {
+            if (n >= golden.size()) { fprintf(stderr, "job %lld: no golden line\n", id); bad++; n++; continue; }
+            std::string g = golden[n];
+            {   // the reference's best is the best last-row score even below minsc; the device keeps only a best >= minsc
+                std::vector<std::string> f; size_t a = 0;
+                for (size_t b; (b = g.find(' ', a)) != std::string::npos; a = b + 1) f.push_back(g.substr(a, b - a));
+                f.push_back(g.substr(a));
+                if (f.size() == 7 && f[4] != "-" && atoll(f[4].c_str()) < minsc) { f[4] = "-"; g = f[0]; for (size_t k = 1; k < 7; k++) g += " " + f[k]; }
+            }
+            // expected refusals: reads over the planes' 256 rows, minsc below -15000, more edits than a hit holds
+            size_t gedits = 0; { size_t p = g.rfind(' '); std::string e = g.substr(p + 1); if (e != "-") { gedits = 1; for (char c : e) if (c == ',') gedits++; } }
+            uint32_t want = 0;
+            if (dp && (W->rd[0].len > HT2_SW_MAX_RDLEN || minsc < -15000)) want = HT2_ERR_SW;
+            else if (dp && gedits > HT2_MAX_EDITS) want = HT2_ERR_EDITS;
+            std::string mine(out); mine = mine.substr(0, mine.rfind(' '));
+            // a rejected candidate whose path runs past the backtrace's HT2_SW_MAX_EDITS edits is flagged as well
+            const bool overran = W->err == HT2_ERR_EDITS && !want && g.compare(0, g.find(' ') + 2, std::to_string(id) + " 0") == 0;
+            if (!overran && (W->err != want || (!want && mine != g))) {
+                fprintf(stderr, "job %lld differs (err %u, expected %u)\n  host:      %s\n  reference: %s\n", id, W->err, want, mine.c_str(), g.c_str());
+                bad++;
+            }
+        }
+        n++;
+    }
+    free(line); fclose(fj);
+    if (goldenPath && n != golden.size()) { fprintf(stderr, "%zu jobs, %zu golden lines\n", n, golden.size()); bad++; }
+    fprintf(stderr, "sw extend: %zu jobs, %zu flagged, %zu mismatches\n", n, flagged, bad);
+    return bad ? 1 : 0;
+}
+
 int main(int argc, char** argv) {
     if (argc >= 3 && !strcmp(argv[1], "--sw-selftest")) return swSelfTest(atoi(argv[2]), argc > 3 ? (unsigned)atoi(argv[3]) : 1u);
+    if (argc >= 4 && !strcmp(argv[1], "--sw-extend")) return swExtend(argv[2], argv[3], argc > 4 ? argv[4] : NULL);
     if (argc >= 5 && !strcmp(argv[1], "--seed-dump")) {
         std::string err;
         Ht2Image* img = ht2_image_load(argv[2], err);

@@ -258,7 +258,8 @@ def test_spliced_corpus_is_deterministic(tmp_path):
 def test_striped_dp_fill_and_backtrace_against_plain_scalar_dp(hostsim_bin):
     """The --bowtie2-dp kernel on its own (ht2_sw.h: striped s16x2 fill with the DPX-style max(a+b,c) steps +
     plane-derived backtrace) against an independent scalar statement of the recurrences: 400 random problems
-    (read lengths 20-255, random penalties / gap barriers / qualities / Ns): every last-row score equal, and
+    (read lengths 1-256 with 256 and every 32k +- 1, rectangles narrowed as at contig ends, random penalties / gap
+    barriers / qualities / Ns): every last-row score equal, and
     the returned edits turn the read into the reference window at exactly the optimal score."""
     r = subprocess.run([hostsim_bin, "--sw-selftest", "400", "3"], check=True, stdout=subprocess.PIPE, stderr=subprocess.PIPE)
     out = r.stdout.decode()

@@ -296,8 +296,8 @@ def test_bundled_graph_index_matches_reference_binary_run_here(h2, sets, name, p
 
 def test_warp_wide_dp_fill_equals_lane_fill_cell_by_cell(h2):
     """ht2_sw.h: the DP rounds of the pool kernel fill the score planes with a whole warp per problem (64 rows per
-    vector, lazy-F across lanes by shuffle).  On 3000 random problems (20..256 rows, random penalties, gap
-    barriers, N's, indels) every H, E and F cell, every last-row score and the best score must equal the lane
+    vector, lazy-F across lanes by shuffle).  On 3000 random problems (1..256 rows with 256 and every 32k +- 1,
+    rectangles narrowed as at contig ends, random penalties, gap barriers, N's, indels) every H, E and F cell, every last-row score and the best score must equal the lane
     fill's, which the host self-test pins to a plain scalar statement of the recurrences (test_cpu.py)."""
     from hisat2_b200 import api
     r = api.sw_selftest(3000, seed=5)
