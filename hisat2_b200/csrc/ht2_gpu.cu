@@ -596,8 +596,8 @@ ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigne
     if (u < units) {
         const unsigned long long at = base + incl - mine;   // in the block
         Ht2SamOut<true> o; o.n = 0;
-        if (staged) { o.p = stage + head + at; F.unit(o, u); }
-        else if (b0 + at + mine <= cap) { o.p = out + b0 + at; F.unit(o, u); }
+        o.p = staged ? stage + head + at : out + b0 + at;
+        if (staged || b0 + at + mine <= cap) F.unit(o, u);   // one call site: the formatter is inlined once
     }
     if (!staged) return;
     __syncthreads();

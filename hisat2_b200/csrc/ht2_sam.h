@@ -58,35 +58,132 @@ enum { HT2_T_NREAD, HT2_T_NPAIRED, HT2_T_NUNPAIRED, HT2_T_NCONCORD_0, HT2_T_NCON
 struct Ht2SamTally { uint32_t c[HT2_T_N]; };
 static_assert(sizeof(ht2gpu_align_counts_t) == HT2_T_N * sizeof(uint64_t), "ht2gpu_align_counts_t follows the tally's order");
 
+// Where a pass's text goes: p + n (WRITE) or only the byte count n (the counting pass).  Ht2SamFmt::unit formats
+// one unit through an Ht2SamCur and adds its length to n.
 template <bool WRITE>
 struct Ht2SamOut {
     char*    p;
     uint64_t n;
-    HT2_HD void c(char ch) { if (WRITE) p[n] = ch; n++; }
-    HT2_HD void s(const char* lit) { while (*lit) { c(*lit); lit++; } }
-    HT2_HD void i64(int64_t v) {
-        uint64_t u = v < 0 ? (uint64_t)0 - (uint64_t)v : (uint64_t)v;
-        if (!WRITE) {   // the counting pass: the number of digits only
-            uint32_t k = 1;
-            for (uint64_t p = 10; k < 20 && u >= p; p *= 10) k++;
-            n += k + (v < 0);
-            return;
-        }
-        char buf[24]; int k = 0;
-        do { buf[k++] = (char)('0' + u % 10); u /= 10; } while (u);
-        if (v < 0) c('-');
-        while (k) c(buf[--k]);
+};
+
+HT2_HD bool ht2_sam_isspace(char ch) { return ch == ' ' || (ch >= 9 && ch <= 13); }
+
+// The emission helpers below are called from dozens of fields.  Each is one out-of-line leaf that takes the
+// destination by value and returns the bytes it wrote (or would write, WRITE = false), so a caller's cursor stays
+// in registers and no helper is copied into every call site.
+
+// v in decimal: the digits are counted first and then stored from the last one backwards, in place.
+template <bool WRITE> HT2_NI uint32_t ht2_sam_i64(char* d, int64_t v) {
+    uint64_t u = v < 0 ? (uint64_t)0 - (uint64_t)v : (uint64_t)v;
+    uint32_t k = 1;
+    if (u >> 32) { for (uint64_t q = u; q >= 10; q /= 10) k++; }
+    else { for (uint32_t q = (uint32_t)u; q >= 10; q /= 10) k++; }
+    const uint32_t len = k + (v < 0);
+    if (WRITE) {
+        char* e = d + len;
+        for (; u >> 32; u /= 10) *--e = (char)('0' + u % 10);
+        uint32_t w = (uint32_t)u;
+        do { *--e = (char)('0' + w % 10); w /= 10; } while (w);
+        if (v < 0) *d = '-';
     }
-    // cnt bytes, byte i = byteAt(i), 4 to a store once the destination is 4-byte aligned (SEQ / QUAL)
-    template <typename F> HT2_HD void run(uint32_t cnt, F byteAt) {
+    return len;
+}
+
+#ifdef __CUDA_ARCH__
+// the 4 bytes at p, from the two aligned words that hold them (p need not be aligned; neither word is read past
+// the one that holds p[3])
+__device__ __forceinline__ uint32_t ht2_sam_ld4(const char* p) {
+    const uintptr_t a = (uintptr_t)p;
+    const uint32_t sh = (uint32_t)(a & 3) * 8;
+    const uint32_t* w = (const uint32_t*)(a & ~(uintptr_t)3);
+    return sh ? __funnelshift_r(w[0], w[1], sh) : w[0];
+}
+#endif
+
+// Length of s up to its first '\0' or white space; atEnd = it stopped at the '\0'.  The device reads aligned words
+// (no word past the one holding the stop byte, so nothing outside the string's allocation granule).
+HT2_HD uint32_t ht2_sam_token(const char* s, bool& atEnd) {
+#ifdef __CUDA_ARCH__
+    const uintptr_t a = (uintptr_t)s;
+    const uint32_t* w = (const uint32_t*)(a & ~(uintptr_t)3);
+    const uint32_t head = (uint32_t)(a & 3);
+    const uint32_t before = (1u << (8 * head)) - 1u;        // bytes ahead of s read as 'A'
+    uint32_t x = (w[0] & ~before) | (0x41414141u & before);
+    for (uint32_t k = 0;; k += 4) {
+        const uint32_t z = __vcmpeq4(x, 0u);
+        const uint32_t st = z | __vcmpeq4(x, 0x20202020u) | (__vcmpgeu4(x, 0x09090909u) & __vcmpleu4(x, 0x0d0d0d0du));
+        if (st) {
+            const uint32_t b = (uint32_t)(__ffs(st) - 1) >> 3;
+            atEnd = (z >> (8 * b)) & 1u;
+            return k + b - head;
+        }
+        x = w[(k >> 2) + 1];
+    }
+#else
+    uint32_t i = 0;
+    while (s[i] && !ht2_sam_isspace(s[i])) i++;
+    atEnd = !s[i];
+    return i;
+#endif
+}
+
+// len bytes of s (all of them before its terminator); 4 to a store once the destination is aligned on the device
+HT2_HD void ht2_sam_copy(char* d, const char* s, uint32_t len) {
+    uint32_t i = 0;
+#ifdef __CUDA_ARCH__
+    for (; i < len && ((uintptr_t)(d + i) & 3); i++) d[i] = s[i];
+    for (; i + 4 <= len; i += 4) *(uint32_t*)(d + i) = ht2_sam_ld4(s + i);
+#endif
+    for (; i < len; i++) d[i] = s[i];
+}
+
+// A read or reference name up to its first white space, at most cap bytes; with omitSlashMate a trailing /1, /2
+// or /3 of the whole name is dropped.  White space cannot come after the '/'
+// of such a suffix, so the suffix only matters when the name ends at its terminator.
+template <bool WRITE> HT2_NI uint32_t ht2_sam_name(char* d, const char* name, bool omitSlashMate, uint32_t cap) {
+    bool atEnd;
+    uint32_t len = ht2_sam_token(name, atEnd);
+    if (atEnd && omitSlashMate && len >= 2 && name[len - 2] == '/' &&
+        (name[len - 1] == '1' || name[len - 1] == '2' || name[len - 1] == '3')) len -= 2;
+    if (len > cap) len = cap;
+    if (WRITE) ht2_sam_copy(d, name, len);
+    return len;
+}
+
+// a '\0'-terminated string of the run (read group, ALT names)
+template <bool WRITE> HT2_NI uint32_t ht2_sam_str(char* d, const char* z) {
+    uint32_t i = 0;
+    for (; z[i]; i++) if (WRITE) d[i] = z[i];
+    return i;
+}
+
+// One unit's text: d + [0, n), a 32-bit offset from the unit's first byte.
+template <bool WRITE>
+struct Ht2SamCur {
+    char*    d;
+    uint32_t n;
+    HT2_HD char* at() const { return WRITE ? d + n : NULL; }
+    HT2_HD void c(char ch) { if (WRITE) d[n] = ch; n++; }
+    // a literal: its length is known at compile time, its bytes are immediates at fixed offsets from one address
+    template <uint32_t N> HT2_HD void s(const char (&lit)[N]) {
         if (WRITE) {
-            char* d = p + n;
+            char* q = d + n;
+#pragma unroll
+            for (uint32_t i = 0; i + 1 < N; i++) q[i] = lit[i];
+        }
+        n += N - 1;
+    }
+    HT2_HD void str(const char* z) { n += ht2_sam_str<WRITE>(at(), z); }
+    HT2_HD void i64(int64_t v) { n += ht2_sam_i64<WRITE>(at(), v); }
+    HT2_HD void name(const char* z, bool omitSlashMate, uint32_t cap) { n += ht2_sam_name<WRITE>(at(), z, omitSlashMate, cap); }
+    // cnt bytes, byte i = byteAt(i); once the destination is 4-byte aligned, bytes i..i+3 = word4(i), one store (SEQ / QUAL)
+    template <typename F, typename G> HT2_HD void run(uint32_t cnt, F byteAt, G word4) {
+        if (WRITE) {
+            char* q = d + n;
             uint32_t i = 0;
-            for (; i < cnt && ((uintptr_t)(d + i) & 3); i++) d[i] = byteAt(i);
-            for (; i + 4 <= cnt; i += 4)
-                *(uint32_t*)(d + i) = (uint32_t)(uint8_t)byteAt(i) | ((uint32_t)(uint8_t)byteAt(i + 1) << 8) |
-                                      ((uint32_t)(uint8_t)byteAt(i + 2) << 16) | ((uint32_t)(uint8_t)byteAt(i + 3) << 24);
-            for (; i < cnt; i++) d[i] = byteAt(i);
+            for (; i < cnt && ((uintptr_t)(q + i) & 3); i++) q[i] = byteAt(i);
+            for (; i + 4 <= cnt; i += 4) *(uint32_t*)(q + i) = word4(i);
+            for (; i < cnt; i++) q[i] = byteAt(i);
         }
         n += cnt;
     }
@@ -131,8 +228,6 @@ struct Ht2SamRead {
     uint8_t lenfilt, nfilt, scfilt;    // 1 = passes (hisat2.cpp:3417-3440)
 };
 
-HT2_HD bool ht2_sam_isspace(char ch) { return ch == ' ' || (ch >= 9 && ch <= 13); }
-
 struct Ht2SamFmt {
     const Ht2SamIn* in;
     const Ht2ImageHeader* IH;
@@ -162,7 +257,21 @@ struct Ht2SamFmt {
         int64_t m = minscOf(rd.len); if (m > 0) m = 0;
         const uint32_t maxns = (uint32_t)((double)0.0f + (double)0.15f * (double)rd.len);
         uint32_t ns = 0;
+#ifdef __CUDA_ARCH__
+        {   // base codes are 0..4, so bit 2 marks an N; aligned words, bytes outside the read masked off
+            const uintptr_t a = (uintptr_t)rd.seq;
+            const uint32_t* w = (const uint32_t*)(a & ~(uintptr_t)3);
+            const uint32_t head = (uint32_t)(a & 3), end = head + rd.len;
+            for (uint32_t k = 0; k < end; k += 4) {
+                uint32_t m = 0x04040404u;
+                if (k == 0) m &= ~((1u << (8 * head)) - 1u);
+                if (k + 4 > end) m &= (1u << (8 * (end - k))) - 1u;
+                ns += (uint32_t)__popc(w[k >> 2] & m);
+            }
+        }
+#else
         for (uint32_t k = 0; k < rd.len; k++) ns += (rd.seq[k] == 4);
+#endif
         rd.nfilt = ns <= maxns; rd.scfilt = (0 >= m); rd.lenfilt = rd.len >= 2;
     }
 
@@ -222,8 +331,15 @@ struct Ht2SamFmt {
     // AlnSinkWrap::selectByScore (aln_sink.h:2680-2755).  rs1 (+ rs2 and pairs for concordant pairs); writes the
     // selected element indexes to sel[] and returns their number.  The sort key is (score key, index), both
     // descending -- std::sort + reverse of pair<key, index> in the reference's restatement -- so the order is total.
+    // One candidate (nearly every read) is selected as it is, without the sort arrays; no shuffle draws from rnd
+    // either way, as a run of equal keys needs two candidates.
     HT2_HD uint32_t selectByScore(const ht2gpu_aln_t* rs1, uint32_t n1, uint32_t len1, const ht2gpu_aln_t* rs2, uint32_t len2,
                                   const uint16_t* pairs, uint32_t npairs, bool usePairs, uint64_t num, uint16_t* sel, Ht2Rng& rnd) const {
+        if ((usePairs ? npairs : n1) == 1 && num > 0) { sel[0] = 0; return 1; }
+        return selectMany(rs1, n1, len1, rs2, len2, pairs, npairs, usePairs, num, sel, rnd);
+    }
+    HT2_NI uint32_t selectMany(const ht2gpu_aln_t* rs1, uint32_t n1, uint32_t len1, const ht2gpu_aln_t* rs2, uint32_t len2,
+                               const uint16_t* pairs, uint32_t npairs, bool usePairs, uint64_t num, uint16_t* sel, Ht2Rng& rnd) const {
         uint32_t sz = usePairs ? npairs : n1;
         if (sz > HT2_SAM_MAXSEL) sz = HT2_SAM_MAXSEL;   // cannot happen: the kernel's per-read capacities are smaller
         if (sz < num) num = sz;
@@ -359,43 +475,63 @@ struct Ht2SamFmt {
         return fraglen;
     }
 
-    template <bool W> HT2_HD void putName(Ht2SamOut<W>& o, const char* name, bool omitSlashMate) const {
-        uint32_t namelen = 0;
-        while (name[namelen]) namelen++;
-        if (omitSlashMate && namelen >= 2 && name[namelen - 2] == '/' &&
-            (name[namelen - 1] == '1' || name[namelen - 1] == '2' || name[namelen - 1] == '3')) namelen -= 2;
-        if (namelen > 255) namelen = 255;
-        for (uint32_t i = 0; i < namelen; i++) { if (ht2_sam_isspace(name[i])) return; o.c(name[i]); }
-    }
-    template <bool W> HT2_HD void putRefName(Ht2SamOut<W>& o, uint32_t tidx) const {
-        for (const char* c = refName(tidx); *c && !ht2_sam_isspace(*c); c++) o.c(*c);
-    }
-    template <bool W> HT2_HD void putSeqQual(Ht2SamOut<W>& o, const Ht2SamRead& rd, bool fw) const {
+    template <bool W> HT2_HD void putRefName(Ht2SamCur<W>& o, uint32_t tidx) const { o.name(refName(tidx), false, 0xffffffffu); }
+    template <bool W> HT2_HD void putSeqQual(Ht2SamCur<W>& o, const Ht2SamRead& rd, bool fw) const {
         const uint32_t n = rd.len;
         if (n == 0) { o.s("*\t*"); return; }   // aln_sink.h:3194, 3210
         const uint8_t* sq = rd.seq; const uint8_t* ql = rd.qual;
-        if (fw) o.run(n, [&](uint32_t i) { return "ACGTN"[sq[i]]; });
-        else o.run(n, [&](uint32_t i) { const uint8_t c = sq[n - i - 1]; return "TGCAN"[c < 4 ? c : 4]; });
+        auto fwBase = [&](uint32_t i) { return "ACGTN"[sq[i]]; };
+        auto rcBase = [&](uint32_t i) { const uint8_t c = sq[n - i - 1]; return "TGCAN"[c < 4 ? c : 4]; };
+        auto fwQual = [&](uint32_t i) { return (char)ql[i]; };
+        auto rcQual = [&](uint32_t i) { return (char)ql[n - i - 1]; };
+#ifdef __CUDA_ARCH__
+        // four bytes per step: aligned word loads of the read, base codes (0..4) to letters with one byte permute
+        // (selector nibble = code; byte 4 of the pair is 'N'), the reverse strand's order by one more permute
+        auto letters = [](uint32_t codes, uint32_t table) {
+            const uint32_t y = codes | (codes >> 4);
+            return __byte_perm(table, 0x4Eu, __byte_perm(y, 0, 0x0020));
+        };
+        const char* sc = (const char*)sq; const char* qc = (const char*)ql;
+        auto fwBase4 = [&](uint32_t i) { return letters(ht2_sam_ld4(sc + i), 0x54474341u); };                          // "ACGT"
+        auto rcBase4 = [&](uint32_t i) { return letters(__byte_perm(ht2_sam_ld4(sc + n - i - 4), 0, 0x0123), 0x41434754u); };   // "TGCA"
+        auto fwQual4 = [&](uint32_t i) { return ht2_sam_ld4(qc + i); };
+        auto rcQual4 = [&](uint32_t i) { return __byte_perm(ht2_sam_ld4(qc + n - i - 4), 0, 0x0123); };
+#else
+        auto word = [](auto byteAt, uint32_t i) {
+            return (uint32_t)(uint8_t)byteAt(i) | ((uint32_t)(uint8_t)byteAt(i + 1) << 8) |
+                   ((uint32_t)(uint8_t)byteAt(i + 2) << 16) | ((uint32_t)(uint8_t)byteAt(i + 3) << 24);
+        };
+        auto fwBase4 = [&](uint32_t i) { return word(fwBase, i); };
+        auto rcBase4 = [&](uint32_t i) { return word(rcBase, i); };
+        auto fwQual4 = [&](uint32_t i) { return word(fwQual, i); };
+        auto rcQual4 = [&](uint32_t i) { return word(rcQual, i); };
+#endif
+        if (fw) o.run(n, fwBase, fwBase4);
+        else o.run(n, rcBase, rcBase4);
         o.c('\t');
-        if (!ql) o.run(n, [&](uint32_t) { return 'I'; });
-        else if (fw) o.run(n, [&](uint32_t i) { return (char)ql[i]; });
-        else o.run(n, [&](uint32_t i) { return (char)ql[n - i - 1]; });
+        if (!ql) o.run(n, [&](uint32_t) { return 'I'; }, [&](uint32_t) { return 0x49494949u; });
+        else if (fw) o.run(n, fwQual, fwQual4);
+        else o.run(n, rcQual, rcQual4);
     }
-    template <bool W> HT2_HD void putYF(Ht2SamOut<W>& o, const Ht2SamRead& rd) const {
+    template <bool W> HT2_HD void putYF(Ht2SamCur<W>& o, const Ht2SamRead& rd) const {
         if (!rd.lenfilt) o.s("\tYF:Z:LN");
         else if (!rd.nfilt) o.s("\tYF:Z:NS");
         else if (!rd.scfilt) o.s("\tYF:Z:SC");
     }
     // the read group follows YT:Z / YF:Z and precedes XS:A / NH:i (sam.h:780, 1102)
-    template <bool W> HT2_HD void putRG(Ht2SamOut<W>& o) const {
-        if (in->rgTag) { o.c('\t'); o.s(in->rgTag); }
+    template <bool W> HT2_HD void putRG(Ht2SamCur<W>& o) const {
+        if (in->rgTag) { o.c('\t'); o.str(in->rgTag); }
+    }
+    template <bool W> HT2_HD void putYT(Ht2SamCur<W>& o, const Ht2SamFlags& fl) const {
+        o.s("\tYT:Z:");
+        if (fl.concordant()) o.s("CP"); else if (fl.discordant()) o.s("DP"); else if (fl.unpairedMate()) o.s("UP"); else o.s("UU");
     }
 
     // SpliceSiteDB::addSpliceSite (splice_site.cpp:190-350) for one printed alignment: every junction whose anchors
     // are long enough (15 bases + 2 per mismatch / gap on its side, + 6 without a canonical motif) is recorded with the
     // alignment's edit distance.  Alignments with soft-trimmed ends are skipped.  (The threshold of a junction that is
     // followed by another one uses the NEXT junction's direction and the mismatches seen so far -- as the reference.)
-    HT2_HD void collectSites(const ht2gpu_aln_t* rs, uint32_t rdlen) const {
+    HT2_NI void collectSites(const ht2gpu_aln_t* rs, uint32_t rdlen) const {
         if (rs->trim5 + rs->trim3 > 0) return;
         const ht2gpu_edit_t* ed = in->edits + rs->edit_off;
         const uint32_t ned = rs->n_edits;
@@ -458,56 +594,26 @@ struct Ht2SamFmt {
         }
     }
 
-    // AlnSinkSam::appendMate (aln_sink.h:3024-3250)
+    // StackedAln of a gapped alignment (StackedAln::init / leftAlign, aligner_result.cpp:660-790), built in this
+    // frame, then its CIGAR (mdz = false: StackedAln::buildCigar, aligner_result.cpp:793-850) or its MD:Z string
+    // (mdz = true: StackedAln::buildMdz, aligner_result.cpp:852-1000).  Out of line so that the column arrays are no
+    // part of the gapless path's frame; a gapped record builds its stack twice.
     template <bool W>
-    HT2_NI void appendMate(Ht2SamOut<W>& o, const Ht2SamRead& rd, uint32_t ordlen, const ht2gpu_aln_t* rs, const ht2gpu_aln_t* rso,
-                           const Ht2SamSumm& summ, const Ht2SamFlags& fl, bool fraglenSet, int64_t fraglen, bool haveOscore) const {
-        if (rs == NULL && in->noUnal) return;
-        putName(o, rd.name, fl.partOfPair());
-        o.c('\t');
-        int flag = 0;
-        if (fl.partOfPair()) {
-            flag |= 1;
-            if (fl.concordant()) flag |= 2;
-            if (!fl.oppAligned) flag |= 8;
-            flag |= fl.readMate1() ? 64 : 128;
-            if (fl.oppAligned && rso != NULL && !rso->fw) flag |= 32;
-        }
-        if (!fl.primary) flag |= 256;
-        if (rs != NULL && !rs->fw) flag |= 16;
-        if (rs == NULL) flag |= 4;
-        o.i64(flag);
-        o.c('\t');
-        const char* ytz = fl.concordant() ? "CP" : fl.discordant() ? "DP" : fl.unpairedMate() ? "UP" : "UU";
-        if (rs == NULL) {
-            if (summ.orefid != -1) { putRefName(o, (uint32_t)summ.orefid); o.c('\t'); o.i64(summ.orefoff + 1); o.s("\t0\t*\t=\t"); o.i64(summ.orefoff + 1); o.s("\t0\t"); }
-            else o.s("*\t0\t0\t*\t*\t0\t0\t");
-            putSeqQual(o, rd, true);
-            o.s("\tYT:Z:"); o.s(ytz);
-            putYF(o, rd);
-            putRG(o);
-            o.c('\n');
-            return;
-        }
-        if (W && in->colCount != NULL) collectSites(rs, rd.len);   // AlnSinkSam::append (aln_sink.h:1571, 1579)
+    HT2_NI uint32_t putStacked(char* d, const uint8_t* seq, uint32_t rdlen, const ht2gpu_aln_t* rs, bool mdz) const {
+        Ht2SamCur<W> o = {d, 0};
         const ht2gpu_edit_t* ed = in->edits + rs->edit_off;
         const uint32_t ned = rs->n_edits;
-        // Gapless alignments (mismatches only; the vast majority): CIGAR and MD:Z follow from the edit positions
-        // directly -- what StackedAln::buildCigar / buildMdz (aligner_result.cpp:793-1000) print for a stack
-        // without I/D columns, with nothing for leftAlign to move.  Everything else goes through the stacked form.
-        bool gapless = true;
-        for (uint32_t i = 0; i < ned; i++) if (ed[i].type != HT2_EDIT_MM) { gapless = false; break; }
         uint32_t trimLS = rs->trim5, trimRS = rs->trim3;
-        const uint32_t len_trimmed = rd.len - trimLS - trimRS;
+        const uint32_t len_trimmed = rdlen - trimLS - trimRS;
         if (!rs->fw) { const uint32_t t = trimLS; trimLS = trimRS; trimRS = t; }
-        // stacked alignment (StackedAln::init, aligner_result.cpp:660-790): columns of (ref, rel, read, snp)
+        // columns of (ref, rel, read, snp)
         char stRef[HT2_SAM_MAXCOLS], stRel[HT2_SAM_MAXCOLS], stRead[HT2_SAM_MAXCOLS];
         uint8_t stSnp[HT2_SAM_MAXCOLS];
         uint32_t ln = 0;
-        if (!gapless) {
+        {
             // AlnRes::initStacked (aligner_result.h:1856-1873): edits and read in reference-forward orientation
             uint32_t rdoff = trimLS;
-            auto rdc = [&](uint32_t i) -> int { if (rs->fw) return rd.seq[i]; const uint8_t c = rd.seq[rd.len - i - 1]; return c < 4 ? (c ^ 3) : 4; };
+            auto rdc = [&](uint32_t i) -> int { if (rs->fw) return seq[i]; const uint8_t c = seq[rdlen - i - 1]; return c < 4 ? (c ^ 3) : 4; };
             for (uint32_t k = 0; k < ned && ln + 2 < HT2_SAM_MAXCOLS; k++) {
                 const ht2gpu_edit_t& e = rs->fw ? ed[k] : ed[ned - 1 - k];
                 uint32_t epos = e.pos;
@@ -520,7 +626,7 @@ struct Ht2SamFmt {
                 else if (e.type == HT2_EDIT_READ_GAP) { stRef[ln] = (char)e.chr; stRel[ln] = 'D'; stSnp[ln] = isSnp; stRead[ln] = '-'; ln++; }
                 else if (e.type == HT2_EDIT_SPL) { stRef[ln] = 'N'; stRel[ln] = 'N'; stSnp[ln] = 0; stRead[ln] = 'N'; ln++; }   // aligner_result.cpp:711-718
             }
-            while (rdoff < rd.len - trimRS && ln + 1 < HT2_SAM_MAXCOLS) { const int c = rdc(rdoff++); stRef[ln] = "ACGTN"[c]; stRel[ln] = '='; stSnp[ln] = 0; stRead[ln] = "ACGTN"[c]; ln++; }
+            while (rdoff < rdlen - trimRS && ln + 1 < HT2_SAM_MAXCOLS) { const int c = rdc(rdoff++); stRef[ln] = "ACGTN"[c]; stRel[ln] = '='; stSnp[ln] = 0; stRead[ln] = "ACGTN"[c]; ln++; }
             // StackedAln::leftAlign(false) (aligner_result.cpp:727-790)
             for (uint32_t i = 0; i < ln; i++) {
                 const char r = stRel[i];
@@ -543,17 +649,7 @@ struct Ht2SamFmt {
                 }
             }
         }
-        putRefName(o, rs->tidx);
-        o.c('\t');
-        o.i64((int64_t)rs->toff + 1);
-        o.c('\t');
-        o.i64(mapqV2(summ, rd.mate < 2, rd.len, ordlen));
-        o.c('\t');
-        if (gapless) {
-            if (trimLS > 0) { o.i64(trimLS); o.c('S'); }
-            if (len_trimmed > 0) { o.i64(len_trimmed); o.c('M'); }
-            if (trimRS > 0) { o.i64(trimRS); o.c('S'); }
-        } else {   // StackedAln::buildCigar (aligner_result.cpp:793-850)
+        if (!mdz) {
             if (trimLS > 0) { o.i64(trimLS); o.c('S'); }
             uint32_t numSkips = 0;
             for (uint32_t i = 0; i < ln; i++) {
@@ -580,53 +676,7 @@ struct Ht2SamFmt {
                 o.i64((int64_t)run); o.c(op);
             }
             if (trimRS > 0) { o.i64(trimRS); o.c('S'); }
-        }
-        o.c('\t');
-        if (fl.partOfPair()) {
-            if (rso != NULL && rs->tidx != rso->tidx) { putRefName(o, rso->tidx); o.c('\t'); }
-            else o.s("=\t");
-            o.i64((int64_t)(rso ? rso->toff : rs->toff) + 1);
-            o.c('\t');
-        } else o.s("*\t0\t");
-        o.i64(fraglenSet ? fraglen : 0);
-        o.c('\t');
-        if (!fl.primary && in->omitSecSeq) o.s("*\t*");
-        else putSeqQual(o, rd, rs->fw != 0);
-        // optional flags (sam.h:525-1010)
-        o.s("\tAS:i:"); o.i64(rs->score);
-        const Ht2SamKey& sb = summ.secbest[rd.mate < 2 ? 0 : 1];
-        if (sb.valid) { o.s("\tZS:i:"); o.i64(sb.score); }
-        o.s("\tXN:i:0");
-        // counts exclude edits that are known ALTs (snpID < #alts, sam.h:574-647)
-        uint32_t num_mm = 0, num_go = 0, num_gx = 0, NM = 0;
-        for (uint32_t i = 0; i < ned; i++) if (ed[i].type != HT2_EDIT_SPL && ed[i].snp_id >= nAlts) NM++;
-        for (uint32_t i = 0; i < ned; i++) {
-            const ht2gpu_edit_t& e = ed[i];
-            if (e.type == HT2_EDIT_MM) { if (e.snp_id >= nAlts) num_mm++; }
-            else if (e.type == HT2_EDIT_READ_GAP) {
-                if (e.snp_id >= nAlts) { num_go++; num_gx++; }
-                while (i + 1 < ned && ed[i + 1].pos == ed[i].pos && ed[i + 1].type == HT2_EDIT_READ_GAP) { i++; if (ed[i].snp_id >= nAlts) num_gx++; }
-            } else if (e.type == HT2_EDIT_REF_GAP) {
-                if (e.snp_id >= nAlts) { num_go++; num_gx++; }
-                while (i + 1 < ned && ed[i + 1].pos == ed[i].pos + 1 && ed[i + 1].type == HT2_EDIT_REF_GAP) { i++; if (ed[i].snp_id >= nAlts) num_gx++; }
-            }
-        }
-        o.s("\tXM:i:"); o.i64(num_mm);
-        o.s("\tXO:i:"); o.i64(num_go);
-        o.s("\tXG:i:"); o.i64(num_gx);
-        o.s("\tNM:i:"); o.i64(NM);
-        o.s("\tMD:Z:");
-        if (gapless) {   // <matches>[<ref char><matches>]..., a 0 between adjacent mismatches and at either end
-            uint32_t prevEnd = 0;
-            for (uint32_t k = 0; k < ned; k++) {
-                const ht2gpu_edit_t& e = rs->fw ? ed[k] : ed[ned - 1 - k];
-                const uint32_t p = rs->fw ? e.pos : len_trimmed - e.pos - 1;
-                o.i64((int64_t)(p - prevEnd));
-                o.c((char)e.chr);
-                prevEnd = p + 1;
-            }
-            o.i64((int64_t)(len_trimmed - prevEnd));
-        } else {   // StackedAln::buildMdz (aligner_result.cpp:852-1000)
+        } else {
             bool mm_last = false, rdgap_last = false, first_print = true;
             for (uint32_t i = 0; i < ln; i++) {
                 const char op = stRel[i];
@@ -653,73 +703,202 @@ struct Ht2SamFmt {
             }
             if (mm_last || rdgap_last) o.c('0');
         }
+        return o.n;
+    }
+
+    // the fields of an unaligned record after FLAG
+    template <bool W>
+    HT2_NI uint32_t putUnaligned(char* d, const Ht2SamRead& rd, const Ht2SamSumm& summ, const Ht2SamFlags& fl) const {
+        Ht2SamCur<W> o = {d, 0};
+        if (summ.orefid != -1) { putRefName(o, (uint32_t)summ.orefid); o.c('\t'); o.i64(summ.orefoff + 1); o.s("\t0\t*\t=\t"); o.i64(summ.orefoff + 1); o.s("\t0\t"); }
+        else o.s("*\t0\t0\t*\t*\t0\t0\t");
+        putSeqQual(o, rd, true);
+        putYT(o, fl);
+        putYF(o, rd);
+        putRG(o);
+        o.c('\n');
+        return o.n;
+    }
+
+#ifdef HT2_ENABLE_SPLICED
+    // XS:A of a spliced alignment: AlnRes::spliced_whichsense_transcript (aligner_result.h:1288-1318, sam.h:925-937);
+    // '+', '-' or 0 for none
+    HT2_NI char xsSense(const ht2gpu_edit_t* ed, uint32_t ned) const {
+        uint32_t whichsense = HT2_SPL_UNKNOWN;
+        for (uint32_t i = 0; i < ned; i++) {
+            if (ed[i].type != HT2_EDIT_SPL) continue;
+            const uint32_t d = ht2_spl_dir(*(const Ht2Edit*)&ed[i]);
+            if (whichsense == HT2_SPL_UNKNOWN) whichsense = d;
+            else if (d != HT2_SPL_UNKNOWN) {
+                if ((whichsense == HT2_SPL_FW || whichsense == HT2_SPL_SEMI_FW) && d != HT2_SPL_FW && d != HT2_SPL_SEMI_FW) return 0;
+                if ((whichsense == HT2_SPL_RC || whichsense == HT2_SPL_SEMI_RC) && d != HT2_SPL_RC && d != HT2_SPL_SEMI_RC) return 0;
+            }
+        }
+        if (whichsense == HT2_SPL_UNKNOWN) return 0;
+        return (whichsense == HT2_SPL_FW || whichsense == HT2_SPL_SEMI_FW) ? '+' : '-';
+    }
+#endif
+
+    // Zs:Z: the known ALTs the alignment went through (sam.h:983-1032); edits in reference-forward order
+    template <bool W>
+    HT2_NI uint32_t putZs(char* d, const ht2gpu_aln_t* rs, uint32_t len_trimmed) const {
+        Ht2SamCur<W> o = {d, 0};
+        const ht2gpu_edit_t* ed = in->edits + rs->edit_off;
+        const uint32_t ned = rs->n_edits;
+        auto nedAt = [&](uint32_t i, uint32_t& pos) -> const ht2gpu_edit_t& {   // Edit::invertPoss (edit.cpp:70-111), sort = false
+            const ht2gpu_edit_t& e = rs->fw ? ed[i] : ed[ned - 1 - i];
+            pos = e.pos;
+            if (!rs->fw) pos = (e.type == HT2_EDIT_READ_GAP || e.type == HT2_EDIT_SPL) ? len_trimmed - e.pos : len_trimmed - e.pos - 1;
+            return e;
+        };
+        bool first = true;
+        uint32_t prev = 0xffffffffu;
+        for (uint32_t i = 0; i < ned; i++) {
+            uint32_t epos;
+            const ht2gpu_edit_t& e = nedAt(i, epos);
+            if (e.type == HT2_EDIT_SPL || e.snp_id >= nAlts) continue;   // a splice edit keeps its site probability in the snpID word
+            const uint32_t si = e.snp_id;
+            const Ht2Alt& snp = altTab[si];
+            if (si == prev) continue;
+            if (first) o.s("\tZs:Z:"); else o.c(',');
+            uint64_t pos = epos;
+            uint32_t j = i;
+            while (j > 0) {
+                uint32_t ppos;
+                const ht2gpu_edit_t& pe = nedAt(j - 1, ppos);
+                if (pe.snp_id < nAlts) {
+                    const Ht2Alt& snp2 = altTab[pe.snp_id];
+                    if (snp2.type == HT2_ALT_SNP_SGL) pos -= (ppos + 1);
+                    else if (snp2.type == HT2_ALT_SNP_DEL) pos -= ppos;
+                    else if (snp2.type == HT2_ALT_SNP_INS) pos -= (ppos + snp.len);
+                    break;
+                }
+                j--;
+            }
+            o.i64((int64_t)pos);
+            if (snp.type == HT2_ALT_SNP_SGL) o.s("|S|"); else if (snp.type == HT2_ALT_SNP_DEL) o.s("|D|"); else o.s("|I|");
+            o.str(altName(si));
+            first = false;
+            prev = si;
+        }
+        return o.n;
+    }
+
+    // AlnSinkSam::appendMate (aln_sink.h:3024-3250): one record at d; returns its length.  The common record (aligned,
+    // gapless, no ALTs) runs in this frame; gapped CIGAR / MD:Z, unaligned records, XS:A, Zs:Z and the junction
+    // collection are out of line.
+    template <bool W>
+    HT2_NI uint32_t appendMate(char* d, const Ht2SamRead& rd, uint32_t ordlen, const ht2gpu_aln_t* rs, const ht2gpu_aln_t* rso,
+                               const Ht2SamSumm& summ, const Ht2SamFlags& fl, bool fraglenSet, int64_t fraglen, bool haveOscore) const {
+        if (rs == NULL && in->noUnal) return 0;
+        Ht2SamCur<W> o = {d, 0};
+        o.name(rd.name, fl.partOfPair(), 255);
+        o.c('\t');
+        int flag = 0;
+        if (fl.partOfPair()) {
+            flag |= 1;
+            if (fl.concordant()) flag |= 2;
+            if (!fl.oppAligned) flag |= 8;
+            flag |= fl.readMate1() ? 64 : 128;
+            if (fl.oppAligned && rso != NULL && !rso->fw) flag |= 32;
+        }
+        if (!fl.primary) flag |= 256;
+        if (rs != NULL && !rs->fw) flag |= 16;
+        if (rs == NULL) flag |= 4;
+        o.i64(flag);
+        o.c('\t');
+        if (rs == NULL) return o.n + putUnaligned<W>(o.at(), rd, summ, fl);
+        if (W && in->colCount != NULL) collectSites(rs, rd.len);   // AlnSinkSam::append (aln_sink.h:1571, 1579)
+        const ht2gpu_edit_t* ed = in->edits + rs->edit_off;
+        const uint32_t ned = rs->n_edits;
+        // Gapless alignments (mismatches only; the vast majority): CIGAR and MD:Z follow from the edit positions
+        // directly -- what StackedAln::buildCigar / buildMdz print for a stack without I/D columns, with nothing for
+        // leftAlign to move.  Everything else goes through the stacked form (putStacked).
+        bool gapless = true;
+        for (uint32_t i = 0; i < ned; i++) if (ed[i].type != HT2_EDIT_MM) { gapless = false; break; }
+        uint32_t trimLS = rs->trim5, trimRS = rs->trim3;
+        const uint32_t len_trimmed = rd.len - trimLS - trimRS;
+        if (!rs->fw) { const uint32_t t = trimLS; trimLS = trimRS; trimRS = t; }
+        putRefName(o, rs->tidx);
+        o.c('\t');
+        o.i64((int64_t)rs->toff + 1);
+        o.c('\t');
+        o.i64(mapqV2(summ, rd.mate < 2, rd.len, ordlen));
+        o.c('\t');
+        if (gapless) {
+            if (trimLS > 0) { o.i64(trimLS); o.c('S'); }
+            if (len_trimmed > 0) { o.i64(len_trimmed); o.c('M'); }
+            if (trimRS > 0) { o.i64(trimRS); o.c('S'); }
+        } else o.n += putStacked<W>(o.at(), rd.seq, rd.len, rs, false);
+        o.c('\t');
+        if (fl.partOfPair()) {
+            if (rso != NULL && rs->tidx != rso->tidx) { putRefName(o, rso->tidx); o.c('\t'); }
+            else o.s("=\t");
+            o.i64((int64_t)(rso ? rso->toff : rs->toff) + 1);
+            o.c('\t');
+        } else o.s("*\t0\t");
+        o.i64(fraglenSet ? fraglen : 0);
+        o.c('\t');
+        if (!fl.primary && in->omitSecSeq) o.s("*\t*");
+        else putSeqQual(o, rd, rs->fw != 0);
+        // optional flags (sam.h:525-1010)
+        o.s("\tAS:i:"); o.i64(rs->score);
+        const Ht2SamKey& sb = summ.secbest[rd.mate < 2 ? 0 : 1];
+        if (sb.valid) { o.s("\tZS:i:"); o.i64(sb.score); }
+        o.s("\tXN:i:0");
+        // counts exclude edits that are known ALTs (snpID < #alts, sam.h:574-647)
+        uint32_t num_mm = 0, num_go = 0, num_gx = 0, NM = 0;
+        bool spliced = false;
+        for (uint32_t i = 0; i < ned; i++) {
+            if (ed[i].type == HT2_EDIT_SPL) spliced = true;
+            else if (ed[i].snp_id >= nAlts) NM++;
+        }
+        for (uint32_t i = 0; i < ned; i++) {
+            const ht2gpu_edit_t& e = ed[i];
+            if (e.type == HT2_EDIT_MM) { if (e.snp_id >= nAlts) num_mm++; }
+            else if (e.type == HT2_EDIT_READ_GAP) {
+                if (e.snp_id >= nAlts) { num_go++; num_gx++; }
+                while (i + 1 < ned && ed[i + 1].pos == ed[i].pos && ed[i + 1].type == HT2_EDIT_READ_GAP) { i++; if (ed[i].snp_id >= nAlts) num_gx++; }
+            } else if (e.type == HT2_EDIT_REF_GAP) {
+                if (e.snp_id >= nAlts) { num_go++; num_gx++; }
+                while (i + 1 < ned && ed[i + 1].pos == ed[i].pos + 1 && ed[i + 1].type == HT2_EDIT_REF_GAP) { i++; if (ed[i].snp_id >= nAlts) num_gx++; }
+            }
+        }
+        o.s("\tXM:i:"); o.i64(num_mm);
+        o.s("\tXO:i:"); o.i64(num_go);
+        o.s("\tXG:i:"); o.i64(num_gx);
+        o.s("\tNM:i:"); o.i64(NM);
+        o.s("\tMD:Z:");
+        if (gapless) {   // <matches>[<ref char><matches>]..., a 0 between adjacent mismatches and at either end
+            uint32_t prevEnd = 0;
+            for (uint32_t k = 0; k < ned; k++) {
+                const ht2gpu_edit_t& e = rs->fw ? ed[k] : ed[ned - 1 - k];
+                const uint32_t p = rs->fw ? e.pos : len_trimmed - e.pos - 1;
+                o.i64((int64_t)(p - prevEnd));
+                o.c((char)e.chr);
+                prevEnd = p + 1;
+            }
+            o.i64((int64_t)(len_trimmed - prevEnd));
+        } else o.n += putStacked<W>(o.at(), rd.seq, rd.len, rs, true);
         if (summ.paired && haveOscore && rso) { o.s("\tYS:i:"); o.i64(rso->score); }
-        o.s("\tYT:Z:"); o.s(ytz);
+        putYT(o, fl);
         putYF(o, rd);
         putRG(o);
 #ifdef HT2_ENABLE_SPLICED
-        {   // XS:A: AlnRes::spliced_whichsense_transcript (aligner_result.h:1288-1318, sam.h:925-937)
-            uint32_t whichsense = HT2_SPL_UNKNOWN; bool any = false;
-            for (uint32_t i = 0; i < ned; i++) {
-                if (ed[i].type != HT2_EDIT_SPL) continue;
-                any = true;
-                const uint32_t d = ht2_spl_dir(*(const Ht2Edit*)&ed[i]);
-                if (whichsense == HT2_SPL_UNKNOWN) whichsense = d;
-                else if (d != HT2_SPL_UNKNOWN) {
-                    if ((whichsense == HT2_SPL_FW || whichsense == HT2_SPL_SEMI_FW) && d != HT2_SPL_FW && d != HT2_SPL_SEMI_FW) { whichsense = HT2_SPL_UNKNOWN; break; }
-                    if ((whichsense == HT2_SPL_RC || whichsense == HT2_SPL_SEMI_RC) && d != HT2_SPL_RC && d != HT2_SPL_SEMI_RC) { whichsense = HT2_SPL_UNKNOWN; break; }
-                }
-            }
-            if (any && whichsense != HT2_SPL_UNKNOWN) { o.s("\tXS:A:"); o.c((whichsense == HT2_SPL_FW || whichsense == HT2_SPL_SEMI_FW) ? '+' : '-'); }
-        }
+        if (spliced) { const char xs = xsSense(ed, ned); if (xs) { o.s("\tXS:A:"); o.c(xs); } }
+#else
+        (void)spliced;
 #endif
         o.s("\tNH:i:");
         if (fl.concordant() || fl.discordant()) o.i64(summ.numAlnsPaired);
         else o.i64((fl.pairing == HT2_PAIR_UNPAIRED || fl.readMate1()) ? summ.numAlns[0] : summ.numAlns[1]);
-        // Zs:Z: the known ALTs the alignment went through (sam.h:983-1032); edits in reference-forward order
-        if (nAlts > 0) {
-            auto nedAt = [&](uint32_t i, uint32_t& pos) -> const ht2gpu_edit_t& {   // Edit::invertPoss (edit.cpp:70-111), sort = false
-                const ht2gpu_edit_t& e = rs->fw ? ed[i] : ed[ned - 1 - i];
-                pos = e.pos;
-                if (!rs->fw) pos = (e.type == HT2_EDIT_READ_GAP || e.type == HT2_EDIT_SPL) ? len_trimmed - e.pos : len_trimmed - e.pos - 1;
-                return e;
-            };
-            bool first = true;
-            uint32_t prev = 0xffffffffu;
-            for (uint32_t i = 0; i < ned; i++) {
-                uint32_t epos;
-                const ht2gpu_edit_t& e = nedAt(i, epos);
-                if (e.type == HT2_EDIT_SPL || e.snp_id >= nAlts) continue;   // a splice edit keeps its site probability in the snpID word
-                const uint32_t si = e.snp_id;
-                const Ht2Alt& snp = altTab[si];
-                if (si == prev) continue;
-                o.s(first ? "\tZs:Z:" : ",");
-                uint64_t pos = epos;
-                uint32_t j = i;
-                while (j > 0) {
-                    uint32_t ppos;
-                    const ht2gpu_edit_t& pe = nedAt(j - 1, ppos);
-                    if (pe.snp_id < nAlts) {
-                        const Ht2Alt& snp2 = altTab[pe.snp_id];
-                        if (snp2.type == HT2_ALT_SNP_SGL) pos -= (ppos + 1);
-                        else if (snp2.type == HT2_ALT_SNP_DEL) pos -= ppos;
-                        else if (snp2.type == HT2_ALT_SNP_INS) pos -= (ppos + snp.len);
-                        break;
-                    }
-                    j--;
-                }
-                o.i64((int64_t)pos);
-                o.s((snp.type == HT2_ALT_SNP_SGL) ? "|S|" : (snp.type == HT2_ALT_SNP_DEL ? "|D|" : "|I|"));
-                o.s(altName(si));
-                first = false;
-                prev = si;
-            }
-        }
+        if (nAlts > 0) o.n += putZs<W>(o.at(), rs, len_trimmed);
         o.c('\n');
+        return o.n;
     }
 
     // finishRead for an unpaired read (aln_sink.h:2213-2557, unpaired branches)
-    template <bool W> HT2_HD void finishUnpaired(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t) const {
+    template <bool W> HT2_HD void finishUnpaired(Ht2SamCur<W>& o, uint32_t u, Ht2SamTally* t) const {
         const ht2gpu_read_result_t& rr = in->reads[u];
         Ht2SamRead rd; mkRead(u, 0, rd);
         Ht2Rng rnd; rnd.last = rr.rng_state;
@@ -737,16 +916,16 @@ struct Ht2SamFmt {
             if (t) { t->c[HT2_T_NUNP_UNI1] += (uint32_t)(nsel == 1); t->c[HT2_T_NUNP_UNI2] += (uint32_t)(nsel != 1); }   // aln_sink.h:2290-2299
             for (uint32_t i = 0; i < nsel; i++) {
                 fl.primary = (i == 0);
-                appendMate(o, rd, 0, &rs[sel[i]], NULL, summ, fl, false, 0, false);
+                o.n += appendMate<W>(o.at(), rd, 0, &rs[sel[i]], NULL, summ, fl, false, 0, false);
             }
         } else {
             if (t) t->c[HT2_T_NUNP_0]++;
-            appendMate(o, rd, 0, NULL, NULL, summ, fl, false, 0, false);
+            o.n += appendMate<W>(o.at(), rd, 0, NULL, NULL, summ, fl, false, 0, false);
         }
     }
 
     // AlnSinkWrap::finishRead for a pair (aln_sink.h:1939-2557)
-    template <bool W> HT2_HD void finishPaired(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t) const {
+    template <bool W> HT2_HD void finishPaired(Ht2SamCur<W>& o, uint32_t u, Ht2SamTally* t) const {
         const ht2gpu_read_result_t& rr = in->reads[u];
         if (t) { t->c[HT2_T_NREAD]++; t->c[HT2_T_NPAIRED]++; }
         Ht2SamRead rd1, rd2; mkRead(2 * u, 1, rd1); mkRead(2 * u + 1, 2, rd2);
@@ -785,8 +964,8 @@ struct Ht2SamFmt {
             for (uint32_t i = 0; i < nsel; i++) {
                 const ht2gpu_aln_t& a = rs1u[pairs[2 * sel[i]]]; const ht2gpu_aln_t& b = rs2u[pairs[2 * sel[i] + 1]];
                 fl1.primary = fl2.primary = (i == 0);
-                appendMate(o, rd1, rd2.len, &a, &b, summ, fl1, true, fragmentLength(a, b, true, true), true);
-                appendMate(o, rd2, rd1.len, &b, &a, summ, fl2, true, fragmentLength(b, a, false, true), true);
+                o.n += appendMate<W>(o.at(), rd1, rd2.len, &a, &b, summ, fl1, true, fragmentLength(a, b, true, true), true);
+                o.n += appendMate<W>(o.at(), rd2, rd1.len, &b, &a, summ, fl2, true, fragmentLength(b, a, false, true), true);
             }
             return;
         } else if (discordant) {
@@ -801,8 +980,8 @@ struct Ht2SamFmt {
             (void)selectByScore(rs1u, n1, rd1.len, rs2u, rd2.len, dp, 1, true, 1, sel, rnd);
             Ht2SamFlags fl1 = {HT2_PAIR_DISCORD_MATE1, true, true}, fl2 = {HT2_PAIR_DISCORD_MATE2, true, true};
             const bool sameRef = a.tidx == b.tidx; // setMateParams (aligner_result.h:1594-1618)
-            appendMate(o, rd1, rd2.len, &a, &b, summ, fl1, sameRef, sameRef ? fragmentLength(a, b, true) : 0, true);
-            appendMate(o, rd2, rd1.len, &b, &a, summ, fl2, sameRef, sameRef ? fragmentLength(b, a, false) : 0, true);
+            o.n += appendMate<W>(o.at(), rd1, rd2.len, &a, &b, summ, fl1, sameRef, sameRef ? fragmentLength(a, b, true) : 0, true);
+            o.n += appendMate<W>(o.at(), rd2, rd1.len, &b, &a, summ, fl2, sameRef, sameRef ? fragmentLength(b, a, false) : 0, true);
             return;
         }
         uint64_t nunpair1 = 0, nunpair2 = 0;
@@ -842,16 +1021,16 @@ struct Ht2SamFmt {
             // AlnSink::reportHits (aln_sink.h:730-790)
             if (repRs2 != NULL) {
                 const ht2gpu_aln_t* r1pri = &rs1u[sel[0]]; const ht2gpu_aln_t* r2pri = &rs2u[sel2[0]];
-                appendMate(o, rd1, rd2.len, r1pri, r2pri, summ1, fl1, false, 0, false);
-                appendMate(o, rd2, rd1.len, r2pri, r1pri, summ1, fl2, false, 0, false);
+                o.n += appendMate<W>(o.at(), rd1, rd2.len, r1pri, r2pri, summ1, fl1, false, 0, false);
+                o.n += appendMate<W>(o.at(), rd2, rd1.len, r2pri, r1pri, summ1, fl2, false, 0, false);
                 fl1.primary = fl2.primary = false;
-                for (uint32_t i = 1; i < nsel1; i++) appendMate(o, rd1, rd2.len, &rs1u[sel[i]], r2pri, summ1, fl1, false, 0, false);
-                for (uint32_t i = 1; i < nsel2; i++) appendMate(o, rd2, rd1.len, &rs2u[sel2[i]], r1pri, summ1, fl2, false, 0, false);
+                for (uint32_t i = 1; i < nsel1; i++) o.n += appendMate<W>(o.at(), rd1, rd2.len, &rs1u[sel[i]], r2pri, summ1, fl1, false, 0, false);
+                for (uint32_t i = 1; i < nsel2; i++) o.n += appendMate<W>(o.at(), rd2, rd1.len, &rs2u[sel2[i]], r1pri, summ1, fl2, false, 0, false);
                 fl1.primary = fl2.primary = true;
             } else {
                 for (uint32_t i = 0; i < nsel1; i++) {
                     fl1.primary = (i == 0);
-                    appendMate(o, rd1, 0, &rs1u[sel[i]], NULL, summ1, fl1, false, 0, false);
+                    o.n += appendMate<W>(o.at(), rd1, 0, &rs1u[sel[i]], NULL, summ1, fl1, false, 0, false);
                 }
                 fl1.primary = true;
             }
@@ -860,7 +1039,7 @@ struct Ht2SamFmt {
         if (rep2 && !rep1) {
             for (uint32_t i = 0; i < nsel2; i++) {
                 fl2.primary = (i == 0);
-                appendMate(o, rd2, 0, &rs2u[sel2[i]], NULL, summ2, fl2, false, 0, false);
+                o.n += appendMate<W>(o.at(), rd2, 0, &rs2u[sel2[i]], NULL, summ2, fl2, false, 0, false);
             }
             fl2.primary = true;
             refid = rs2u[sel2[0]].tidx; refoff = rs2u[sel2[0]].toff;
@@ -869,19 +1048,21 @@ struct Ht2SamFmt {
             Ht2SamSumm s; s.reset();
             if (nunpair2 > 0) { s.orefid = refid; s.orefoff = refoff; }
             Ht2SamFlags fl = {HT2_PAIR_UNPAIRED_MATE1, true, repRs2 != NULL};
-            appendMate(o, rd1, 0, NULL, NULL, s, fl, false, 0, false);
+            o.n += appendMate<W>(o.at(), rd1, 0, NULL, NULL, s, fl, false, 0, false);
         }
         if (nunpair2 == 0) {
             Ht2SamSumm s; s.reset();
             if (nunpair1 > 0) { s.orefid = refid; s.orefoff = refoff; }
             Ht2SamFlags fl = {HT2_PAIR_UNPAIRED_MATE2, true, repRs1 != NULL};
-            appendMate(o, rd2, 0, NULL, NULL, s, fl, false, 0, false);
+            o.n += appendMate<W>(o.at(), rd2, 0, NULL, NULL, s, fl, false, 0, false);
         }
     }
 
     // t != NULL: also tally the unit's outcome (the counting pass)
     template <bool W> HT2_HD void unit(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t = NULL) const {
-        if (in->paired) finishPaired(o, u, t); else finishUnpaired(o, u, t);
+        Ht2SamCur<W> c = {W ? o.p + o.n : NULL, 0};
+        if (in->paired) finishPaired(c, u, t); else finishUnpaired(c, u, t);
+        o.n += c.n;
     }
 };
 
