@@ -82,6 +82,69 @@ class CParsedReads(C.Structure):
 
 SINK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
 
+# The read files of --un, --al, --un-conc, --al-conc and --al-conc-disc, in the order of HT2GPU_READS_* (ht2gpu.h)
+READ_FILES = ("un", "al", "un_conc", "al_conc", "al_conc_disc")
+READS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t)
+
+
+class CReadRoutes(C.Structure):
+    _fields_ = [("mask", C.c_uint32), ("write", READS_FN), ("ctx", C.c_void_p), ("n_spans", C.c_uint64), ("bytes", C.c_uint64),
+                ("s_route", C.c_double)]
+
+
+def _read_routes(read_files):
+    """(CReadRoutes, {(output, mate): [chunks]}) collecting the spans of the outputs in read_files.  mate is 0 for
+    un / al and 1 / 2 for the -conc outputs."""
+    unknown = set(read_files) - set(READ_FILES)
+    if unknown:
+        raise ValueError("unknown read files %s (choose from %s)" % (sorted(unknown), READ_FILES))
+    chunks = {}
+    for w in read_files:
+        for m in ((0,) if READ_FILES.index(w) < 2 else (1, 2)):
+            chunks[(w, m)] = []
+
+    def _write(ctx, which, mate, ptr, n):
+        chunks[(READ_FILES[which], mate)].append(C.string_at(ptr, n))
+        return 0
+    rt = CReadRoutes()
+    rt.mask = sum(1 << READ_FILES.index(w) for w in read_files)
+    rt.write = READS_FN(_write)
+    return rt, chunks
+
+
+def _reads_input(path1=None, path2=None, data1=None, data2=None, fastq=False, **kw):
+    """(CReadsInput, buffers to keep alive) for FASTA / FASTQ files or bytes in host memory."""
+    ri = CReadsInput()
+    keep = []
+    if path1 is not None:
+        ri.path1 = os.fsencode(path1)
+    if path2 is not None:
+        ri.path2 = os.fsencode(path2)
+    for name, d in (("1", data1), ("2", data2)):
+        if d is not None:
+            buf = np.frombuffer(d, dtype=np.uint8)
+            keep.append(buf)
+            setattr(ri, "data" + name, buf.ctypes.data)
+            setattr(ri, "len" + name, buf.nbytes)
+    ri.format = 1 if fastq else 0
+    for k, v in kw.items():
+        setattr(ri, k, v)
+    return ri, keep
+
+
+def route_reads(outcomes, path1=None, path2=None, data1=None, data2=None, fastq=False, read_files=READ_FILES, **kw):
+    """ht2gpu_route_reads, host only: the records of an input (after skip / upto) written to the read files by their
+    units' outcome bytes (HT2GPU_OUTCOME_*, e.g. Index.unit_outcomes).  Returns {(output, mate): bytes}."""
+    lib = load_library()
+    ri, keep = _reads_input(path1, path2, data1, data2, fastq, **kw)
+    out = np.ascontiguousarray(outcomes, dtype=np.uint8)
+    rt, chunks = _read_routes(read_files)
+    err = C.create_string_buffer(512)
+    rc = lib.ht2gpu_route_reads(C.byref(ri), out.ctypes.data, len(out), C.byref(rt), err, 512)
+    if rc != 0:
+        raise Ht2GpuError("ht2gpu_route_reads rc=%d: %s" % (rc, err.value.decode()))
+    return {k: b"".join(v) for k, v in chunks.items()}
+
 
 class CSamOutput(C.Structure):
     _fields_ = [("no_unal", C.c_int32), ("omit_sec_seq", C.c_int32), ("no_sq", C.c_int32), ("rg_id", C.c_char_p),
@@ -107,7 +170,8 @@ EXPORTS = [
     "ht2gpu_host_alloc", "ht2gpu_host_free", "ht2gpu_set_error", "ht2gpu_parse_reads", "ht2gpu_free_parsed",
     "ht2gpu_ctx_get", "ht2gpu_ctx_set", "ht2gpu_run_reads_multi", "ht2gpu_open_peer", "ht2gpu_sw_selftest", "ht2gpu_load_splicesites", "ht2gpu_collect_splicesites",
     "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry", "ht2gpu_set_sam_output", "ht2gpu_align_counts",
-    "ht2gpu_format_align_summary", "ht2gpu_sw_extend",
+    "ht2gpu_format_align_summary", "ht2gpu_sw_extend", "ht2gpu_record_outcomes", "ht2gpu_unit_outcomes",
+    "ht2gpu_run_reads_routed", "ht2gpu_route_reads",
 ]
 
 
@@ -166,6 +230,11 @@ def load_library(path=None):
     lib.ht2gpu_align_sam.argtypes = [C.c_void_p, C.POINTER(CReadBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(CSamResult)]
     lib.ht2gpu_run_reads.argtypes = [C.c_void_p, C.POINTER(CReadsInput), SINK_FN, C.c_void_p, C.POINTER(CRunStats)]
     lib.ht2gpu_run_reads_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(CReadsInput), SINK_FN, C.c_void_p, C.POINTER(CRunStats)]
+    lib.ht2gpu_run_reads_routed.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(CReadsInput), SINK_FN, C.c_void_p,
+                                            C.POINTER(CReadRoutes), C.POINTER(CRunStats)]
+    lib.ht2gpu_route_reads.argtypes = [C.POINTER(CReadsInput), C.c_void_p, C.c_uint64, C.POINTER(CReadRoutes), C.c_char_p, C.c_size_t]
+    lib.ht2gpu_record_outcomes.argtypes = [C.c_void_p, C.c_int]
+    lib.ht2gpu_unit_outcomes.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
     lib.ht2gpu_open_peer.argtypes = [C.c_void_p, C.POINTER(Options), C.POINTER(C.c_void_p)]
     lib.ht2gpu_host_alloc.argtypes = [C.c_size_t]; lib.ht2gpu_host_alloc.restype = C.c_void_p
     lib.ht2gpu_host_free.argtypes = [C.c_void_p]
@@ -542,6 +611,17 @@ class Index(object):
             return s, {k: getattr(cr, k) for k, _ in CSamResult._fields_ if k != "sam"}
         return s
 
+    def record_outcomes(self, enable=True):
+        """ht2gpu_record_outcomes: the SAM counting pass stores each unit's outcome byte (for unit_outcomes)."""
+        self._check(self._lib.ht2gpu_record_outcomes(self._h, 1 if enable else 0), "ht2gpu_record_outcomes")
+
+    def unit_outcomes(self, slot=0):
+        """ht2gpu_unit_outcomes: a copy of the outcome bytes (HT2GPU_OUTCOME_AL1 | AL2 | CONC per read or pair) of the
+        slot's last batch; align_sam uses slot 0.  Needs record_outcomes() before that batch."""
+        p, n = C.c_void_p(), C.c_uint32()
+        self._check(self._lib.ht2gpu_unit_outcomes(self._h, slot, C.byref(p), C.byref(n)), "ht2gpu_unit_outcomes")
+        return np.frombuffer(C.string_at(p.value, n.value), dtype=np.uint8).copy() if n.value else np.zeros(0, np.uint8)
+
     def load_splicesites(self, known=None, novel=None):
         """ht2gpu_load_splicesites: --known-splicesite-infile / --novel-splicesite-infile; returns the number of sites kept."""
         n = C.c_uint32(0)
@@ -601,25 +681,14 @@ class Index(object):
             other.set_sam_output(**self._sam_output)
         return other
 
-    def run_reads(self, path1=None, path2=None, data1=None, data2=None, fastq=False, collect=True, peers=(), sink=None, **kw):
+    def run_reads(self, path1=None, path2=None, data1=None, data2=None, fastq=False, collect=True, peers=(), sink=None,
+                  read_files=(), **kw):
         """ht2gpu_run_reads(_multi): FASTA/FASTQ (files or bytes in host memory) -> SAM records through the overlapped
         pipeline, on this index's device and on the devices of `peers`.  Returns (sam bytes or None, stats dict).
-        `sink(ptr, n)`, if given, sees the SAM text of every batch in read order while it is valid (pinned host memory)."""
-        ri = CReadsInput()
-        keep = []
-        if path1 is not None:
-            ri.path1 = os.fsencode(path1)
-        if path2 is not None:
-            ri.path2 = os.fsencode(path2)
-        for name, d in (("1", data1), ("2", data2)):
-            if d is not None:
-                buf = np.frombuffer(d, dtype=np.uint8)
-                keep.append(buf)
-                setattr(ri, "data" + name, buf.ctypes.data)
-                setattr(ri, "len" + name, buf.nbytes)
-        ri.format = 1 if fastq else 0
-        for k, v in kw.items():
-            setattr(ri, k, v)
+        `sink(ptr, n)`, if given, sees the SAM text of every batch in read order while it is valid (pinned host memory).
+        With read_files (names of READ_FILES) the records are also routed (ht2gpu_run_reads_routed) and the call returns
+        (sam, stats, {(output, mate): bytes}); stats then also holds route_spans, route_bytes and s_route."""
+        ri, keep = _reads_input(path1, path2, data1, data2, fastq, **kw)
         chunks = []
         total = [0]
 
@@ -633,9 +702,16 @@ class Index(object):
         cb = SINK_FN(_sink) if (collect or sink is not None) else SINK_FN()     # NULL sink: the text still lands in pinned host memory
         st = CRunStats()
         hs = (C.c_void_p * (1 + len(peers)))(self._h, *[p._h for p in peers])
-        self._check(self._lib.ht2gpu_run_reads_multi(hs, len(hs), C.byref(ri), cb, None, C.byref(st)), "ht2gpu_run_reads")
+        if read_files:
+            rt, files = _read_routes(read_files)
+            self._check(self._lib.ht2gpu_run_reads_routed(hs, len(hs), C.byref(ri), cb, None, C.byref(rt), C.byref(st)), "ht2gpu_run_reads_routed")
+        else:
+            self._check(self._lib.ht2gpu_run_reads_multi(hs, len(hs), C.byref(ri), cb, None, C.byref(st)), "ht2gpu_run_reads")
         stats = {k: getattr(st, k) for k, _ in CRunStats._fields_ if k != "pad"}
-        return (b"".join(chunks) if collect else None), stats
+        if not read_files:
+            return (b"".join(chunks) if collect else None), stats
+        stats.update(route_spans=rt.n_spans, route_bytes=rt.bytes, s_route=rt.s_route)
+        return (b"".join(chunks) if collect else None), stats, {k: b"".join(v) for k, v in files.items()}
 
     def is_graph(self):
         return bool(self._lib.ht2gpu_index_is_graph(self._h))

@@ -5,9 +5,71 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <sys/stat.h>
+#include <sys/wait.h>
 #include <string>
 #include <vector>
 #include "ht2gpu.h"
+
+// --un / --al / --un-conc / --al-conc / --al-conc-disc and their -gz / -bz2 forms: the read files of the hisat2
+// wrapper (hisat2:546-650).  Outputs are opened before the run; compressed ones are piped through gzip -c / bzip2 -c.
+static const char* const kReadOpt[HT2GPU_READS_N] = {"un", "al", "un-conc", "al-conc", "al-conc-disc"};
+struct ReadFile { FILE* f = NULL; bool pipe = false; std::string path; };
+static bool closeReadFile(ReadFile& rf);
+struct ReadFiles {
+    std::string spec[HT2GPU_READS_N];
+    int compress[HT2GPU_READS_N] = {0, 0, 0, 0, 0};   // 0 none, 1 gzip, 2 bzip2
+    ReadFile file[HT2GPU_READS_N][2];                // [output][mate 1 or unpaired, mate 2]
+    uint32_t mask() const { uint32_t m = 0; for (int w = 0; w < HT2GPU_READS_N; w++) if (!spec[w].empty()) m |= 1u << w; return m; }
+    ~ReadFiles() { for (auto& f : file) { closeReadFile(f[0]); closeReadFile(f[1]); } }   // every exit waits for gzip / bzip2
+};
+// The wrapper's names (File::Spec->splitpath + catpath): a directory (or a path ending in '/') gets <opt>-seqs, or
+// <opt>-mate.1 / .2; with -conc a '%' in the name becomes 1 / 2, else .1 / .2 goes in before the last extension, else
+// it is appended.
+static std::string readFileName(const std::string& spec, int which, int mate)
+{
+    struct stat st;
+    const bool isDir = stat(spec.c_str(), &st) == 0 && S_ISDIR(st.st_mode);
+    std::string dir, base;
+    if (isDir) dir = spec;
+    else { const size_t k = spec.rfind('/'); dir = k == std::string::npos ? "" : spec.substr(0, k + 1); base = spec.substr(dir.size()); }
+    const bool conc = which >= HT2GPU_READS_UN_CONC;
+    if (base.empty()) base = std::string(kReadOpt[which]) + (conc ? "-mate" : "-seqs");
+    else if (!conc) return spec;
+    if (conc) {
+        const char m = mate == 2 ? '2' : '1';
+        const size_t dot = base.rfind('.');
+        if (base.find('%') != std::string::npos) { for (char& c : base) if (c == '%') c = m; }
+        else if (dot != std::string::npos) base = base.substr(0, dot) + "." + m + base.substr(dot);
+        else base += std::string(".") + m;
+    }
+    if (!dir.empty() && dir.back() != '/') dir += '/';
+    return dir + base;
+}
+static bool openReadFile(ReadFile& rf, const std::string& path, int compress)
+{
+    rf.path = path;
+    FILE* f = fopen(path.c_str(), "wb");   // the wrapper's open(): an unwritable path is an error before anything runs
+    if (!f) return false;
+    if (!compress) { rf.f = f; return true; }
+    fclose(f);
+    std::string q = "'";
+    for (char c : path) { if (c == '\'') q += "'\\''"; else q += c; }
+    q += "'";
+    const std::string cmd = std::string(compress == 1 ? "gzip -c > " : "bzip2 -c > ") + q;
+    rf.f = popen(cmd.c_str(), "w");
+    rf.pipe = true;
+    return rf.f != NULL;
+}
+static bool closeReadFile(ReadFile& rf)
+{
+    if (!rf.f) return true;
+    bool ok = fflush(rf.f) == 0 && !ferror(rf.f);
+    if (rf.pipe) { const int st = pclose(rf.f); ok = ok && st != -1 && WIFEXITED(st) && WEXITSTATUS(st) == 0; }
+    else ok = fclose(rf.f) == 0 && ok;
+    rf.f = NULL;
+    return ok;
+}
 
 static void usage() {
     fprintf(stderr, "hisat2-b200 -x <index> {-U <r> | -1 <m1> -2 <m2>} [-S out.sam] [-f|-q] --no-spliced-alignment [-k N]\n"
@@ -17,7 +79,10 @@ static void usage() {
                     "            [--known-splicesite-infile F] [--novel-splicesite-infile F] [--novel-splicesite-outfile F]\n"
                     "            [--bowtie2-dp 0|1|2] [--score-min F,C,L] [--gbar N] [--sensitive] [--very-sensitive] [--fast]\n"
                     "            [--no-unal] [--omit-sec-seq] [--no-hd] [--no-sq] [--rg-id ID] [--rg TEXT]...\n"
-                    "            [--summary-file F] [--new-summary] [--quiet]\n");
+                    "            [--summary-file F] [--new-summary] [--quiet]\n"
+                    "            [--un P] [--al P] [--un-conc P] [--al-conc P] [--al-conc-disc P], each also as --<opt>-gz\n"
+                    "            and --<opt>-bz2: write unpaired reads that did not / did align, pairs that did not / did align\n"
+                    "            concordantly, and pairs with at least one aligned mate (P.1 / P.2, or '%%' in P replaced by 1 / 2)\n");
 }
 static void two(const char* a, int32_t& x, int32_t& y) { sscanf(a, "%d,%d", &x, &y); }
 
@@ -36,6 +101,7 @@ int main(int argc, char** argv)
     int32_t noUnal = 0, omitSecSeq = 0, noSq = 0;
     std::string rgId; std::vector<std::string> rgFields;
     const char* summaryFile = NULL;
+    ReadFiles rfs;
     bool mpGiven = false;   // "--mp a,b" becomes MMP=Q,a,b, which switches the cost model back to quality-aware even
                             // under --ignore-quals (aligner_seed_policy.cpp:396-418)
     for (int i = 1; i < argc; i++) {
@@ -83,6 +149,11 @@ int main(int argc, char** argv)
         }
         else if (a == "--summary-file") summaryFile = next(); else if (a == "--new-summary") newSummary = true;
         else if (a == "--quiet") quiet = true;   // no alignment summary (hisat2.cpp:4165)
+        else if (a.compare(0, 2, "--") == 0 && [&]() {
+                     for (int w = 0; w < HT2GPU_READS_N; w++)
+                         for (int c = 0; c < 3; c++)
+                             if (a == std::string("--") + kReadOpt[w] + (c == 1 ? "-gz" : c == 2 ? "-bz2" : "")) { rfs.spec[w] = next(); rfs.compress[w] = c; return true; }
+                     return false; }()) {}
         else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--fr" || a == "--no-unal-ignored") {}
         else if (a == "-h" || a == "--help") { usage(); return 0; }
         else { fprintf(stderr, "Error: option %s is not supported by hisat2-b200\n", a.c_str()); return 1; }
@@ -104,6 +175,18 @@ int main(int argc, char** argv)
         o.score_min_type = 'L'; o.score_min_const = (double)0.0f; o.score_min_coeff = (double)-1.0f;
     }
     o.seed = gseed;
+    // read files: opened before the run starts, like the wrapper
+    for (int w = 0; w < HT2GPU_READS_N; w++) {
+        if (rfs.spec[w].empty()) continue;
+        const int nMates = w >= HT2GPU_READS_UN_CONC ? 2 : 1;
+        for (int m = 0; m < nMates; m++) {
+            const std::string fn = readFileName(rfs.spec[w], w, nMates == 2 ? m + 1 : 0);
+            if (!openReadFile(rfs.file[w][m], fn, rfs.compress[w])) {
+                fprintf(stderr, "Error: could not open --%s%s output file '%s'\n", kReadOpt[w], nMates == 2 ? (m ? " mate-2" : " mate-1") : "", fn.c_str());
+                return 1;
+            }
+        }
+    }
     ht2gpu_handle_t* h = NULL;
     if (ht2gpu_open(idx, &o, &h) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
     const bool paired = m1 != NULL;
@@ -123,6 +206,12 @@ int main(int argc, char** argv)
     in.path1 = paired ? m1 : u; in.path2 = paired ? m2 : NULL;
     in.format = fastq ? 1 : 0; in.trim5 = trim5; in.trim3 = trim3; in.phred64 = phred64 ? 1 : 0; in.seed = gseed;
     in.skip = skip; in.upto = upto; in.batch_reads = (uint32_t)batchSz; in.threads = threads;
+    ht2gpu_read_routes_t routes; memset(&routes, 0, sizeof(routes));
+    routes.mask = rfs.mask(); routes.ctx = &rfs;
+    routes.write = [](void* ctx, int which, int mate, const char* data, size_t len) -> int {
+        FILE* f = ((ReadFiles*)ctx)->file[which][mate == 2 ? 1 : 0].f;
+        return fwrite(data, 1, len, f) == len ? 0 : 1;
+    };
     ht2gpu_run_stats_t st;
     auto sink = [](void* ctx, const char* sam, size_t len) -> int { return fwrite(sam, 1, len, (FILE*)ctx) == len ? 0 : 1; };
     std::vector<ht2gpu_handle_t*> hs(1, h);
@@ -141,7 +230,15 @@ int main(int argc, char** argv)
     if (novelOut)
         for (ht2gpu_handle_t* hh : hs)
             if (ht2gpu_collect_splicesites(hh, 1) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(hh)); return 1; }
-    if (ht2gpu_run_reads_multi(hs.data(), (int)hs.size(), &in, sink, fo, &st) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
+    const int runRc = ht2gpu_run_reads_routed(hs.data(), (int)hs.size(), &in, sink, fo, &routes, &st);
+    bool filesOk = true;
+    for (int w = 0; w < HT2GPU_READS_N; w++)
+        for (int m = 0; m < 2; m++) {
+            ReadFile& rf = rfs.file[w][m];
+            if (rf.f && !closeReadFile(rf)) { fprintf(stderr, "Error: could not write --%s output file '%s'\n", kReadOpt[w], rf.path.c_str()); filesOk = false; }
+        }
+    if (runRc != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
+    if (!filesOk) return 1;
     if (novelOut) {
         uint64_t nw = 0;
         if (ht2gpu_write_novel_splicesites(hs.data(), (int)hs.size(), novelOut, &nw) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }

@@ -652,6 +652,9 @@ struct SamSlot {
     char* dSam; size_t capSam;
     Ht2SsRec* dColRecs; size_t capCol;            // --novel-splicesite-outfile: junction records of the batch (count in dCounters[6])
     unsigned long long* dTally;                   // ReportingMetrics of the batch (HT2_T_N counters, ht2_sam.h), zeroed per SAM pass
+    uint8_t* dOut; size_t capOut;                 // ht2gpu_record_outcomes: one HT2GPU_OUTCOME_* byte per unit (counting pass)
+    uint8_t* hOut; size_t capHOut;                // ... copied back with the meta (pinned)
+    bool outValid;                                // hOut holds the outcomes of the batch the last ht2gpu_wait_sam returned
     char* hSam; size_t capHSam;                   // pinned
     unsigned long long* hMeta;                    // pinned: [0] total SAM bytes, [1..4] result counters, [5] reads with errors,
                                                   //         [HT2_META_TALLY ..] the batch's ReportingMetrics
@@ -698,6 +701,7 @@ struct ht2gpu_handle {
     void*          dSplT;    // spliced builds: Ht2SplTables on the device
     uint8_t*       dSsT;     // the run's splice-site DB on the device (ht2gpu_load_splicesites) or NULL
     bool           collectSs; // --novel-splicesite-outfile: collect the junctions of printed alignments
+    bool           recordOut; // ht2gpu_record_outcomes: the SAM counting pass stores each unit's outcome byte
     Ht2NovelSites  novel;     // ... aggregated here (ht2gpu_wait_sam), written by ht2gpu_write_novel_splicesites
     std::mutex     novelMu;
     std::vector<uint8_t> ssBlob;   // ... and its host copy (host formatter)
@@ -887,7 +891,7 @@ static int finishOpen(ht2gpu_handle* h)
 static ht2gpu_handle* newHandle(const ht2gpu_options_t* opt)
 {
     ht2gpu_handle* h = new ht2gpu_handle();
-    h->img = NULL; h->dBlob = NULL; h->ownBlob = false; h->blobBytes = 0; h->pool = NULL; h->nWork = 0; h->dMinsc = NULL; h->dSplT = NULL; h->dSsT = NULL; h->collectSs = false;
+    h->img = NULL; h->dBlob = NULL; h->ownBlob = false; h->blobBytes = 0; h->pool = NULL; h->nWork = 0; h->dMinsc = NULL; h->dSplT = NULL; h->dSsT = NULL; h->collectSs = false; h->recordOut = false;
     h->stream = 0;
     h->dStats = NULL;
     memset((void*)h->slots, 0, sizeof(h->slots));
@@ -1039,8 +1043,9 @@ extern "C" int ht2gpu_close(ht2gpu_handle_t* h)
         cudaStreamSynchronize(S.stream);
         cudaFree(S.dSeq); cudaFree(S.dQual); cudaFree(S.dOffs); cudaFree(S.dSeeds); cudaFree(S.dNames); cudaFree(S.dNameOffs);
         cudaFree(S.dReads); cudaFree(S.dAlns); cudaFree(S.dEdits); cudaFree(S.dPairs); cudaFree(S.dCounters);
-        cudaFree(S.dSamLen); cudaFree(S.dBlk); cudaFree(S.dSam); cudaFree(S.dColRecs); cudaFree(S.dTally);
+        cudaFree(S.dSamLen); cudaFree(S.dBlk); cudaFree(S.dSam); cudaFree(S.dColRecs); cudaFree(S.dTally); cudaFree(S.dOut);
         if (S.hSam) cudaFreeHost(S.hSam);
+        if (S.hOut) cudaFreeHost(S.hOut);
         if (S.hMeta) cudaFreeHost(S.hMeta);
         cudaStreamDestroy(S.stream);
         for (int i = 0; i < 6; i++) cudaEventDestroy(S.ev[i]);
@@ -1323,6 +1328,7 @@ static Ht2SamIn samIn(const ht2gpu_handle* h, const SamSlot& S)
     in.khits = h->P.khits; in.secondary = h->P.secondary; in.mixed = h->P.mixed; in.discord = h->P.discord; in.ssT = h->dSsT;
     in.colCount = h->collectSs ? S.dCounters + 6 : NULL; in.colRecs = S.dColRecs; in.colCap = (uint32_t)S.capCol;
     in.noUnal = h->samOut.noUnal; in.omitSecSeq = h->samOut.omitSecSeq; in.rgTag = h->dRgTag;
+    in.unitOut = h->recordOut ? S.dOut : NULL;
     return in;
 }
 
@@ -1335,6 +1341,15 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
     CK(growBuf(S.dSamLen, S.capSamLen, units));
     CK(growBuf(S.dBlk, S.capBlk, (size_t)nBlk + 2));
     if (h->collectSs) CK(growBuf(S.dColRecs, S.capCol, (size_t)S.batch.n_reads * 4 + 1024, 1, 1));
+    if (h->recordOut) {
+        CK(growBuf(S.dOut, S.capOut, units));
+        if (units > S.capHOut) {
+            if (S.hOut) CK(cudaFreeHost(S.hOut));
+            S.hOut = NULL; S.capHOut = 0;
+            CK(cudaHostAlloc(&S.hOut, (size_t)units + units / 8 + 4096, cudaHostAllocPortable));
+            S.capHOut = (size_t)units + units / 8 + 4096;
+        }
+    }
     std::lock_guard<std::mutex> lk(h->pool->mu);
     CK(cudaStreamWaitEvent(S.stream, h->pool->evDone, 0));
     if (withAlign) { int rc = launchAlign(h, S, &S.batch, units, S.ev[2]); if (rc) return rc; S.nLaunch++; }
@@ -1359,6 +1374,7 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
     CK(cudaMemcpyAsync(&S.hMeta[0], S.dBlk + nBlk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
     CK(cudaMemcpyAsync(&S.hMeta[1], S.dCounters, 8 * sizeof(unsigned int), cudaMemcpyDeviceToHost, S.stream));
     CK(cudaMemcpyAsync(&S.hMeta[HT2_META_TALLY], S.dTally, HT2_T_N * sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
+    if (h->recordOut) CK(cudaMemcpyAsync(S.hOut, S.dOut, units, cudaMemcpyDeviceToHost, S.stream));
     return HT2GPU_OK;
 }
 
@@ -1381,7 +1397,7 @@ extern "C" int ht2gpu_submit_sam(ht2gpu_handle_t* h, int slot, const ht2gpu_read
     if (rc) return rc;
     if (S.pending) { h->err = "ht2gpu_submit_sam: the slot still holds a batch (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
     S.batch = *b; S.units = b->paired ? b->n_reads / 2 : b->n_reads; S.namesBytes = names_bytes; S.nLaunch = 0; S.h2dBytes = 0;
-    S.pending = true;
+    S.pending = true; S.outValid = false;
     if (b->n_reads == 0) return HT2GPU_OK;
     CK(cudaEventRecord(S.ev[0], S.stream));
     rc = uploadBatch(h, S, b, names, name_offs, names_bytes, S.h2dBytes);
@@ -1405,7 +1421,7 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
     if (!S.init || !S.pending) { h->err = "ht2gpu_wait_sam: nothing was submitted on this slot"; return HT2GPU_ERR_ARG; }
     S.pending = false;
     out->n_units = S.units;
-    if (S.batch.n_reads == 0) { out->sam = S.hSam ? S.hSam : (char*)""; return HT2GPU_OK; }
+    if (S.batch.n_reads == 0) { out->sam = S.hSam ? S.hSam : (char*)""; S.outValid = h->recordOut; return HT2GPU_OK; }
     CK(cudaSetDevice(h->device));
     for (int attempt = 0; ; attempt++) {
         CK(cudaStreamSynchronize(S.stream));
@@ -1456,13 +1472,14 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
                 total / ((ms[0] + ms[1] + ms[2]) * 1e6), total / (ms[2] * 1e6));
     }
     const unsigned int* c = (const unsigned int*)&S.hMeta[1];
+    S.outValid = h->recordOut;
     out->sam = S.hSam; out->sam_len = total;
     out->n_alns = c[0]; out->n_err_reads = c[4];
     CK(cudaEventElapsedTime(&out->ms_h2d, S.ev[0], S.ev[1]));
     CK(cudaEventElapsedTime(&out->ms_align, S.ev[2], S.ev[3]));
     CK(cudaEventElapsedTime(&out->ms_sam, S.ev[3], S.ev[4]));
     CK(cudaEventElapsedTime(&out->ms_d2h, S.ev[4], S.ev[5]));
-    out->h2d_bytes = S.h2dBytes; out->d2h_bytes = total + 9 * sizeof(unsigned long long);
+    out->h2d_bytes = S.h2dBytes; out->d2h_bytes = total + 9 * sizeof(unsigned long long) + (h->recordOut ? S.units : 0);
     out->n_launches = S.nLaunch;
     if (c[4]) {
         char buf[160]; snprintf(buf, sizeof(buf), "device capacity exceeded for %u read(s) of the batch; their SAM records are unreliable", c[4]);
@@ -1853,6 +1870,30 @@ extern "C" int ht2gpu_format_sam(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* 
     if (const char* e = getenv("HT2GPU_THREADS")) nth = (unsigned)atoi(e);
     return ht2_format_batch(*h->img, h->P, b, names, res, out, out_len, nth, h->ssBlob.empty() ? NULL : h->ssBlob.data(),
                             NULL, NULL, 0, &h->samOut) ? HT2GPU_OK : HT2GPU_ERR_ARG;
+}
+
+// Read outcomes for --un / --al / --un-conc / --al-conc / --al-conc-disc (ht2gpu.h): the counting pass stores them
+// only while enabled, so a handle that never asks runs exactly the kernels and copies it ran without them.
+extern "C" int ht2gpu_record_outcomes(ht2gpu_handle_t* h, int enable)
+{
+    if (!h) return HT2GPU_ERR_ARG;
+    for (int k = 0; k < HT2GPU_N_SLOTS; k++)
+        if (h->slots[k].pending) { h->err = "ht2gpu_record_outcomes: a batch is in flight (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
+    h->recordOut = enable != 0;
+    return HT2GPU_OK;
+}
+
+extern "C" int ht2gpu_unit_outcomes(ht2gpu_handle_t* h, int slot, const uint8_t** bytes, uint32_t* n_units)
+{
+    if (!h || !bytes || !n_units || slot < 0 || slot >= HT2GPU_N_SLOTS) return HT2GPU_ERR_ARG;
+    const SamSlot& S = h->slots[slot];
+    *bytes = NULL; *n_units = 0;
+    if (!S.init || !S.outValid) {
+        h->err = "ht2gpu_unit_outcomes: the slot holds no outcomes (ht2gpu_record_outcomes, then ht2gpu_wait_sam)";
+        return HT2GPU_ERR_ARG;
+    }
+    *bytes = S.hOut; *n_units = S.units;
+    return HT2GPU_OK;
 }
 
 // SAM output settings (--no-unal, --omit-sec-seq, --no-sq, --rg-id / --rg).  The read group's "RG:Z:<id>" is uploaded

@@ -369,7 +369,7 @@ extern "C" int ht2gpu_format_align_summary(const ht2gpu_align_counts_t* c, int n
 // over the ranges, a writing pass straight into the output (records in read order = --reorder).
 bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read_batch_t* b, const char* names,
                       const ht2gpu_result_batch_t* res, char** out, size_t* out_len, unsigned nth, const uint8_t* ssT, uint32_t* colCount, Ht2SsRec* colRecs, uint32_t colCap,
-                      const Ht2SamOutput* so, ht2gpu_align_counts_t* counts)
+                      const Ht2SamOutput* so, ht2gpu_align_counts_t* counts, uint8_t* unitOut)
 {
     const std::string rgTag = so ? so->rgTag() : std::string();
     const uint32_t units = b->paired ? b->n_reads / 2 : b->n_reads;
@@ -386,6 +386,7 @@ bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read
     in.reads = res->reads; in.alns = res->alns; in.edits = res->edits; in.pairs = res->pairs;
     in.khits = P.khits; in.secondary = P.secondary; in.mixed = P.mixed; in.discord = P.discord; in.ssT = ssT; in.colCount = colCount; in.colRecs = colRecs; in.colCap = colCap;
     in.noUnal = so && so->noUnal; in.omitSecSeq = so && so->omitSecSeq; in.rgTag = rgTag.empty() ? NULL : rgTag.c_str();
+    in.unitOut = unitOut;
     Ht2SamFmt F; F.bind(&in);
     if (nth > 64) nth = 64;
     if (nth < 1 || units < 4096) nth = 1;

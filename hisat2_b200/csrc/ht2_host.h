@@ -62,7 +62,7 @@ void ht2_sam_header(std::string& o, const Ht2Image& img, const Ht2SamOutput* so 
 bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read_batch_t* b, const char* names,
                       const ht2gpu_result_batch_t* res, char** out, size_t* out_len, unsigned nthreads, const uint8_t* ssT = NULL,
                       uint32_t* colCount = NULL, struct Ht2SsRec* colRecs = NULL, uint32_t colCap = 0,
-                      const Ht2SamOutput* so = NULL, ht2gpu_align_counts_t* counts = NULL);
+                      const Ht2SamOutput* so = NULL, ht2gpu_align_counts_t* counts = NULL, uint8_t* unitOut = NULL);
 // AlnSink::printAlSumm (aln_sink.h:1613-1816) with canRep = false (mhits is always 0, hisat2.cpp:1882-1884)
 void ht2_format_align_summary(std::string& o, const ht2gpu_align_counts_t& c, bool newStyle, bool discord, bool mixed);
 

@@ -49,22 +49,85 @@ PipeCtx* ctxOf(ht2gpu_handle_t* h, unsigned nth, int nSlots)
     }
     return c;
 }
+
+// Routes records to the read files of ht2gpu_read_routes_t by their units' outcomes.  Each of the nine streams
+// (output x mate) keeps one pending span; a record that continues it extends it, anything else flushes it first, so a
+// run of consecutive records with the same destination reaches the callback as one span straight from the input.
+struct Router {
+    ht2gpu_read_routes_t* R;
+    bool fastq;
+    const char* data[2];             // mate 1 / unpaired, mate 2
+    uint64_t pb[HT2GPU_READS_N * 2], pe[HT2GPU_READS_N * 2];
+    int rc;
+    Router(ht2gpu_read_routes_t* r, bool fq, const char* d1, const char* d2) : R(r), fastq(fq), rc(0)
+    {
+        data[0] = d1; data[1] = d2;
+        for (int k = 0; k < HT2GPU_READS_N * 2; k++) pb[k] = pe[k] = 0;
+    }
+    void flush(int k)
+    {
+        if (pe[k] > pb[k] && rc == 0) {
+            const int which = k >> 1, mate = which < HT2GPU_READS_UN_CONC ? 0 : (k & 1) + 1;
+            R->n_spans++; R->bytes += pe[k] - pb[k];
+            if (R->write(R->ctx, which, mate, data[k & 1] + pb[k], (size_t)(pe[k] - pb[k])) != 0) rc = 1;
+        }
+        pb[k] = pe[k] = 0;
+    }
+    void put(int which, int m, uint64_t b, uint64_t e)   // m: 0 mate 1 / unpaired, 1 mate 2
+    {
+        if (!(R->mask & (1u << which))) return;
+        const int k = which * 2 + m;
+        if (pe[k] != b || pe[k] == pb[k]) { flush(k); pb[k] = b; }
+        pe[k] = e;
+    }
+    // Read::readOrigBuf of record r (rec[r] .. rec[r + 1]): the FASTQ parser keeps the blank lines before the first
+    // record (pat.cpp:867-874), and FileBuf keeps at most LASTN_BUF_SZ = 8192 bytes (filebuf.h:109, 262)
+    void span(const uint64_t* rec, uint64_t i, uint64_t r, uint64_t& b, uint64_t& e) const
+    {
+        b = (fastq && r == 0) ? 0 : rec[i]; e = rec[i + 1];
+        if (e - b > 8192) e = b + 8192;
+    }
+    // units [r0, r0 + n): recA / recB hold the record starts rec[r0 .. r0 + n] of the two inputs
+    void batch(const uint64_t* recA, const uint64_t* recB, uint64_t r0, uint64_t n, const uint8_t* out)
+    {
+        for (uint64_t i = 0; i < n && rc == 0; i++) {
+            const uint8_t o = out[i];
+            uint64_t b1, e1; span(recA, i, r0 + i, b1, e1);
+            if (!recB) { put((o & HT2GPU_OUTCOME_AL1) ? HT2GPU_READS_AL : HT2GPU_READS_UN, 0, b1, e1); continue; }
+            uint64_t b2, e2; span(recB, i, r0 + i, b2, e2);
+            const int conc = (o & HT2GPU_OUTCOME_CONC) ? HT2GPU_READS_AL_CONC : HT2GPU_READS_UN_CONC;
+            put(conc, 0, b1, e1); put(conc, 1, b2, e2);
+            if (o & (HT2GPU_OUTCOME_AL1 | HT2GPU_OUTCOME_AL2)) { put(HT2GPU_READS_AL_CONC_DISC, 0, b1, e1); put(HT2GPU_READS_AL_CONC_DISC, 1, b2, e2); }
+        }
+    }
+    void finish() { for (int k = 0; k < HT2GPU_READS_N * 2; k++) flush(k); }
+};
 }
 
 extern "C" int ht2gpu_run_reads(ht2gpu_handle_t* h, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx, ht2gpu_run_stats_t* st)
 {
-    return ht2gpu_run_reads_multi(&h, 1, in, sink, ctx, st);
+    return ht2gpu_run_reads_routed(&h, 1, in, sink, ctx, NULL, st);
+}
+
+extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
+                                      ht2gpu_run_stats_t* st)
+{
+    return ht2gpu_run_reads_routed(hs, nDev, in, sink, ctx, NULL, st);
 }
 
 // The same pipeline over several devices of one process (hisat2-b200 --gpus N): batch i goes to handle i % n,
 // the sink still receives the batches in input order.  The index is replicated (ht2gpu_open_peer), reads are the
 // only thing that is sharded, no data-path collective.  Context (thread pool, pinned staging) lives in hs[0].
-extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
-                                      ht2gpu_run_stats_t* st)
+// With routes, every device records its units' outcomes and the records of batch i are routed right after its wait.
+extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
+                                       ht2gpu_read_routes_t* routes, ht2gpu_run_stats_t* st)
 {
     if (!hs || nDev < 1 || !in) return HT2GPU_ERR_ARG;
     for (int i = 0; i < nDev; i++) if (!hs[i]) return HT2GPU_ERR_ARG;
     ht2gpu_handle_t* h = hs[0];
+    const bool route = routes && routes->mask;
+    if (route && !routes->write) return HT2GPU_ERR_ARG;
+    if (routes) { routes->n_spans = 0; routes->bytes = 0; routes->s_route = 0; }
     for (int i = 1; i < nDev; i++)
         if (!ht2_same_sam_output(h, hs[i])) { ht2gpu_set_error(h, "ht2gpu_run_reads_multi: the handles' SAM output settings differ"); return HT2GPU_ERR_ARG; }
     ht2gpu_run_stats_t S; memset(&S, 0, sizeof(S));
@@ -82,6 +145,10 @@ extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2g
     std::string err;
     const bool paired = in->path2 != NULL || in->data2 != NULL;
     auto fail = [&](int rc, const std::string& m) { ht2gpu_set_error(h, m.c_str()); ht2_source_close(a); ht2_source_close(b); if (st) *st = S; return rc; };
+    if (route) for (int i = 0; i < nDev; i++) { const int rc = ht2gpu_record_outcomes(hs[i], 1); if (rc) return fail(rc, ht2gpu_last_error(hs[i])); }
+    // the record starts of each submitted batch (the producer keeps appending to the sources' indexes meanwhile)
+    struct SlotRecs { uint64_t r0; std::vector<uint64_t> a, b; };
+    std::vector<SlotRecs> recs(route ? (size_t)nSlots : 0);
     if (in->path1) { if (!ht2_source_open(a, in->path1, err)) return fail(HT2GPU_ERR_ARG, err); }
     else if (in->data1) ht2_source_memory(a, in->data1, in->len1);
     else return fail(HT2GPU_ERR_ARG, "ht2gpu_run_reads: no input");
@@ -137,6 +204,12 @@ extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2g
                 if (!ht2_parse_batch(a, paired ? &b : NULL, r, q1, ro, stage[slot], pool, C->scratch, e)) rc = HT2GPU_ERR_ARG;
                 parseS += nowS() - tp;
             }
+            if (rc == HT2GPU_OK && route) {
+                SlotRecs& sr = recs[slot];
+                sr.r0 = r;
+                sr.a.assign(a.rec.begin() + (ptrdiff_t)r, a.rec.begin() + (ptrdiff_t)q1 + 1);
+                if (paired) sr.b.assign(b.rec.begin() + (ptrdiff_t)r, b.rec.begin() + (ptrdiff_t)q1 + 1);
+            }
             if (rc == HT2GPU_OK) {
                 Ht2HostBatch& hb = stage[slot];
                 ht2gpu_read_batch_t rb; memset(&rb, 0, sizeof(rb));
@@ -158,6 +231,8 @@ extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2g
     });
 
     int rc = HT2GPU_OK;
+    double routeS = 0;
+    Router router(routes, fastq, a.data, b.data);
     for (uint64_t i = 0; ; i++) {
         const int slot = (int)(i % (uint64_t)nSlots);
         {
@@ -176,11 +251,31 @@ extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2g
         const double tk = nowS();
         if (sink && r.sam_len) { if (sink(ctx, r.sam, r.sam_len) != 0) { rc = HT2GPU_ERR_ARG; prodErr = "the SAM sink reported an error"; } }
         sinkS += nowS() - tk;
+        if (route && rc == HT2GPU_OK) {
+            const double tr = nowS();
+            const uint8_t* ob = NULL; uint32_t nu = 0;
+            rc = ht2gpu_unit_outcomes(hs[slot % nDev], slot / nDev, &ob, &nu);
+            if (rc != HT2GPU_OK) prodErr = ht2gpu_last_error(hs[slot % nDev]);
+            else {
+                const SlotRecs& sr = recs[slot];
+                router.batch(sr.a.data(), paired ? sr.b.data() : NULL, sr.r0, nu, ob);
+                if (router.rc) { rc = HT2GPU_ERR_ARG; prodErr = "the read-file writer reported an error"; }
+            }
+            routeS += nowS() - tr;
+        }
         { std::lock_guard<std::mutex> lk(mu); state[slot] = 0; if (rc != HT2GPU_OK) prodRc = rc; cv.notify_all(); }
         if (rc != HT2GPU_OK) break;
     }
     { std::lock_guard<std::mutex> lk(mu); if (rc != HT2GPU_OK && prodRc == HT2GPU_OK) prodRc = rc; cv.notify_all(); }
     producer.join();
+    if (route) {
+        const double tr = nowS();
+        router.finish();
+        if (router.rc && rc == HT2GPU_OK) { rc = HT2GPU_ERR_ARG; prodErr = "the read-file writer reported an error"; }
+        routeS += nowS() - tr;
+        routes->s_route = routeS;
+        for (int i = 0; i < nDev; i++) ht2gpu_record_outcomes(hs[i], 0);
+    }
     // drain anything still in flight after an error
     if (rc != HT2GPU_OK) for (int s = 0; s < nSlots; s++) if (state[s] == 1) { ht2gpu_sam_result_t r; ht2gpu_wait_sam(hs[s % nDev], s / nDev, &r); }
     ht2_source_close(a); ht2_source_close(b);
@@ -228,6 +323,47 @@ extern "C" int ht2gpu_parse_reads(const ht2gpu_reads_input_t* in, ht2gpu_parsed_
     out->names = hb->names; out->name_offs = hb->nameOffs; out->names_bytes = hb->namesBytes; out->priv = hb;
     return HT2GPU_OK;
 }
+// Host-only routing of a whole input by given outcomes (ht2gpu_unit_outcomes of callers that batch for themselves).
+extern "C" int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t* outcomes, uint64_t n_units, ht2gpu_read_routes_t* routes,
+                                  char* errbuf, size_t errbuf_len)
+{
+    if (!in || !routes || (n_units && !outcomes) || (routes->mask && !routes->write)) return HT2GPU_ERR_ARG;
+    routes->n_spans = 0; routes->bytes = 0; routes->s_route = 0;
+    auto fail = [&](const std::string& m) { if (errbuf && errbuf_len) { strncpy(errbuf, m.c_str(), errbuf_len - 1); errbuf[errbuf_len - 1] = 0; } return HT2GPU_ERR_ARG; };
+    const double t0 = nowS();
+    unsigned nth = in->threads > 0 ? (unsigned)in->threads : std::thread::hardware_concurrency();
+    if (nth < 1) nth = 1;
+    if (nth > 64) nth = 64;
+    Ht2ThreadPool pool(nth);
+    Ht2ReadSource a, b;
+    std::string err;
+    const bool paired = in->path2 != NULL || in->data2 != NULL;
+    if (in->path1) { if (!ht2_source_open(a, in->path1, err)) return fail(err); }
+    else if (in->data1) ht2_source_memory(a, in->data1, in->len1);
+    else return fail("no input");
+    if (in->path2) { if (!ht2_source_open(b, in->path2, err)) { ht2_source_close(a); return fail(err); } }
+    else if (in->data2) ht2_source_memory(b, in->data2, in->len2);
+    const bool fastq = in->format == 1;
+    bool ok = ht2_source_index(a, fastq, pool, err) && (!paired || ht2_source_index(b, fastq, pool, err));
+    if (ok && paired && a.nRecords() != b.nRecords()) { ok = false; err = "mate files have different numbers of reads"; }
+    uint64_t r0 = in->skip, r1 = a.nRecords();
+    if (r0 > r1) r0 = r1;
+    if (in->upto && r0 + in->upto < r1) r1 = r0 + in->upto;
+    if (ok && r1 - r0 != n_units) { ok = false; err = "the outcomes do not cover the input's " + std::to_string(r1 - r0) + " units"; }
+    int rc = HT2GPU_OK;
+    if (ok && routes->mask) {
+        Router router(routes, fastq, a.data, b.data);
+        router.batch(a.rec.data() + r0, paired ? b.rec.data() + r0 : NULL, r0, r1 - r0, outcomes);
+        router.finish();
+        if (router.rc) { rc = HT2GPU_ERR_ARG; err = "the read-file writer reported an error"; }
+    }
+    ht2_source_close(a); ht2_source_close(b);
+    routes->s_route = nowS() - t0;
+    if (!ok) return fail(err);
+    if (rc) return fail(err);
+    return HT2GPU_OK;
+}
+
 extern "C" void ht2gpu_free_parsed(ht2gpu_parsed_reads_t* p)
 {
     if (p && p->priv) { Ht2HostBatch* hb = (Ht2HostBatch*)p->priv; hb->freeAll(); delete hb; p->priv = NULL; }

@@ -47,6 +47,7 @@ struct Ht2SamIn {
     uint32_t        noUnal;      // --no-unal: appendMate prints nothing for rs == NULL (aln_sink.h:3040)
     uint32_t        omitSecSeq;  // --omit-sec-seq: SEQ / QUAL '*' in non-primary records (aln_sink.h:3190-3215)
     const char*     rgTag;       // "RG:Z:<id>" or NULL (sam.h:780, 1102)
+    uint8_t*        unitOut;     // ht2gpu_record_outcomes: the counting pass stores each unit's HT2GPU_OUTCOME_* bits here, or NULL
 };
 
 // ReportingMetrics (aln_sink.h:2007-2346) of the units a formatter pass went through, in the field order of
@@ -55,7 +56,7 @@ struct Ht2SamIn {
 // they are not kept.
 enum { HT2_T_NREAD, HT2_T_NPAIRED, HT2_T_NUNPAIRED, HT2_T_NCONCORD_0, HT2_T_NCONCORD_UNI1, HT2_T_NCONCORD_UNI2, HT2_T_NDISCORD,
        HT2_T_NUNP_0_0, HT2_T_NUNP_0_UNI1, HT2_T_NUNP_0_UNI2, HT2_T_NUNP_0, HT2_T_NUNP_UNI1, HT2_T_NUNP_UNI2, HT2_T_N };
-struct Ht2SamTally { uint32_t c[HT2_T_N]; };
+struct Ht2SamTally { uint32_t c[HT2_T_N]; uint32_t outcome; };   // outcome: the last unit's HT2GPU_OUTCOME_* bits
 static_assert(sizeof(ht2gpu_align_counts_t) == HT2_T_N * sizeof(uint64_t), "ht2gpu_align_counts_t follows the tally's order");
 
 // Where a pass's text goes: p + n (WRITE) or only the byte count n (the counting pass).  Ht2SamFmt::unit formats
@@ -907,7 +908,7 @@ struct Ht2SamFmt {
         const uint64_t nunpair1 = n < in->khits ? n : in->khits;   // ReportingState::getReport
         Ht2SamSumm summ; summ.reset();
         Ht2SamFlags fl = {HT2_PAIR_UNPAIRED, true, false};
-        if (t) { t->c[HT2_T_NREAD]++; t->c[HT2_T_NUNPAIRED]++; }
+        if (t) { t->c[HT2_T_NREAD]++; t->c[HT2_T_NUNPAIRED]++; t->outcome = nunpair1 > 0 ? HT2GPU_OUTCOME_AL1 : 0; }
         if (nunpair1 > 0) {
             addUnp(summ, 0, rs, n, rd.len);
             uint16_t sel[HT2_SAM_MAXSEL];
@@ -959,7 +960,10 @@ struct Ht2SamFmt {
             addUnp(summ, 0, rs1u, n1, rd1.len); addUnp(summ, 1, rs2u, n2, rd2.len);
             const uint32_t nsel = selectByScore(rs1u, n1, rd1.len, rs2u, rd2.len, pairs, np, true, nconcord, sel, rnd);
             summ.numAlnsPaired = nsel;
-            if (t) { t->c[HT2_T_NCONCORD_UNI1] += (uint32_t)(nsel == 1); t->c[HT2_T_NCONCORD_UNI2] += (uint32_t)(nsel != 1); }   // select1_.size(), aln_sink.h:2100-2110
+            if (t) {   // select1_.size(), aln_sink.h:2100-2110
+                t->c[HT2_T_NCONCORD_UNI1] += (uint32_t)(nsel == 1); t->c[HT2_T_NCONCORD_UNI2] += (uint32_t)(nsel != 1);
+                t->outcome = HT2GPU_OUTCOME_AL1 | HT2GPU_OUTCOME_AL2 | HT2GPU_OUTCOME_CONC;
+            }
             Ht2SamFlags fl1 = {HT2_PAIR_CONCORD_MATE1, true, true}, fl2 = {HT2_PAIR_CONCORD_MATE2, true, true};
             for (uint32_t i = 0; i < nsel; i++) {
                 const ht2gpu_aln_t& a = rs1u[pairs[2 * sel[i]]]; const ht2gpu_aln_t& b = rs2u[pairs[2 * sel[i] + 1]];
@@ -969,7 +973,7 @@ struct Ht2SamFmt {
             }
             return;
         } else if (discordant) {
-            if (t) { t->c[HT2_T_NCONCORD_0]++; t->c[HT2_T_NDISCORD]++; }   // aln_sink.h:2191-2192
+            if (t) { t->c[HT2_T_NCONCORD_0]++; t->c[HT2_T_NDISCORD]++; t->outcome = HT2GPU_OUTCOME_AL1 | HT2GPU_OUTCOME_AL2; }   // aln_sink.h:2191-2192
             Ht2SamSumm summ; summ.reset();
             summ.paired = true;
             const ht2gpu_aln_t& a = rs1u[0]; const ht2gpu_aln_t& b = rs2u[0];
@@ -1014,6 +1018,7 @@ struct Ht2SamFmt {
             t->c[HT2_T_NUNP_0_0] += (uint32_t)!rep1 + (uint32_t)!rep2;
             t->c[HT2_T_NUNP_0_UNI1] += (uint32_t)(rep1 && nsel1 == 1) + (uint32_t)(rep2 && nsel2 == 1);
             t->c[HT2_T_NUNP_0_UNI2] += (uint32_t)(rep1 && nsel1 != 1) + (uint32_t)(rep2 && nsel2 != 1);
+            t->outcome = (rep1 ? HT2GPU_OUTCOME_AL1 : 0) | (rep2 ? HT2GPU_OUTCOME_AL2 : 0);
         }
         Ht2SamFlags fl1 = {HT2_PAIR_UNPAIRED_MATE1, true, repRs2 != NULL}, fl2 = {HT2_PAIR_UNPAIRED_MATE2, true, repRs1 != NULL};
         int64_t refid = -1, refoff = -1;
@@ -1062,6 +1067,7 @@ struct Ht2SamFmt {
     template <bool W> HT2_HD void unit(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t = NULL) const {
         Ht2SamCur<W> c = {W ? o.p + o.n : NULL, 0};
         if (in->paired) finishPaired(c, u, t); else finishUnpaired(c, u, t);
+        if (t && in->unitOut) in->unitOut[u] = (uint8_t)t->outcome;
         o.n += c.n;
     }
 };

@@ -248,6 +248,43 @@ int ht2gpu_run_reads(ht2gpu_handle_t* h, const ht2gpu_reads_input_t* in, ht2gpu_
  * SAM output settings (ht2gpu_set_sam_output) differ are refused with HT2GPU_ERR_ARG. */
 int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int n, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
                            ht2gpu_run_stats_t* stats);
+
+/* ---- reads routed to files by their outcome (--un, --al, --un-conc, --al-conc, --al-conc-disc) -----------------
+ * The hisat2 wrapper's read files (hisat2:546-650), decided from the same choices that set the SAM FLAGs of each read's
+ * primary records.  With ht2gpu_record_outcomes(h, 1) the SAM counting pass stores one byte per unit (read or pair);
+ * ht2gpu_unit_outcomes hands back the bytes of the slot's last ht2gpu_wait_sam (valid until the next submit on that
+ * slot).  Off by default, and refused while a batch is in flight. */
+#define HT2GPU_OUTCOME_AL1  1   /* mate 1 / the unpaired read has an alignment (its primary record has FLAG & 4 clear) */
+#define HT2GPU_OUTCOME_AL2  2   /* mate 2 has an alignment */
+#define HT2GPU_OUTCOME_CONC 4   /* the primary records are concordant (FLAG & 2) */
+int ht2gpu_record_outcomes(ht2gpu_handle_t* h, int enable);
+int ht2gpu_unit_outcomes(ht2gpu_handle_t* h, int slot, const uint8_t** bytes, uint32_t* n_units);
+
+/* The five outputs; bit (1 << which) of ht2gpu_read_routes_t.mask selects one.  Unpaired reads go to UN / AL, pairs to
+ * UN_CONC / AL_CONC (mate 1 and mate 2 to separate files) and AL_CONC_DISC (both mates of every pair with at least
+ * one aligned mate).  write receives the records' original input text, runs of consecutive records with the same
+ * destination as one span straight from the input (mate 0 = unpaired, 1 / 2); it returns 0 to continue.  What is
+ * written is what the reference's parser keeps of a record (Read::readOrigBuf): the bytes from its '>' / '@' up to
+ * the next record's, with the blank lines before the first FASTQ record, and at most its first 8192 bytes. */
+enum { HT2GPU_READS_UN = 0, HT2GPU_READS_AL, HT2GPU_READS_UN_CONC, HT2GPU_READS_AL_CONC, HT2GPU_READS_AL_CONC_DISC, HT2GPU_READS_N };
+typedef int (*ht2gpu_reads_fn)(void* ctx, int which, int mate, const char* data, size_t len);
+typedef struct {
+    uint32_t        mask;
+    ht2gpu_reads_fn write;
+    void*           ctx;
+    /* filled by the call */
+    uint64_t        n_spans, bytes;
+    double          s_route;        /* host wall clock spent routing, write calls included */
+} ht2gpu_read_routes_t;
+/* ht2gpu_run_reads_multi that also routes every batch's records by their outcomes, in read order; routes = NULL or a
+ * zero mask is ht2gpu_run_reads_multi. */
+int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int n, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
+                            ht2gpu_read_routes_t* routes, ht2gpu_run_stats_t* stats);
+/* Host only (no device): route the records of an input (after -s / -u) by outcomes[0 .. n_units), e.g. the bytes of
+ * ht2gpu_unit_outcomes of callers that batch through ht2gpu_align_sam.  n_units must equal the input's units. */
+int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t* outcomes, uint64_t n_units, ht2gpu_read_routes_t* routes,
+                       char* errbuf, size_t errbuf_len);
+
 /* Replicate an open index onto another device of this process: the packed image is copied device to device
  * (cudaMemcpyPeer: NVLink / NVSwitch when peer access exists), options as given (opt->device = the target). */
 int ht2gpu_open_peer(const ht2gpu_handle_t* src, const ht2gpu_options_t* opt, ht2gpu_handle_t** out);
