@@ -490,7 +490,9 @@ HT2_HD int64_t ht2_intron_pen(int intronlen) {
 // NOSPL = true compiles the aligner for --no-spliced-alignment only: every spliced branch (the spliced join of
 // combineWith, splice scoring, intron windows) becomes dead code.  The pool kernel is bound by instruction fetch
 // (DESIGN.md 4.1), so the DNA configuration gets its own, smaller instantiation; NOSPL = false reads the option.
-template <bool GRAPH, bool NOSPL = false>
+// DP = false likewise compiles it for a run without --bowtie2-dp: TS_HYB_DP is never entered, so the dynamic-programming
+// extension of ht2_sw.h (frame, fill, backtrace) is dead code; DP = true reads the option.
+template <bool GRAPH, bool NOSPL = false, bool DP = true>
 struct Ht2AlignerT {
     HT2_HD bool noSpl() const { return NOSPL ? true : (P->noSplicedAlignment != 0); }
     const uint8_t*        blob;
@@ -600,7 +602,7 @@ struct Ht2AlignerT {
             else ed[i].pos = (uint32_t)(sz - ed[i].pos - 1);
         }
     }
-    HT2_HD Ht2Hit* poolAlloc() {
+    HT2_NI Ht2Hit* poolAlloc() {
         if (W->poolTop >= HT2_POOL) { W->err |= HT2_ERR_POOL; return &W->pool[HT2_POOL - 1]; }
         HT2_HIWATER(maxPool, W->poolTop + 1);
         return &W->pool[W->poolTop++];
@@ -1972,7 +1974,7 @@ struct Ht2AlignerT {
 
     // ---- policy --------------------------------------------------------------
     // ReadBWTHit::searchScore (hi_aligner.h:321-334)
-    HT2_HD int64_t searchScore(const Ht2ReadHits& h) const {
+    HT2_NI int64_t searchScore(const Ht2ReadHits& h) const {
         int64_t score = 0;
         const int64_t penaltyPerOffset = (int64_t)P->minK * P->minK;
         for (uint32_t i = 0; i < h.nhits; i++) { uint32_t len = h.hits[i].len; score += (int64_t)(uint32_t)(len * len); }
@@ -2155,7 +2157,7 @@ struct Ht2AlignerT {
     HT2_NI bool peConcordant(int64_t off1, uint32_t len1, bool fw1, int64_t off2, uint32_t len2, bool fw2) const;
     HT2_NI void alignMateAnchors(uint32_t rdi, bool fw, uint32_t tidx, uint32_t toff);
     // explicit-stack formulation (ht2_machine.h)
-    HT2_HD void pushFrame(uint32_t rdi, const Ht2Hit* hit, uint32_t hitoff, uint32_t hitlen, bool alignMate, uint32_t dep);
+    HT2_NI void pushFrame(uint32_t rdi, const Ht2Hit* hit, uint32_t hitoff, uint32_t hitlen, bool alignMate, uint32_t dep);
     HT2_NI void runFrame();
     HT2_NI void runTop();
     HT2_HD void machineStart();

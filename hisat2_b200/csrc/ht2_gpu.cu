@@ -73,7 +73,7 @@ __device__ __forceinline__ uint32_t ht2_comp4(uint32_t x)
 // Read i of the batch into the workspace: forward and reverse-complement bases, forward and reversed qualities
 // (Read::finalize, read.h:84-92).  Word-wise: one lane loads a whole read, so byte accesses (404 byte stores and
 // 202 byte loads per 101-bp read) made this the most expensive glue state of the kernel.
-__device__ __forceinline__ void ht2_load_read(Ht2Read& dst, const DevBatch& b, uint32_t ri, uint32_t& err)
+__device__ __noinline__ void ht2_load_read(Ht2Read& dst, const DevBatch& b, uint32_t ri, uint32_t& err)
 {
     uint64_t o0 = b.offs[ri], o1 = b.offs[ri + 1];
     uint32_t n = (uint32_t)(o1 - o0);
@@ -272,8 +272,8 @@ __device__ __forceinline__ uint32_t rg_code(const Ht2Work* W)
 // fills the score planes of one problem after the other (ht2_sw.h swFillCoop: a 64-row vector per column instead of
 // a lone lane's 2), and the lanes go back to their own candidates / backtraces (swExtendAnchor -> swFinish).  Run by
 // the pool kernel and by ht2gpu_sw_extend's harness; all 32 lanes must call it.
-template <bool GRAPH, bool NOSPL>
-__device__ __forceinline__ void ht2_dp_round(Ht2AlignerT<GRAPH, NOSPL>& A, Ht2Work* base, int my, uint32_t lane)
+template <bool GRAPH, bool NOSPL, bool DP>
+__device__ __forceinline__ void ht2_dp_round(Ht2AlignerT<GRAPH, NOSPL, DP>& A, Ht2Work* base, int my, uint32_t lane)
 {
     bool fill = false;
     if (my >= 0) {
@@ -310,9 +310,11 @@ __device__ __forceinline__ void ht2_dp_round(Ht2AlignerT<GRAPH, NOSPL>& A, Ht2Wo
 // of an SM execute the same code most of the time (instruction fetch is the scarce resource: the L1.5 I-cache and
 // the GPC instruction cache saturate when every warp walks different code) while groups are drawn from a pool
 // large enough to fill all 32 lanes.
+// One block per SM is the design point and is stated in the launch bounds: without it ptxas stops at 128 registers
+// and spills (DESIGN.md 4.1).
 // ---------------------------------------------------------------------------
-template <int NW, int K, bool GRAPH, bool NOSPL>
-__global__ void __launch_bounds__(32 * NW)
+template <int NW, int K, bool GRAPH, bool NOSPL, bool DP>
+__global__ void __launch_bounds__(32 * NW, 1)
 ht2_align_pool_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatch b, DevOut o, Ht2Work* work)
 {
     constexpr int S = NW * 32 * K;      // slots of this block
@@ -328,7 +330,7 @@ ht2_align_pool_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatc
     for (int i = t; i < RG_BINS * NWORD; i += 32 * NW) sBits[i / NWORD][i % NWORD] = (i / NWORD == (int)RG_NEED) ? 0xffffffffu : 0u;
     if (t < RG_BINS) sCount[t] = (t == RG_NEED) ? S : 0;
     if (t == 0) { sTarget = RG_NEED; sExit = 0; }
-    Ht2AlignerT<GRAPH, NOSPL> A;
+    Ht2AlignerT<GRAPH, NOSPL, DP> A;
     A.bind(blob, &P, base);
     A.sw = b.sw ? b.sw + ((size_t)blockIdx.x * blockDim.x + threadIdx.x) : NULL;
     A.swPl = b.swPool ? b.swPool + ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * (size_t)HT2_SW_POOL_WORDS : NULL;
@@ -403,9 +405,7 @@ ht2_align_pool_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatc
         }
         __threadfence_block();   // acquire: the previous owner's workspace writes
         const long long t0 = o.stats ? clock64() : 0;
-#ifndef HT2_NO_DP
-        if (T == RG_TOP + TS_HYB_DP) ht2_dp_round(A, base, my, lane);
-#endif
+        if (DP && T == RG_TOP + TS_HYB_DP) ht2_dp_round(A, base, my, lane);
         if (my >= 0) {
             Ht2Work* W = base + my;
             uint32_t nc;
@@ -877,8 +877,8 @@ static int finishOpen(ht2gpu_handle* h)
         // known call tree; graph indexes recurse through alignWithALTs (ht2_alt.h, depth <= HT2_ALT_MAXDEP).
         size_t need = 0;
         cudaFuncAttributes fa;
-        if (h->graph) { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, true, false>)); need = fa.localSizeBytes + 36 * 1024; }
-        else { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, false, false>)); need = fa.localSizeBytes + 4 * 1024; }
+        if (h->graph) { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, true, false, true>)); need = fa.localSizeBytes + 36 * 1024; }
+        else { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, false, false, true>)); need = fa.localSizeBytes + 4 * 1024; }
         CK(cudaFuncGetAttributes(&fa, ht2_sam_kernel<true>));
         if (fa.localSizeBytes + 2048 > need) need = fa.localSizeBytes + 2048;
         // the writing pass's staging buffer: what leaves room for HT2_SAM_STAGE_BLOCKS blocks per SM (1 KB of every
@@ -1168,22 +1168,27 @@ static int launchAlign(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* 
     if (evStart) CK(cudaEventRecord(evStart, S.stream));   // kernel time is counted from here: after the waits for the previous kernels
     Ht2Work* work = wp->dWork;
     const bool nospl = h->P.noSplicedAlignment != 0;   // the DNA-only instantiation has less code (DESIGN.md 4.1)
+    const bool dp = h->P.bowtie2Dp != 0;               // and so has the one without the --bowtie2-dp extension, built for the DNA-only linear kernels
+#define HT2_POOL_LAUNCH(NW, K, GRAPH, NOSPL, DP, TPB) ht2_align_pool_kernel<NW, K, GRAPH, NOSPL, DP><<<grid, TPB, 0, S.stream>>>(h->dBlob, h->P, db, o, work)
     if (h->graph) {
-        if (nospl) ht2_align_pool_kernel<8, 4, true, true><<<grid, 256, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
-        else ht2_align_pool_kernel<8, 4, true, false><<<grid, 256, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
+        if (nospl) HT2_POOL_LAUNCH(8, 4, true, true, true, 256);
+        else HT2_POOL_LAUNCH(8, 4, true, false, true, 256);
     } else {
         switch (h->poolWarps * 100 + h->rgK) {
             case 802:
-                if (nospl) ht2_align_pool_kernel<8, 2, false, true><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
-                else ht2_align_pool_kernel<8, 2, false, false><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
+                if (!nospl) HT2_POOL_LAUNCH(8, 2, false, false, true, h->tpb);
+                else if (dp) HT2_POOL_LAUNCH(8, 2, false, true, true, h->tpb);
+                else HT2_POOL_LAUNCH(8, 2, false, true, false, h->tpb);
                 break;
-            case 408:  ht2_align_pool_kernel<4, 8, false, false><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work); break;
+            case 408:  HT2_POOL_LAUNCH(4, 8, false, false, true, h->tpb); break;
             default:
-                if (nospl) ht2_align_pool_kernel<8, 4, false, true><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
-                else ht2_align_pool_kernel<8, 4, false, false><<<grid, h->tpb, 0, S.stream>>>(h->dBlob, h->P, db, o, work);
+                if (!nospl) HT2_POOL_LAUNCH(8, 4, false, false, true, h->tpb);
+                else if (dp) HT2_POOL_LAUNCH(8, 4, false, true, true, h->tpb);
+                else HT2_POOL_LAUNCH(8, 4, false, true, false, h->tpb);
                 break;
         }
     }
+#undef HT2_POOL_LAUNCH
     CK(cudaGetLastError());
     return HT2GPU_OK;
 }

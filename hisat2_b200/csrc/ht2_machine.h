@@ -36,7 +36,7 @@ enum {
 };
 
 // push a child frame (== a recursive call of hybridSearch_recur)
-template <bool GRAPH, bool NOSPL> HT2_HD void Ht2AlignerT<GRAPH, NOSPL>::pushFrame(uint32_t rdi, const Ht2Hit* hit, uint32_t hitoff, uint32_t hitlen, bool alignMate, uint32_t dep)
+template <bool GRAPH, bool NOSPL, bool DP> HT2_NI void Ht2AlignerT<GRAPH, NOSPL, DP>::pushFrame(uint32_t rdi, const Ht2Hit* hit, uint32_t hitoff, uint32_t hitlen, bool alignMate, uint32_t dep)
 {
     if (W->nFrames >= HT2_DEPTH_CAP) { W->err |= HT2_ERR_DEPTH; W->childRet = HT2_MIN_I64; return; }
     Ht2Frame& f = W->frames[W->nFrames++];
@@ -44,7 +44,7 @@ template <bool GRAPH, bool NOSPL> HT2_HD void Ht2AlignerT<GRAPH, NOSPL>::pushFra
 }
 
 // One segment of one hybridSearch_recur activation.
-template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runFrame()
+template <bool GRAPH, bool NOSPL, bool DP> HT2_NI void Ht2AlignerT<GRAPH, NOSPL, DP>::runFrame()
 {
     Ht2Frame& f = W->frames[W->nFrames - 1];
     const uint32_t rdi = f.rdi;
@@ -789,7 +789,7 @@ template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runFram
 }
 
 // One segment of the top-level control (go / nextBWT / align / hybridSearch / alignMate).
-template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runTop()
+template <bool GRAPH, bool NOSPL, bool DP> HT2_NI void Ht2AlignerT<GRAPH, NOSPL, DP>::runTop()
 {
     switch (W->st) {
     case TS_START: {
@@ -907,8 +907,7 @@ template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runTop(
     case TS_HYB_RET: {
         // --bowtie2-dp: dynamic programming around the anchor, then one more recursion on the
         // full-length hit (spliced_aligner.h:209-320)
-#ifndef HT2_NO_DP
-        if (P->bowtie2Dp == 2 || (P->bowtie2Dp == 1 && W->childRet < minsc[W->curRdi])) {
+        if (DP && (P->bowtie2Dp == 2 || (P->bowtie2Dp == 1 && W->childRet < minsc[W->curRdi]))) {
             Ht2Hit& gh = W->genomeHits[W->hybHj];
             if (!W->err) {
                 if (gh.len < W->rd[W->curRdi].len) { W->st = TS_HYB_DP; break; }   // a DP problem: its own heavy state, so that
@@ -918,7 +917,6 @@ template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runTop(
                 break;
             }
         }
-#endif
         W->genomeHitsDone[W->hybHj] = 1;
         W->hybIter++;
         W->st = TS_HYB_PICK;
@@ -926,7 +924,7 @@ template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runTop(
     }
     case TS_HYB_DP: {
         Ht2Hit& gh = W->genomeHits[W->hybHj];
-        if (swExtendAnchor(W->curRdi, gh)) {
+        if (DP && swExtendAnchor(W->curRdi, gh)) {
             W->st = TS_HYB_DP_RET;
             pushFrame(W->curRdi, &gh, gh.rdoff, gh.len, false, 0);
             break;
@@ -1000,9 +998,9 @@ template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::runTop(
 }
 
 // Run one read (pair) to completion (host build and the one-lane-per-read kernel loop).
-template <bool GRAPH, bool NOSPL> HT2_HD void Ht2AlignerT<GRAPH, NOSPL>::machineStart() { W->st = TS_START; W->nFrames = 0; W->psCont = 0; W->psG.active = 0; }
-template <bool GRAPH, bool NOSPL> HT2_HD bool Ht2AlignerT<GRAPH, NOSPL>::machineDone() const { return W->st == TS_DONE && W->nFrames == 0; }
-template <bool GRAPH, bool NOSPL> HT2_HD void Ht2AlignerT<GRAPH, NOSPL>::machineStep()
+template <bool GRAPH, bool NOSPL, bool DP> HT2_HD void Ht2AlignerT<GRAPH, NOSPL, DP>::machineStart() { W->st = TS_START; W->nFrames = 0; W->psCont = 0; W->psG.active = 0; }
+template <bool GRAPH, bool NOSPL, bool DP> HT2_HD bool Ht2AlignerT<GRAPH, NOSPL, DP>::machineDone() const { return W->st == TS_DONE && W->nFrames == 0; }
+template <bool GRAPH, bool NOSPL, bool DP> HT2_HD void Ht2AlignerT<GRAPH, NOSPL, DP>::machineStep()
 {
     if (W->nFrames > 0) runFrame();
     else runTop();
@@ -1010,7 +1008,7 @@ template <bool GRAPH, bool NOSPL> HT2_HD void Ht2AlignerT<GRAPH, NOSPL>::machine
 // "Heavy" states are the ones worth regrouping lanes for (index searches,
 // reference extension, combine); everything else is short glue that is chained
 // onto the end of the previous segment.
-template <bool GRAPH, bool NOSPL> HT2_HD bool Ht2AlignerT<GRAPH, NOSPL>::machineAtHeavyState() const
+template <bool GRAPH, bool NOSPL, bool DP> HT2_HD bool Ht2AlignerT<GRAPH, NOSPL, DP>::machineAtHeavyState() const
 {
     if (W->nFrames > 0) {
         switch (W->frames[W->nFrames - 1].pc) {
@@ -1028,7 +1026,7 @@ template <bool GRAPH, bool NOSPL> HT2_HD bool Ht2AlignerT<GRAPH, NOSPL>::machine
     }
 }
 // run one heavy segment plus the glue that follows it
-template <bool GRAPH, bool NOSPL> HT2_HD void Ht2AlignerT<GRAPH, NOSPL>::machineRun()
+template <bool GRAPH, bool NOSPL, bool DP> HT2_HD void Ht2AlignerT<GRAPH, NOSPL, DP>::machineRun()
 {
     do { machineStep(); } while (!machineAtHeavyState());
 }

@@ -6,7 +6,7 @@
 // PairedEndPolicy::peClassifyPair (pe.cpp:38-132) with the hisat2 defaults
 // olapOk = containOk = expandToFit = true, dovetailOk = false (hisat2.cpp:348-352).
 // Returns true iff the pair is NOT discordant.
-template <bool GRAPH, bool NOSPL> HT2_NI bool Ht2AlignerT<GRAPH, NOSPL>::peConcordant(int64_t off1, uint32_t len1, bool fw1, int64_t off2, uint32_t len2, bool fw2) const
+template <bool GRAPH, bool NOSPL, bool DP> HT2_NI bool Ht2AlignerT<GRAPH, NOSPL, DP>::peConcordant(int64_t off1, uint32_t len1, bool fw1, int64_t off2, uint32_t len2, bool fw2) const
 {
     uint32_t maxfrag = P->maxFrag;
     if (len1 > maxfrag) maxfrag = len1;
@@ -37,7 +37,7 @@ template <bool GRAPH, bool NOSPL> HT2_NI bool Ht2AlignerT<GRAPH, NOSPL>::peConco
 
 // HI_Aligner::pairReads (hi_aligner.h:5948-6057) + AlnSinkWrap::report for a
 // pair (aln_sink.h:2565-2611) + ReportingState::foundConcordant (aln_sink.cpp:72-92).
-template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::pairReads()
+template <bool GRAPH, bool NOSPL, bool DP> HT2_NI void Ht2AlignerT<GRAPH, NOSPL, DP>::pairReads()
 {
     const uint32_t n1 = W->nRes[0], n2 = W->nRes[1];
     uint32_t start_i = W->concordInspected[0], start_j = W->concordInspected[1];
@@ -96,7 +96,7 @@ template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::pairRea
 }
 
 // anchor search part of alignMate (hi_aligner.h:5600-5717): fills W->genomeHits
-template <bool GRAPH, bool NOSPL> HT2_NI void Ht2AlignerT<GRAPH, NOSPL>::alignMateAnchors(uint32_t rdi, bool fw, uint32_t tidx, uint32_t toff)
+template <bool GRAPH, bool NOSPL, bool DP> HT2_NI void Ht2AlignerT<GRAPH, NOSPL, DP>::alignMateAnchors(uint32_t rdi, bool fw, uint32_t tidx, uint32_t toff)
 {
     const uint32_t ordi = 1 - rdi;
     const bool ofw = (fw == (P->gMate2fw != 0)) ? (P->gMate1fw != 0) : (P->gMate2fw != 0);
