@@ -171,8 +171,41 @@ EXPORTS = [
     "ht2gpu_ctx_get", "ht2gpu_ctx_set", "ht2gpu_run_reads_multi", "ht2gpu_open_peer", "ht2gpu_sw_selftest", "ht2gpu_load_splicesites", "ht2gpu_collect_splicesites",
     "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry", "ht2gpu_set_sam_output", "ht2gpu_align_counts",
     "ht2gpu_format_align_summary", "ht2gpu_sw_extend", "ht2gpu_record_outcomes", "ht2gpu_unit_outcomes",
-    "ht2gpu_run_reads_routed", "ht2gpu_route_reads",
+    "ht2gpu_run_reads_routed", "ht2gpu_route_reads", "ht2gpu_gunzip", "ht2gpu_gunzip_error", "ht2gpu_run_gunzip_stats",
 ]
+
+
+class CGunzipOpts(C.Structure):
+    _fields_ = [("chunk_bytes", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class CGunzipStats(C.Structure):
+    _fields_ = ([(n, C.c_uint64) for n in ("in_bytes", "out_bytes", "members", "blocks", "chunks", "chunks_confirmed",
+                                            "chunks_merged_no_candidate", "chunks_merged_false_positive", "windows",
+                                            "decode_rounds", "windows_cut", "peak_device_bytes")]
+                + [("chunk_bytes", C.c_uint32), ("pad", C.c_uint32)]
+                + [(n, C.c_float) for n in ("ms_find", "ms_decode", "ms_window", "ms_replace", "ms_crc", "ms_copy")])
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "pad"}
+
+
+def gunzip(data_or_path, device=0, chunk_bytes=0):
+    """ht2gpu_gunzip: a whole gzip file (bytes, or a path) inflated on `device`.  Returns (bytes, stats dict).
+    chunk_bytes: compressed bytes per chunk (0 = chosen from the compression ratio).  Raises Ht2GpuError for input that
+    is not valid gzip."""
+    lib = load_library()
+    data = data_or_path if isinstance(data_or_path, (bytes, bytearray, memoryview)) else open(data_or_path, "rb").read()
+    data = bytes(data)
+    out, n, st = C.c_void_p(), C.c_size_t(), CGunzipStats()
+    opts = CGunzipOpts(chunk_bytes, 0)
+    rc = lib.ht2gpu_gunzip(device, data, len(data), C.byref(opts), C.byref(out), C.byref(n), C.byref(st))
+    if rc != 0:
+        raise Ht2GpuError("ht2gpu_gunzip rc=%d: %s" % (rc, lib.ht2gpu_gunzip_error().decode()))
+    try:
+        return C.string_at(out, n.value), st.as_dict()
+    finally:
+        lib.ht2gpu_free_text(out)
 
 
 class CSeedResult(C.Structure):
@@ -233,6 +266,10 @@ def load_library(path=None):
     lib.ht2gpu_run_reads_routed.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(CReadsInput), SINK_FN, C.c_void_p,
                                             C.POINTER(CReadRoutes), C.POINTER(CRunStats)]
     lib.ht2gpu_route_reads.argtypes = [C.POINTER(CReadsInput), C.c_void_p, C.c_uint64, C.POINTER(CReadRoutes), C.c_char_p, C.c_size_t]
+    lib.ht2gpu_gunzip.argtypes = [C.c_int, C.c_char_p, C.c_size_t, C.POINTER(CGunzipOpts), C.POINTER(C.c_void_p),
+                                  C.POINTER(C.c_size_t), C.POINTER(CGunzipStats)]
+    lib.ht2gpu_gunzip_error.argtypes = []; lib.ht2gpu_gunzip_error.restype = C.c_char_p
+    lib.ht2gpu_run_gunzip_stats.argtypes = [C.c_void_p, C.POINTER(CGunzipStats)]
     lib.ht2gpu_record_outcomes.argtypes = [C.c_void_p, C.c_int]
     lib.ht2gpu_unit_outcomes.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
     lib.ht2gpu_open_peer.argtypes = [C.c_void_p, C.POINTER(Options), C.POINTER(C.c_void_p)]
@@ -712,6 +749,12 @@ class Index(object):
             return (b"".join(chunks) if collect else None), stats
         stats.update(route_spans=rt.n_spans, route_bytes=rt.bytes, s_route=rt.s_route)
         return (b"".join(chunks) if collect else None), stats, {k: b"".join(v) for k, v in files.items()}
+
+    def gunzip_stats(self):
+        """ht2gpu_run_gunzip_stats: the inflate stats of the gzip inputs of this handle's last run_reads."""
+        st = CGunzipStats()
+        self._check(self._lib.ht2gpu_run_gunzip_stats(self._h, C.byref(st)), "ht2gpu_run_gunzip_stats")
+        return st.as_dict()
 
     def is_graph(self):
         return bool(self._lib.ht2gpu_index_is_graph(self._h))

@@ -18,7 +18,7 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++14",
     "-Xcompiler", "-fPIC", "-cudart", "static",
 ]
-LIB_SRCS = ["ht2_gpu.cu", "ht2_index.cpp", "ht2_host.cpp", "ht2_reads.cpp", "ht2_pipeline.cpp", "ht2_compat.cpp"]
+LIB_SRCS = ["ht2_gpu.cu", "ht2_inflate.cu", "ht2_index.cpp", "ht2_host.cpp", "ht2_reads.cpp", "ht2_pipeline.cpp", "ht2_compat.cpp"]
 
 
 def _newer(target, srcs):

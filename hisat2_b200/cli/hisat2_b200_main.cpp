@@ -82,7 +82,9 @@ static void usage() {
                     "            [--summary-file F] [--new-summary] [--quiet]\n"
                     "            [--un P] [--al P] [--un-conc P] [--al-conc P] [--al-conc-disc P], each also as --<opt>-gz\n"
                     "            and --<opt>-bz2: write unpaired reads that did not / did align, pairs that did not / did align\n"
-                    "            concordantly, and pairs with at least one aligned mate (P.1 / P.2, or '%%' in P replaced by 1 / 2)\n");
+                    "            concordantly, and pairs with at least one aligned mate (P.1 / P.2, or '%%' in P replaced by 1 / 2)\n"
+                    "  Read files (and '-' for stdin) may be gzip-compressed (.gz, BGZF, multi-member); they are recognised by\n"
+                    "  their first bytes, whatever their name, and inflated on the GPU.  For bzip2 use a pipe: -U <(bzip2 -dc r.bz2)\n");
 }
 static void two(const char* a, int32_t& x, int32_t& y) { sscanf(a, "%d,%d", &x, &y); }
 

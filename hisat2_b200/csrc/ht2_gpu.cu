@@ -1938,6 +1938,7 @@ extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output
 
 // The output settings of two handles are the same (ht2gpu_run_reads_multi: one run prints one kind of record)
 bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b) { return a->samOut == b->samOut; }
+int ht2_handle_device(const ht2gpu_handle_t* h) { return h->device; }
 
 extern "C" int ht2gpu_align_counts(ht2gpu_handle_t** hs, int n, int reset, ht2gpu_align_counts_t* out)
 {

@@ -17,9 +17,17 @@
 #include <thread>
 
 #include "../../include/ht2gpu.h"
+#include "ht2_inflate.h"
 #include "ht2_reads.h"
 
+#include <sys/mman.h>
+#include <atomic>
+#include <memory>
+
 bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b);   // ht2_gpu.cu
+int ht2_handle_device(const ht2gpu_handle_t* h);                                  // ht2_gpu.cu
+int ht2_gunzip_to(int device, const void* src, size_t n, uint32_t chunkBytes, Ht2zOut& out, size_t* outLen,
+                  ht2gpu_gunzip_stats_t* stats, std::string& err);               // ht2_inflate.cu
 
 namespace {
 double nowS() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
@@ -33,7 +41,8 @@ struct PipeCtx {
     Ht2ParseScratch scratch;
     std::vector<Ht2HostBatch> stage;
     std::mutex mu;               // one run at a time per handle
-    PipeCtx() : pool(NULL) {}
+    ht2gpu_gunzip_stats_t gz;    // inflate stats of the last run's gzip inputs
+    PipeCtx() : pool(NULL) { memset(&gz, 0, sizeof(gz)); }
     ~PipeCtx() { for (auto& hb : stage) hb.freeAll(); delete pool; }
 };
 void freeCtx(void* p) { delete (PipeCtx*)p; }
@@ -48,6 +57,89 @@ PipeCtx* ctxOf(ht2gpu_handle_t* h, unsigned nth, int nSlots)
         for (auto& hb : c->stage) { hb.alloc = pinAlloc; hb.release = pinFree; }
     }
     return c;
+}
+
+// Compressed input is recognised by its magic bytes, not by a file name suffix.
+bool isGzip(const Ht2ReadSource& s) { return s.size >= 2 && (uint8_t)s.data[0] == 0x1f && (uint8_t)s.data[1] == 0x8b; }
+bool isBzip2(const Ht2ReadSource& s) { return s.size >= 3 && memcmp(s.data, "BZh", 3) == 0; }
+const char* kBzip2Msg = "bzip2-compressed reads are not supported: decompress them through a pipe (bzip2 -dc reads.bz2 | ... -U -)";
+
+// A gzip source is inflated on the device, on a thread of its own, into an address range reserved for the largest
+// output DEFLATE allows (1032 bytes per input byte); pages are committed as the windows land, so the text never moves
+// and the producer indexes and parses it while later windows are still being decoded.  The compressed input is kept
+// until the inflate has finished.  The consumer hands no SAM and routes no read before every member's CRC-32 and
+// ISIZE are verified (Inflater::verified), so corrupt input never produces output.
+struct Inflater : Ht2zOut {
+    Ht2ReadSource comp;                 // the compressed bytes
+    Ht2SourceStream stream;
+    char* base = NULL;
+    size_t reserved = 0, committed = 0;
+    std::atomic<bool> stop{false};
+    ht2gpu_gunzip_stats_t st;
+    std::thread th;
+    char* grow(size_t need)
+    {
+        if (need > reserved) return NULL;
+        if (need > committed) {
+            size_t c = committed + ((size_t)64 << 20) > need ? committed + ((size_t)64 << 20) : need;
+            c = (c + 4095) & ~(size_t)4095;
+            if (c > reserved) c = reserved;
+            if (mprotect(base + committed, c - committed, PROT_READ | PROT_WRITE) != 0) return NULL;
+            committed = c;
+        }
+        return base;
+    }
+    bool landed(size_t len) { stream.publish(len); return !stop.load(); }
+    // takes over s's compressed bytes; s becomes the (growing) decompressed text
+    bool start(Ht2ReadSource& s, int device, std::string& err)
+    {
+        memset(&st, 0, sizeof(st));
+        std::swap(comp.data, s.data); std::swap(comp.size, s.size); std::swap(comp.map, s.map); std::swap(comp.mapLen, s.mapLen);
+        std::swap(comp.own, s.own);
+        if (comp.own.size()) comp.data = comp.own.data();
+        const size_t n = comp.size;
+        reserved = n > ((size_t)1 << 40) / 1032 ? (size_t)1 << 40 : n * 1032 + ((size_t)1 << 20);
+        void* m = mmap(NULL, reserved, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
+        if (m == MAP_FAILED) { err = "gzip input: could not reserve address space for the decompressed reads"; return false; }
+        base = (char*)m;
+        s.data = base; s.size = 0; s.map = m; s.mapLen = reserved; s.stream = &stream;
+        th = std::thread([this, device]() {
+            std::string e;
+            size_t len = 0;
+            const int rc = ht2_gunzip_to(device, comp.data, comp.size, 0, *this, &len, &st, e);
+            stream.finish(rc, rc == HT2GPU_OK ? std::string() : "gzip input: " + e);
+        });
+        return true;
+    }
+    // waits for the inflate; HT2GPU_OK when all of it is there and verified
+    int verified(std::string& err)
+    {
+        std::unique_lock<std::mutex> lk(stream.mu);
+        stream.cv.wait(lk, [&] { return stream.done; });
+        if (stream.rc) err = stream.err;
+        return stream.rc;
+    }
+    void join() { if (th.joinable()) { stop = true; th.join(); } ht2_source_close(comp); }
+    ~Inflater() { join(); }
+};
+
+void addGunzipStats(ht2gpu_gunzip_stats_t& acc, const ht2gpu_gunzip_stats_t& g)
+{
+    acc.in_bytes += g.in_bytes; acc.out_bytes += g.out_bytes; acc.members += g.members; acc.blocks += g.blocks; acc.chunks += g.chunks;
+    acc.chunks_confirmed += g.chunks_confirmed; acc.chunks_merged_no_candidate += g.chunks_merged_no_candidate;
+    acc.chunks_merged_false_positive += g.chunks_merged_false_positive; acc.windows += g.windows; acc.decode_rounds += g.decode_rounds;
+    acc.peak_device_bytes += g.peak_device_bytes;   // the mate files are inflated at the same time
+    acc.windows_cut += g.windows_cut;
+    acc.chunk_bytes = g.chunk_bytes;
+    acc.ms_find += g.ms_find; acc.ms_decode += g.ms_decode; acc.ms_window += g.ms_window; acc.ms_replace += g.ms_replace;
+    acc.ms_crc += g.ms_crc; acc.ms_copy += g.ms_copy;
+}
+// ht2gpu_parse_reads / ht2gpu_route_reads are host-only: compressed input is refused, not inflated on the CPU
+bool refuseCompressed(const Ht2ReadSource& s, std::string& err)
+{
+    if (isBzip2(s)) { err = kBzip2Msg; return true; }
+    if (isGzip(s)) { err = "gzip-compressed reads: this call is host-only; inflate them with ht2gpu_gunzip first"; return true; }
+    return false;
 }
 
 // Routes records to the read files of ht2gpu_read_routes_t by their units' outcomes.  Each of the nine streams
@@ -144,7 +236,11 @@ extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2
     Ht2ReadSource a, b;
     std::string err;
     const bool paired = in->path2 != NULL || in->data2 != NULL;
-    auto fail = [&](int rc, const std::string& m) { ht2gpu_set_error(h, m.c_str()); ht2_source_close(a); ht2_source_close(b); if (st) *st = S; return rc; };
+    std::unique_ptr<Inflater> gzs[2];   // gzip inputs being inflated into a / b
+    auto joinInflate = [&]() { for (auto& g : gzs) if (g) g->join(); };
+    auto fail = [&](int rc, const std::string& m) {
+        ht2gpu_set_error(h, m.c_str()); joinInflate(); ht2_source_close(a); ht2_source_close(b); if (st) *st = S; return rc;
+    };
     if (route) for (int i = 0; i < nDev; i++) { const int rc = ht2gpu_record_outcomes(hs[i], 1); if (rc) return fail(rc, ht2gpu_last_error(hs[i])); }
     // the record starts of each submitted batch (the producer keeps appending to the sources' indexes meanwhile)
     struct SlotRecs { uint64_t r0; std::vector<uint64_t> a, b; };
@@ -154,6 +250,15 @@ extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2
     else return fail(HT2GPU_ERR_ARG, "ht2gpu_run_reads: no input");
     if (in->path2) { if (!ht2_source_open(b, in->path2, err)) return fail(HT2GPU_ERR_ARG, err); }
     else if (in->data2) ht2_source_memory(b, in->data2, in->len2);
+    memset(&C->gz, 0, sizeof(C->gz));
+    for (int k = 0; k < 2; k++) {   // the mate files are inflated at the same time, and while they are read
+        Ht2ReadSource& src = k ? b : a;
+        if (isBzip2(src)) return fail(HT2GPU_ERR_ARG, kBzip2Msg);
+        if (!isGzip(src)) continue;
+        gzs[k].reset(new Inflater());
+        if (!gzs[k]->start(src, ht2_handle_device(h), err)) return fail(HT2GPU_ERR_ARG, err);
+    }
+    bool gzChecked = !gzs[0] && !gzs[1];
     const bool fastq = in->format == 1;
     // -s / -u (hisat2.cpp:1959-1964, 3319): records [skip, skip + upto)
     const uint64_t r0 = in->skip;
@@ -186,7 +291,9 @@ extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2
             const double ti = nowS();
             for (int k = 0; k < (paired ? 2 : 1) && rc == HT2GPU_OK; k++) {
                 Ht2ReadSource& src = k ? b : a;
-                while (!src.scanDone && src.nRecords() < r + want)
+                // a source still being inflated hands over what has landed once it holds a quarter of a batch, so
+                // that the first batches are aligned while the rest is decoded
+                while (!src.scanDone && src.nRecords() < r + want && !(src.stream && src.nRecords() >= r + (want + 3) / 4))
                     if (!ht2_source_scan(src, fastq, pool, (size_t)256 << 20, e)) { rc = HT2GPU_ERR_ARG; break; }
             }
             indexS += nowS() - ti;
@@ -248,8 +355,12 @@ extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2
         S.n_batches++; S.n_units += r.n_units; S.n_reads += stage[slot].n_reads; S.sam_bytes += r.sam_len; S.n_err_reads += r.n_err_reads;
         S.ms_align += r.ms_align; S.ms_sam += r.ms_sam; S.ms_h2d += r.ms_h2d; S.ms_d2h += r.ms_d2h;
         S.h2d_bytes += r.h2d_bytes; S.d2h_bytes += r.d2h_bytes; S.n_launches += r.n_launches;
+        if (!gzChecked) {   // nothing leaves the run before the gzip inputs are verified
+            for (auto& g : gzs) if (g && rc == HT2GPU_OK && (rc = g->verified(prodErr)) != HT2GPU_OK) break;
+            gzChecked = true;
+        }
         const double tk = nowS();
-        if (sink && r.sam_len) { if (sink(ctx, r.sam, r.sam_len) != 0) { rc = HT2GPU_ERR_ARG; prodErr = "the SAM sink reported an error"; } }
+        if (rc == HT2GPU_OK && sink && r.sam_len) { if (sink(ctx, r.sam, r.sam_len) != 0) { rc = HT2GPU_ERR_ARG; prodErr = "the SAM sink reported an error"; } }
         sinkS += nowS() - tk;
         if (route && rc == HT2GPU_OK) {
             const double tr = nowS();
@@ -268,6 +379,11 @@ extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2
     }
     { std::lock_guard<std::mutex> lk(mu); if (rc != HT2GPU_OK && prodRc == HT2GPU_OK) prodRc = rc; cv.notify_all(); }
     producer.join();
+    if (!gzChecked && rc == HT2GPU_OK) for (auto& g : gzs) if (g && rc == HT2GPU_OK) rc = g->verified(prodErr);
+    for (auto& g : gzs)   // a failed inflate explains a failed run better than what the parser made of its bytes
+        if (g && rc != HT2GPU_OK) { std::lock_guard<std::mutex> lk(g->stream.mu); if (g->stream.done && g->stream.rc) { rc = g->stream.rc; prodErr = g->stream.err; } }
+    joinInflate();
+    for (auto& g : gzs) if (g) addGunzipStats(C->gz, g->st);
     if (route) {
         const double tr = nowS();
         router.finish();
@@ -304,6 +420,7 @@ extern "C" int ht2gpu_parse_reads(const ht2gpu_reads_input_t* in, ht2gpu_parsed_
     else return fail("no input");
     if (in->path2) { if (!ht2_source_open(b, in->path2, err)) { ht2_source_close(a); return fail(err); } }
     else if (in->data2) ht2_source_memory(b, in->data2, in->len2);
+    if (refuseCompressed(a, err) || refuseCompressed(b, err)) { ht2_source_close(a); ht2_source_close(b); return fail(err); }
     const bool fastq = in->format == 1;
     bool ok = ht2_source_index(a, fastq, pool, err) && (!paired || ht2_source_index(b, fastq, pool, err));
     if (ok && paired && a.nRecords() != b.nRecords()) { ok = false; err = "mate files have different numbers of reads"; }
@@ -343,6 +460,7 @@ extern "C" int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t*
     else return fail("no input");
     if (in->path2) { if (!ht2_source_open(b, in->path2, err)) { ht2_source_close(a); return fail(err); } }
     else if (in->data2) ht2_source_memory(b, in->data2, in->len2);
+    if (refuseCompressed(a, err) || refuseCompressed(b, err)) { ht2_source_close(a); ht2_source_close(b); return fail(err); }
     const bool fastq = in->format == 1;
     bool ok = ht2_source_index(a, fastq, pool, err) && (!paired || ht2_source_index(b, fastq, pool, err));
     if (ok && paired && a.nRecords() != b.nRecords()) { ok = false; err = "mate files have different numbers of reads"; }
@@ -367,4 +485,13 @@ extern "C" int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t*
 extern "C" void ht2gpu_free_parsed(ht2gpu_parsed_reads_t* p)
 {
     if (p && p->priv) { Ht2HostBatch* hb = (Ht2HostBatch*)p->priv; hb->freeAll(); delete hb; p->priv = NULL; }
+}
+
+extern "C" int ht2gpu_run_gunzip_stats(ht2gpu_handle_t* h, ht2gpu_gunzip_stats_t* st)
+{
+    if (!h || !st) return HT2GPU_ERR_ARG;
+    PipeCtx* c = (PipeCtx*)ht2gpu_ctx_get(h);
+    if (c) { std::lock_guard<std::mutex> lk(c->mu); *st = c->gz; }
+    else memset(st, 0, sizeof(*st));
+    return HT2GPU_OK;
 }

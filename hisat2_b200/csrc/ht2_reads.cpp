@@ -3,6 +3,7 @@
 
 #include <fcntl.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
@@ -80,22 +81,35 @@ void ht2_source_memory(Ht2ReadSource& s, const char* data, size_t n) { s.data = 
 void ht2_source_close(Ht2ReadSource& s)
 {
     if (s.map) munmap(s.map, s.mapLen);
-    s.map = NULL; s.data = NULL; s.size = 0; s.own.clear(); s.rec.clear(); s.scanPos = 0; s.scanDone = false; s.lineCarry = 0; s.strictFastq = true;
+    s.map = NULL; s.stream = NULL; s.data = NULL; s.size = 0; s.own.clear(); s.rec.clear(); s.scanPos = 0; s.scanDone = false; s.lineCarry = 0; s.strictFastq = true;
 }
 
 // Scan the next block of the input for record starts (appended to s.rec).  Blocks are scanned by all threads; the
 // pipeline calls this only as far ahead as the next batch needs, so that indexing overlaps the device work instead
 // of preceding it.  When the end of the input is reached the sentinel (== size) is appended and scanDone is set.
+// A source whose bytes are still arriving is scanned as far as they go, less one byte (so that the byte after each
+// newline scanned is there to be looked at); the sentinel waits for the last byte.
 bool ht2_source_scan(Ht2ReadSource& s, bool fastq, Ht2ThreadPool& pool, size_t blockBytes, std::string& err)
 {
     if (s.scanDone) return true;
+    bool more = false;
+    if (s.stream) {
+        Ht2SourceStream& q = *s.stream;
+        std::unique_lock<std::mutex> lk(q.mu);
+        q.cv.wait(lk, [&] { return q.done || q.avail > s.scanPos + 1; });
+        if (q.rc) { err = q.err; return false; }
+        if (!q.done && fastq && !s.strictFastq) q.cv.wait(lk, [&] { return q.done; });   // the sequential scan below reads to the end
+        if (q.rc) { err = q.err; return false; }
+        s.size = q.avail; more = !q.done;
+    }
     const char* d = s.data; const size_t n = s.size;
-    const size_t b0 = s.scanPos, b1 = (blockBytes == 0 || n - b0 <= blockBytes) ? n : b0 + blockBytes;
+    const size_t lim = more ? n - 1 : n;
+    const size_t b0 = s.scanPos, b1 = (blockBytes == 0 || lim - b0 <= blockBytes) ? lim : b0 + blockBytes;
     const size_t len = b1 - b0;
     const unsigned T = (len < (1u << 20)) ? 1 : pool.size();
     std::vector<std::vector<uint64_t> > part(T);
     auto chunk = [&](unsigned t, size_t& c0, size_t& c1) { c0 = b0 + len / T * t; c1 = (t + 1 == T) ? b1 : b0 + len / T * (t + 1); };
-    auto finish = [&]() { s.scanPos = b1; if (b1 == n) { s.rec.push_back(n); s.scanDone = true; } return true; };
+    auto finish = [&]() { s.scanPos = b1; if (b1 == n && !more) { s.rec.push_back(n); s.scanDone = true; } return true; };
     if (!fastq) {
         // a record starts at a '>' that begins a line
         auto scan = [&](unsigned t) {
@@ -113,7 +127,7 @@ bool ht2_source_scan(Ht2ReadSource& s, bool fastq, Ht2ThreadPool& pool, size_t b
         if (T == 1) scan(0); else pool.run(scan);
         const bool hadNone = s.rec.empty();
         for (auto& v : part) s.rec.insert(s.rec.end(), v.begin(), v.end());
-        if (hadNone && (!s.rec.empty() || b1 == n)) {
+        if (hadNone && (!s.rec.empty() || (b1 == n && !more))) {
             // what precedes the first record may only be blank or comment lines (pat.cpp:741-756)
             size_t p = 0; const size_t first = s.rec.empty() ? n : (size_t)s.rec[0];
             while (p < first) {
@@ -170,6 +184,7 @@ bool ht2_source_scan(Ht2ReadSource& s, bool fastq, Ht2ThreadPool& pool, size_t b
             return finish();
         }
         s.strictFastq = false;   // blank lines between records: fall through to the sequential scan of the rest
+        if (more) return ht2_source_scan(s, fastq, pool, blockBytes, err);   // once all the bytes are there
     }
     {
         // blank lines between records (FastqPatternSource skips them): one sequential pass over the rest, from the

@@ -42,18 +42,31 @@ private:
     void worker(unsigned t);
 };
 
+// The bytes of a source that are still arriving (a gzip input being inflated): ht2_source_scan waits for them.
+struct Ht2SourceStream {
+    std::mutex mu;
+    std::condition_variable cv;
+    size_t avail = 0;           // bytes of the source written so far
+    bool done = false;          // all written (or failed)
+    int rc = 0;                 // nonzero: the source failed, err says why
+    std::string err;
+    void publish(size_t n) { { std::lock_guard<std::mutex> lk(mu); avail = n; } cv.notify_all(); }
+    void finish(int r, const std::string& e) { { std::lock_guard<std::mutex> lk(mu); done = true; rc = r; err = e; } cv.notify_all(); }
+};
+
 struct Ht2ReadSource {          // one input file (or memory range) and its record index
     const char* data;
     size_t      size;
     void*       map;            // mmap base (NULL when not mapped)
     size_t      mapLen;
     std::vector<char> own;      // slurped input (stdin)
+    Ht2SourceStream* stream;    // not NULL while the bytes are still arriving: size grows up to stream->avail
     std::vector<uint64_t> rec;  // offsets of the record starts found so far; a final sentinel == size once scanDone
     size_t      scanPos;        // incremental index: bytes scanned so far
     bool        scanDone;
     uint64_t    lineCarry;      // FASTQ: newlines before scanPos
     bool        strictFastq;    // FASTQ: still in the 4-lines-per-record fast path
-    Ht2ReadSource() : data(NULL), size(0), map(NULL), mapLen(0), scanPos(0), scanDone(false), lineCarry(0), strictFastq(true) {}
+    Ht2ReadSource() : data(NULL), size(0), map(NULL), mapLen(0), stream(NULL), scanPos(0), scanDone(false), lineCarry(0), strictFastq(true) {}
     // records whose END is known: record k spans [rec[k], rec[k+1])
     uint64_t nRecords() const { return rec.empty() ? 0 : rec.size() - 1; }
 };

@@ -285,6 +285,43 @@ int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int n, const ht2gpu_reads_inpu
 int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t* outcomes, uint64_t n_units, ht2gpu_read_routes_t* routes,
                        char* errbuf, size_t errbuf_len);
 
+/* ---- gzip input, inflated on the device --------------------------------------------------------------------------
+ * ht2gpu_gunzip inflates a complete gzip file (one or more RFC 1952 members: gzip, pigz, BGZF, `cat a.gz b.gz`) on a
+ * device: the compressed input is cut into chunks that are decoded in parallel from the first block start found in each
+ * (DESIGN.md 5.2).  Every member's CRC-32 and ISIZE are checked; trailing zero bytes are ignored, anything else after the
+ * last member is an error.  Corrupt input returns HT2GPU_ERR_DATA with no output (ht2gpu_gunzip_error has the reason).
+ * Device memory is a fixed cap (ht2gpu_gunzip_stats_t.peak_device_bytes) whatever the file size, all freed on return.
+ * *out is malloc'ed (free with ht2gpu_free_text).
+ * ht2gpu_run_reads(_multi, _routed) inflate a path or data1 / data2 buffer that begins with 1f 8b this way, on the
+ * first handle's device, while its reads are parsed and aligned; no SAM reaches the sink before every member is
+ * verified.  ht2gpu_parse_reads and ht2gpu_route_reads refuse such input. */
+#define HT2GPU_ERR_DATA -6   /* compressed input that is not valid gzip */
+typedef struct {
+    uint32_t chunk_bytes;   /* compressed bytes per chunk; 0 = chosen per window from the compression ratio */
+    uint32_t reserved;
+} ht2gpu_gunzip_opts_t;
+typedef struct {
+    uint64_t in_bytes, out_bytes;
+    uint64_t members, blocks;
+    uint64_t chunks;                        /* chunks whose output was kept, each counted once */
+    uint64_t chunks_confirmed;              /* of those, decoded speculatively from a confirmed start */
+    uint64_t chunks_merged_no_candidate;    /* chunks in which no block start was found, decoded by their predecessor */
+    uint64_t chunks_merged_false_positive;  /* chunks whose start was not a real one, decoded by their predecessor */
+    uint64_t windows, decode_rounds;        /* windows of compressed input; launches of the chunk decoder */
+    uint64_t windows_cut;                   /* windows ended early because a chunk's output (or its list of member
+                                               ends) was full: the rest of such a window is decoded again */
+    uint64_t peak_device_bytes;             /* device memory the call allocates; all of it is allocated up front */
+    uint32_t chunk_bytes, pad;              /* chunk size of the last window */
+    float    ms_find, ms_decode, ms_window, ms_replace, ms_crc, ms_copy;   /* CUDA-event time per phase */
+} ht2gpu_gunzip_stats_t;
+int ht2gpu_gunzip(int device, const void* src, size_t n, const ht2gpu_gunzip_opts_t* opts, char** out, size_t* out_len,
+                  ht2gpu_gunzip_stats_t* stats);
+/* The reason the calling thread's last ht2gpu_gunzip (or gzip input of a run) failed. */
+const char* ht2gpu_gunzip_error(void);
+/* The summed inflate stats of the gzip inputs of the handle's last ht2gpu_run_reads(_multi, _routed) (zero when its
+ * inputs were plain text). */
+int ht2gpu_run_gunzip_stats(ht2gpu_handle_t* h, ht2gpu_gunzip_stats_t* stats);
+
 /* Replicate an open index onto another device of this process: the packed image is copied device to device
  * (cudaMemcpyPeer: NVLink / NVSwitch when peer access exists), options as given (opt->device = the target). */
 int ht2gpu_open_peer(const ht2gpu_handle_t* src, const ht2gpu_options_t* opt, ht2gpu_handle_t** out);
