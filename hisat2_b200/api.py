@@ -68,6 +68,23 @@ class CReadsInput(C.Structure):
                 ("batch_reads", C.c_uint32), ("threads", C.c_int32)]
 
 
+class CReadsFiles(C.Structure):
+    _fields_ = [("paths1", C.POINTER(C.c_char_p)), ("n1", C.c_uint32), ("paths2", C.POINTER(C.c_char_p)), ("n2", C.c_uint32),
+                ("paths_u", C.POINTER(C.c_char_p)), ("n_u", C.c_uint32)]
+
+
+def _reads_files(paths1=(), paths2=(), unpaired=()):
+    """(CReadsFiles, arrays to keep alive) for lists of -1, -2 and -U files."""
+    rf = CReadsFiles()
+    keep = []
+    for name, ps in (("paths1", paths1), ("paths2", paths2), ("paths_u", unpaired)):
+        arr = (C.c_char_p * max(1, len(ps)))(*[os.fsencode(p) for p in ps])
+        keep.append(arr)
+        setattr(rf, name, C.cast(arr, C.POINTER(C.c_char_p)))
+        setattr(rf, {"paths1": "n1", "paths2": "n2", "paths_u": "n_u"}[name], len(ps))
+    return rf, keep
+
+
 class CRunStats(C.Structure):
     _fields_ = [("n_reads", C.c_uint64), ("n_units", C.c_uint64), ("sam_bytes", C.c_uint64), ("n_err_reads", C.c_uint64),
                 ("n_batches", C.c_uint64), ("s_index", C.c_double), ("s_parse", C.c_double), ("s_total", C.c_double),
@@ -172,6 +189,7 @@ EXPORTS = [
     "ht2gpu_write_novel_splicesites", "ht2gpu_launch_geometry", "ht2gpu_set_sam_output", "ht2gpu_align_counts",
     "ht2gpu_format_align_summary", "ht2gpu_sw_extend", "ht2gpu_record_outcomes", "ht2gpu_unit_outcomes",
     "ht2gpu_run_reads_routed", "ht2gpu_route_reads", "ht2gpu_gunzip", "ht2gpu_gunzip_error", "ht2gpu_run_gunzip_stats",
+    "ht2gpu_run_reads_files",
 ]
 
 
@@ -265,6 +283,8 @@ def load_library(path=None):
     lib.ht2gpu_run_reads_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(CReadsInput), SINK_FN, C.c_void_p, C.POINTER(CRunStats)]
     lib.ht2gpu_run_reads_routed.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(CReadsInput), SINK_FN, C.c_void_p,
                                             C.POINTER(CReadRoutes), C.POINTER(CRunStats)]
+    lib.ht2gpu_run_reads_files.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(CReadsFiles), C.POINTER(CReadsInput), SINK_FN,
+                                           C.c_void_p, C.POINTER(CReadRoutes), C.POINTER(CRunStats)]
     lib.ht2gpu_route_reads.argtypes = [C.POINTER(CReadsInput), C.c_void_p, C.c_uint64, C.POINTER(CReadRoutes), C.c_char_p, C.c_size_t]
     lib.ht2gpu_gunzip.argtypes = [C.c_int, C.c_char_p, C.c_size_t, C.POINTER(CGunzipOpts), C.POINTER(C.c_void_p),
                                   C.POINTER(C.c_size_t), C.POINTER(CGunzipStats)]
@@ -719,13 +739,26 @@ class Index(object):
         return other
 
     def run_reads(self, path1=None, path2=None, data1=None, data2=None, fastq=False, collect=True, peers=(), sink=None,
-                  read_files=(), **kw):
+                  read_files=(), unpaired=None, **kw):
         """ht2gpu_run_reads(_multi): FASTA/FASTQ (files or bytes in host memory) -> SAM records through the overlapped
         pipeline, on this index's device and on the devices of `peers`.  Returns (sam bytes or None, stats dict).
         `sink(ptr, n)`, if given, sees the SAM text of every batch in read order while it is valid (pinned host memory).
         With read_files (names of READ_FILES) the records are also routed (ht2gpu_run_reads_routed) and the call returns
-        (sam, stats, {(output, mate): bytes}); stats then also holds route_spans, route_bytes and s_route."""
-        ri, keep = _reads_input(path1, path2, data1, data2, fastq, **kw)
+        (sam, stats, {(output, mate): bytes}); stats then also holds route_spans, route_bytes and s_route.
+        Lists of files (path1 / path2 as lists, and / or `unpaired`, a list of unpaired-read files aligned after the
+        pairs) run through ht2gpu_run_reads_files: like hisat2 -1 a1,a2 -2 b1,b2 -U u1,u2."""
+        if unpaired is not None or isinstance(path1, (list, tuple)) or isinstance(path2, (list, tuple)):
+            if data1 is not None or data2 is not None:
+                raise ValueError("run_reads: lists of read files take paths, not data")
+            as_list = lambda p: [] if p is None else ([p] if isinstance(p, (str, bytes, os.PathLike)) else list(p))
+            rf, keep_files = _reads_files(as_list(path1), as_list(path2), as_list(unpaired))
+            ri, keep = _reads_input(fastq=fastq, **kw)
+            keep.append(keep_files)
+            run = lambda hs, cb, rt, st: self._lib.ht2gpu_run_reads_files(hs, len(hs), C.byref(rf), C.byref(ri), cb, None,
+                                                                          C.byref(rt) if rt is not None else None, C.byref(st))
+        else:
+            ri, keep = _reads_input(path1, path2, data1, data2, fastq, **kw)
+            run = None
         chunks = []
         total = [0]
 
@@ -739,7 +772,10 @@ class Index(object):
         cb = SINK_FN(_sink) if (collect or sink is not None) else SINK_FN()     # NULL sink: the text still lands in pinned host memory
         st = CRunStats()
         hs = (C.c_void_p * (1 + len(peers)))(self._h, *[p._h for p in peers])
-        if read_files:
+        if run is not None:
+            rt, files = _read_routes(read_files) if read_files else (None, None)
+            self._check(run(hs, cb, rt, st), "ht2gpu_run_reads_files")
+        elif read_files:
             rt, files = _read_routes(read_files)
             self._check(self._lib.ht2gpu_run_reads_routed(hs, len(hs), C.byref(ri), cb, None, C.byref(rt), C.byref(st)), "ht2gpu_run_reads_routed")
         else:

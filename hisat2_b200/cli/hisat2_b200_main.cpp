@@ -72,7 +72,7 @@ static bool closeReadFile(ReadFile& rf)
 }
 
 static void usage() {
-    fprintf(stderr, "hisat2-b200 -x <index> {-U <r> | -1 <m1> -2 <m2>} [-S out.sam] [-f|-q] --no-spliced-alignment [-k N]\n"
+    fprintf(stderr, "hisat2-b200 -x <index> {-U <r> | -1 <m1> -2 <m2> [-U <r>]} [-S out.sam] [-f|-q] --no-spliced-alignment [-k N]\n"
                     "            [--mp MX,MN] [--sp MX,MN] [--np N] [--rdg C,L] [--rfg C,L] [--ignore-quals] [--nofw] [--norc]\n"
                     "            [-I N] [-X N] [--no-mixed] [--no-discordant] [--seed N] [--batch N] [--device N] [--gpus N] [-p N]\n"
                     "            [-5 N] [-3 N] [-s N] [-u N] [--phred33|--phred64] [--no-temp-splicesite]\n"
@@ -84,15 +84,29 @@ static void usage() {
                     "            and --<opt>-bz2: write unpaired reads that did not / did align, pairs that did not / did align\n"
                     "            concordantly, and pairs with at least one aligned mate (P.1 / P.2, or '%%' in P replaced by 1 / 2)\n"
                     "  Read files (and '-' for stdin) may be gzip-compressed (.gz, BGZF, multi-member); they are recognised by\n"
-                    "  their first bytes, whatever their name, and inflated on the GPU.  For bzip2 use a pipe: -U <(bzip2 -dc r.bz2)\n");
+                    "  their first bytes, whatever their name, and inflated on the GPU.  For bzip2 use a pipe: -U <(bzip2 -dc r.bz2)\n"
+                    "  -U, -1 and -2 take comma-separated lists and may be repeated; as many -1 as -2 files.  The -1 / -2 files\n"
+                    "  are one stream of pairs, the -U files one stream of unpaired reads, aligned after the pairs\n");
 }
 static void two(const char* a, int32_t& x, int32_t& y) { sscanf(a, "%d,%d", &x, &y); }
+// -U / -1 / -2 a,b,c: appended to the list, empty names dropped (tokenize, hisat2.cpp:1120-1121, 1621-1626)
+static void addFiles(std::vector<std::string>& v, const char* arg)
+{
+    std::string a = arg;
+    for (size_t p = 0; p <= a.size();) {
+        size_t c = a.find(',', p);
+        if (c == std::string::npos) c = a.size();
+        if (c > p) v.push_back(a.substr(p, c - p));
+        p = c + 1;
+    }
+}
 
 int main(int argc, char** argv)
 {
     ht2gpu_options_t o; ht2gpu_default_options(&o);
     o.no_spliced_alignment = 0; // must be requested explicitly, like the reference's default is spliced
-    const char *idx = NULL, *u = NULL, *m1 = NULL, *m2 = NULL, *out = NULL;
+    const char *idx = NULL, *out = NULL;
+    std::vector<std::string> us, m1s, m2s;   // -U, -1, -2
     bool fastq = true; size_t batchSz = 0 /* library default */; uint32_t gseed = 0;
     int trim5 = 0, trim3 = 0, threads = 0, gpus = 1; bool phred64 = false; uint64_t skip = 0, upto = 0;
     bool sensitive = false, verySensitive = false, fast = false, noTempSpliceSite = false;
@@ -109,7 +123,7 @@ int main(int argc, char** argv)
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
         auto next = [&]() -> const char* { if (i + 1 >= argc) { usage(); exit(1); } return argv[++i]; };
-        if (a == "-x") idx = next(); else if (a == "-U") u = next(); else if (a == "-1") m1 = next(); else if (a == "-2") m2 = next();
+        if (a == "-x") idx = next(); else if (a == "-U") addFiles(us, next()); else if (a == "-1") addFiles(m1s, next()); else if (a == "-2") addFiles(m2s, next());
         else if (a == "-S") out = next(); else if (a == "-f") fastq = false; else if (a == "-q") fastq = true;
         else if (a == "--no-spliced-alignment") o.no_spliced_alignment = 1;
         else if (a == "--no-temp-splicesite") noTempSpliceSite = true;   // spliced mode with an empty splice-site DB: the only spliced form a (HT2_SPLICED=1) library build honours
@@ -160,7 +174,18 @@ int main(int argc, char** argv)
         else if (a == "-h" || a == "--help") { usage(); return 0; }
         else { fprintf(stderr, "Error: option %s is not supported by hisat2-b200\n", a.c_str()); return 1; }
     }
-    if (!idx || (!u && !(m1 && m2))) { usage(); return 1; }
+    if (!idx || (us.empty() && m1s.empty() && m2s.empty())) { usage(); return 1; }
+    if (m1s.size() != m2s.size()) {   // hisat2.cpp:1911-1913
+        fprintf(stderr, "Error: %zu mate files/sequences were specified with -1, but %zu\n"
+                        "mate files/sequences were specified with -2.  The same number of mate files/\n"
+                        "sequences must be specified with -1 and -2.\n", m1s.size(), m2s.size());
+        return 1;
+    }
+    {
+        int nStdin = 0;
+        for (const auto* v : {&us, &m1s, &m2s}) for (const std::string& f : *v) nStdin += f == "-";
+        if (nStdin > 1) { fprintf(stderr, "Error: standard input ('-') can be read only once\n"); return 1; }
+    }
     if (!o.no_spliced_alignment && !noTempSpliceSite)
         fprintf(stderr, "Warning: temporary splice sites (the reference's default) make results depend on the order reads are processed in;\n"
                         "         hisat2-b200 aligns every read independently, i.e. as with --no-temp-splicesite\n");
@@ -191,7 +216,6 @@ int main(int argc, char** argv)
     }
     ht2gpu_handle_t* h = NULL;
     if (ht2gpu_open(idx, &o, &h) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
-    const bool paired = m1 != NULL;
     FILE* fo = out ? fopen(out, "wb") : stdout;
     if (!fo) { fprintf(stderr, "Error: cannot write %s\n", out); return 1; }
     std::vector<const char*> rgPtrs;
@@ -205,7 +229,16 @@ int main(int argc, char** argv)
         fprintf(fo, "@PG\tID:hisat2\tPN:hisat2-b200\tVN:0.2\n");
     }
     ht2gpu_reads_input_t in; memset(&in, 0, sizeof(in));
-    in.path1 = paired ? m1 : u; in.path2 = paired ? m2 : NULL;
+    // one file of one kind goes through ht2gpu_run_reads_routed, lists and pairs with unpaired reads through the list call
+    const bool single = (m1s.empty() && us.size() == 1) || (us.empty() && m1s.size() == 1);
+    if (single) { in.path1 = m1s.empty() ? us[0].c_str() : m1s[0].c_str(); in.path2 = m1s.empty() ? NULL : m2s[0].c_str(); }
+    std::vector<const char*> p1, p2, pu;
+    for (const std::string& f : m1s) p1.push_back(f.c_str());
+    for (const std::string& f : m2s) p2.push_back(f.c_str());
+    for (const std::string& f : us) pu.push_back(f.c_str());
+    ht2gpu_reads_files_t lists;
+    lists.paths1 = p1.data(); lists.n1 = (uint32_t)p1.size(); lists.paths2 = p2.data(); lists.n2 = (uint32_t)p2.size();
+    lists.paths_u = pu.data(); lists.n_u = (uint32_t)pu.size();
     in.format = fastq ? 1 : 0; in.trim5 = trim5; in.trim3 = trim3; in.phred64 = phred64 ? 1 : 0; in.seed = gseed;
     in.skip = skip; in.upto = upto; in.batch_reads = (uint32_t)batchSz; in.threads = threads;
     ht2gpu_read_routes_t routes; memset(&routes, 0, sizeof(routes));
@@ -232,7 +265,8 @@ int main(int argc, char** argv)
     if (novelOut)
         for (ht2gpu_handle_t* hh : hs)
             if (ht2gpu_collect_splicesites(hh, 1) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(hh)); return 1; }
-    const int runRc = ht2gpu_run_reads_routed(hs.data(), (int)hs.size(), &in, sink, fo, &routes, &st);
+    const int runRc = single ? ht2gpu_run_reads_routed(hs.data(), (int)hs.size(), &in, sink, fo, &routes, &st)
+                             : ht2gpu_run_reads_files(hs.data(), (int)hs.size(), &lists, &in, sink, fo, &routes, &st);
     bool filesOk = true;
     for (int w = 0; w < HT2GPU_READS_N; w++)
         for (int m = 0; m < 2; m++) {

@@ -276,8 +276,9 @@ inline uint32_t genSeed(const uint8_t* sq, const uint8_t* ql, uint32_t n, const 
     return rseed;
 }
 
-// Parse one record of 'src' and append it to L.  mate: 0 unpaired, 1 / 2 = fix the mate name.
-bool parseRecord(const Ht2ReadSource& src, uint64_t r, int mate, const Ht2ReadsOpts& o, Local& L)
+// Parse record r of 'src' and append it to L.  mate: 0 unpaired, 1 / 2 = fix the mate name.  rdid is the read's
+// ordinal in its stream (the files of one kind back to back), the default name of an unnamed read.
+bool parseRecord(const Ht2ReadSource& src, uint64_t r, uint64_t rdid, int mate, const Ht2ReadsOpts& o, Local& L)
 {
     const char* d = src.data;
     size_t p = (size_t)src.rec[r]; const size_t e = (size_t)src.rec[r + 1];
@@ -331,7 +332,7 @@ bool parseRecord(const Ht2ReadSource& src, uint64_t r, int mate, const Ht2ReadsO
         if (n && lo < 33) { L.err = "quality value below Phred+33 range in read " + std::string(nm, nl); return false; }
         L.qual.n += n;
     }
-    if (nl == 0) nl = (size_t)snprintf(nm, 24, "%llu", (unsigned long long)r);   // unnamed read: the read ordinal
+    if (nl == 0) nl = (size_t)snprintf(nm, 24, "%llu", (unsigned long long)rdid);   // unnamed read: the read ordinal
     if (mate) {   // Read::fixMateName (read.h:171-196)
         const char want = mate == 1 ? '1' : '2';
         if (nl < 2 || nm[nl - 2] != '/' || nm[nl - 1] != want) { nm[nl++] = '/'; nm[nl++] = want; }
@@ -361,7 +362,15 @@ Ht2ParseScratch::~Ht2ParseScratch() { delete (std::vector<Local>*)impl; }
 bool ht2_parse_batch(const Ht2ReadSource& a, const Ht2ReadSource* b, uint64_t r0, uint64_t r1, const Ht2ReadsOpts& o,
                      Ht2HostBatch& out, Ht2ThreadPool& pool, Ht2ParseScratch& scratch, std::string& err)
 {
-    const uint64_t nrec = r1 - r0;
+    const Ht2BatchPiece pc = {&a, b, r0, r0, r1 - r0, r0};
+    return ht2_parse_pieces(&pc, 1, o, out, pool, scratch, err);
+}
+
+bool ht2_parse_pieces(const Ht2BatchPiece* pcs, size_t npc, const Ht2ReadsOpts& o, Ht2HostBatch& out, Ht2ThreadPool& pool,
+                      Ht2ParseScratch& scratch, std::string& err)
+{
+    uint64_t nrec = 0;
+    for (size_t k = 0; k < npc; k++) nrec += pcs[k].n;
     const unsigned T = nrec < 2048 ? 1 : pool.size();
     std::vector<Local>& loc = *(std::vector<Local>*)scratch.impl;
     if (loc.size() < T) loc.resize(T);
@@ -369,10 +378,16 @@ bool ht2_parse_batch(const Ht2ReadSource& a, const Ht2ReadSource* b, uint64_t r0
         if (t >= T) return;
         Local& L = loc[t];
         L.clear();
-        const uint64_t q0 = r0 + nrec * t / T, q1 = r0 + nrec * (t + 1) / T;
-        for (uint64_t r = q0; r < q1; r++) {
-            if (!parseRecord(a, r, b ? 1 : 0, o, L)) return;
-            if (b && !parseRecord(*b, r, 2, o, L)) return;
+        uint64_t q0 = nrec * t / T, q1 = nrec * (t + 1) / T;   // units of the batch, over the pieces in order
+        for (size_t k = 0, at = 0; k < npc && q0 < q1; at += pcs[k].n, k++) {
+            const Ht2BatchPiece& pc = pcs[k];
+            if (q0 >= at + pc.n) continue;
+            const uint64_t e = q1 < at + pc.n ? q1 : at + pc.n;
+            for (uint64_t u = q0 - at; u < e - at; u++) {
+                if (!parseRecord(*pc.a, pc.ra + u, pc.rdid + u, pc.b ? 1 : 0, o, L)) return;
+                if (pc.b && !parseRecord(*pc.b, pc.rb + u, pc.rdid + u, 2, o, L)) return;
+            }
+            q0 = e;
         }
     };
     if (T == 1) parse(0); else pool.run(parse);

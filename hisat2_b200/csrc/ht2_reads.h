@@ -111,4 +111,14 @@ struct Ht2ParseScratch {
 bool ht2_parse_batch(const Ht2ReadSource& a, const Ht2ReadSource* b, uint64_t r0, uint64_t r1, const Ht2ReadsOpts& o,
                      Ht2HostBatch& out, Ht2ThreadPool& pool, Ht2ParseScratch& scratch, std::string& err);
 
+// A run of a batch's units that lies in one file per mate: records [ra, ra + n) of 'a' (with records [rb, rb + n) of
+// 'b' for pairs), whose first unit has ordinal rdid in its stream.  A batch over several files is a list of pieces.
+struct Ht2BatchPiece {
+    const Ht2ReadSource* a;
+    const Ht2ReadSource* b;
+    uint64_t ra, rb, n, rdid;
+};
+bool ht2_parse_pieces(const Ht2BatchPiece* pcs, size_t npc, const Ht2ReadsOpts& o, Ht2HostBatch& out, Ht2ThreadPool& pool,
+                      Ht2ParseScratch& scratch, std::string& err);
+
 #endif

@@ -280,6 +280,24 @@ typedef struct {
  * zero mask is ht2gpu_run_reads_multi. */
 int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int n, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx,
                             ht2gpu_read_routes_t* routes, ht2gpu_run_stats_t* stats);
+/* Lists of read files (hisat2 -1 a1,a2 -2 b1,b2 -U u1,u2).  The -1 files back to back and the -2 files back to back
+ * are one stream of pairs: record k of the one goes with record k of the other, wherever the files end.  The -U
+ * files back to back are one stream of unpaired reads, aligned after every pair (PairedDualPatternSource,
+ * pat.cpp:234-304).  Each file keeps its own records and is detected as plain or gzip on its own.  "-" (stdin) may
+ * appear once over all lists. */
+typedef struct {
+    const char* const* paths1;  uint32_t n1;    /* -1 */
+    const char* const* paths2;  uint32_t n2;    /* -2: as many as -1 */
+    const char* const* paths_u; uint32_t n_u;   /* -U */
+} ht2gpu_reads_files_t;
+/* ht2gpu_run_reads_routed over lists of files.  Format, trims, --phred64, seed, batch size and threads come from
+ * 'in', whose path and data fields must be NULL.  Read ids, default names of unnamed reads, -s and -u count per stream
+ * (the first unpaired read is rdid 0 again); the read loop ends at the first unit with rdid >= skip + upto, so with -u
+ * below the number of pairs no unpaired read is aligned.  A batch holds units of one stream only.  Pairs are routed to
+ * the -conc outputs, unpaired reads to UN / AL.  Different -1 and -2 counts are HT2GPU_ERR_ARG with the reference's
+ * message (hisat2.cpp:1911-1913). */
+int ht2gpu_run_reads_files(ht2gpu_handle_t** hs, int n, const ht2gpu_reads_files_t* files, const ht2gpu_reads_input_t* in,
+                           ht2gpu_sink_fn sink, void* ctx, ht2gpu_read_routes_t* routes, ht2gpu_run_stats_t* stats);
 /* Host only (no device): route the records of an input (after -s / -u) by outcomes[0 .. n_units), e.g. the bytes of
  * ht2gpu_unit_outcomes of callers that batch through ht2gpu_align_sam.  n_units must equal the input's units. */
 int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t* outcomes, uint64_t n_units, ht2gpu_read_routes_t* routes,
