@@ -229,9 +229,6 @@ int main(int argc, char** argv)
         fprintf(fo, "@PG\tID:hisat2\tPN:hisat2-b200\tVN:0.2\n");
     }
     ht2gpu_reads_input_t in; memset(&in, 0, sizeof(in));
-    // one file of one kind goes through ht2gpu_run_reads_routed, lists and pairs with unpaired reads through the list call
-    const bool single = (m1s.empty() && us.size() == 1) || (us.empty() && m1s.size() == 1);
-    if (single) { in.path1 = m1s.empty() ? us[0].c_str() : m1s[0].c_str(); in.path2 = m1s.empty() ? NULL : m2s[0].c_str(); }
     std::vector<const char*> p1, p2, pu;
     for (const std::string& f : m1s) p1.push_back(f.c_str());
     for (const std::string& f : m2s) p2.push_back(f.c_str());
@@ -265,8 +262,7 @@ int main(int argc, char** argv)
     if (novelOut)
         for (ht2gpu_handle_t* hh : hs)
             if (ht2gpu_collect_splicesites(hh, 1) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(hh)); return 1; }
-    const int runRc = single ? ht2gpu_run_reads_routed(hs.data(), (int)hs.size(), &in, sink, fo, &routes, &st)
-                             : ht2gpu_run_reads_files(hs.data(), (int)hs.size(), &lists, &in, sink, fo, &routes, &st);
+    const int runRc = ht2gpu_run_reads_files(hs.data(), (int)hs.size(), &lists, &in, sink, fo, &routes, &st);
     bool filesOk = true;
     for (int w = 0; w < HT2GPU_READS_N; w++)
         for (int m = 0; m < 2; m++) {

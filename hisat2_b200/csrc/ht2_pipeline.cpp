@@ -32,8 +32,6 @@ int ht2_gunzip_to(int device, const void* src, size_t n, uint32_t chunkBytes, Ht
 
 namespace {
 double nowS() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-void* pinAlloc(size_t n) { return ht2gpu_host_alloc(n); }
-void pinFree(void* p) { ht2gpu_host_free(p); }
 
 // What a handle keeps between ht2gpu_run_reads calls: the parser's thread pool, its per-thread buffers and the
 // pinned staging buffers of every slot (allocating pinned memory costs more than parsing a batch).
@@ -55,7 +53,7 @@ PipeCtx* ctxOf(ht2gpu_handle_t* h, unsigned nth, int nSlots)
     if ((int)c->stage.size() != nSlots) {
         for (auto& hb : c->stage) hb.freeAll();
         c->stage.assign((size_t)nSlots, Ht2HostBatch());
-        for (auto& hb : c->stage) { hb.alloc = pinAlloc; hb.release = pinFree; }
+        for (auto& hb : c->stage) { hb.alloc = ht2gpu_host_alloc; hb.release = ht2gpu_host_free; }
     }
     return c;
 }
@@ -65,19 +63,52 @@ bool isGzip(const Ht2ReadSource& s) { return s.size >= 2 && (uint8_t)s.data[0] =
 bool isBzip2(const Ht2ReadSource& s) { return s.size >= 3 && memcmp(s.data, "BZh", 3) == 0; }
 const char* kBzip2Msg = "bzip2-compressed reads are not supported: decompress them through a pipe (bzip2 -dc reads.bz2 | ... -U -)";
 
-// A gzip source is inflated on the device, on a thread of its own, into an address range reserved for the largest
-// output DEFLATE allows (1032 bytes per input byte); pages are committed as the windows land, so the text never moves
-// and the producer indexes and parses it while later windows are still being decoded.  The compressed input is kept
-// until the inflate has finished.  The consumer hands no SAM and routes no read before every member's CRC-32 and
-// ISIZE are verified (Inflater::verified), so corrupt input never produces output.
-struct Inflater : Ht2zOut {
-    Ht2ReadSource comp;                 // the compressed bytes
+void addGunzipStats(ht2gpu_gunzip_stats_t& acc, const ht2gpu_gunzip_stats_t& g)
+{
+    acc.in_bytes += g.in_bytes; acc.out_bytes += g.out_bytes; acc.members += g.members; acc.blocks += g.blocks; acc.chunks += g.chunks;
+    acc.chunks_confirmed += g.chunks_confirmed; acc.chunks_merged_no_candidate += g.chunks_merged_no_candidate;
+    acc.chunks_merged_false_positive += g.chunks_merged_false_positive; acc.windows += g.windows; acc.decode_rounds += g.decode_rounds;
+    acc.peak_device_bytes += g.peak_device_bytes;   // the mate files are inflated at the same time
+    acc.windows_cut += g.windows_cut;
+    acc.chunk_bytes = g.chunk_bytes;
+    acc.ms_find += g.ms_find; acc.ms_decode += g.ms_decode; acc.ms_window += g.ms_window; acc.ms_replace += g.ms_replace;
+    acc.ms_crc += g.ms_crc; acc.ms_copy += g.ms_copy;
+}
+
+struct InputSpec { const char* path; const char* data; size_t len; };
+bool openSpec(Ht2ReadSource& s, const InputSpec& sp, std::string& err)
+{
+    if (!sp.path) { ht2_source_memory(s, sp.data, sp.len); return true; }
+    return ht2_source_open(s, sp.path, err);
+}
+// One input of a stream: a file (or memory range) and its record index; the consumer verifies and releases it.  A gzip
+// source is inflated on the device, on a thread of its own, into an address range reserved for the largest output
+// DEFLATE allows (1032 bytes per input byte); pages are committed as the windows land, so the text never moves and the
+// producer indexes and parses it while later windows are still being decoded.  The compressed input is kept until the
+// inflate has finished.  The consumer hands no SAM and routes no read before every member's CRC-32 and ISIZE are
+// verified (verify), so corrupt input never produces output.
+struct InFile : Ht2zOut {
+    Ht2ReadSource src;
+    bool gzip = false;
+    bool started = false;                // plain, or inflate started: src holds the text
+    bool released = false;
+    std::atomic<bool> exhausted{false};  // producer: moved past its last record, never touches it again
+    std::atomic<int64_t> lastBatch{-1};  // the last batch holding records of it
+    Ht2ReadSource comp;                  // gzip: the compressed bytes
     Ht2SourceStream stream;
     char* base = NULL;
     size_t reserved = 0, committed = 0;
     std::atomic<bool> stop{false};
     ht2gpu_gunzip_stats_t st;
     std::thread th;
+    ~InFile() { if (th.joinable()) { stop = true; th.join(); } }
+    bool open(const InputSpec& sp, std::string& err) { return openSpec(src, sp, err); }
+    bool detect(std::string& err)
+    {
+        if (isBzip2(src)) { err = kBzip2Msg; return false; }
+        started = !(gzip = isGzip(src));
+        return true;
+    }
     char* grow(size_t need)
     {
         if (need > reserved) return NULL;
@@ -91,19 +122,21 @@ struct Inflater : Ht2zOut {
         return base;
     }
     bool landed(size_t len) { stream.publish(len); return !stop.load(); }
-    // takes over s's compressed bytes; s becomes the (growing) decompressed text
-    bool start(Ht2ReadSource& s, int device, std::string& err)
+    // takes over src's compressed bytes; src becomes the (growing) decompressed text
+    bool startInflate(int device, std::string& err)
     {
+        if (started) return true;
+        started = true;
         memset(&st, 0, sizeof(st));
-        std::swap(comp.data, s.data); std::swap(comp.size, s.size); std::swap(comp.map, s.map); std::swap(comp.mapLen, s.mapLen);
-        std::swap(comp.own, s.own);
+        std::swap(comp.data, src.data); std::swap(comp.size, src.size); std::swap(comp.map, src.map); std::swap(comp.mapLen, src.mapLen);
+        std::swap(comp.own, src.own);
         if (comp.own.size()) comp.data = comp.own.data();
         const size_t n = comp.size;
         reserved = n > ((size_t)1 << 40) / 1032 ? (size_t)1 << 40 : n * 1032 + ((size_t)1 << 20);
         void* m = mmap(NULL, reserved, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
         if (m == MAP_FAILED) { err = "gzip input: could not reserve address space for the decompressed reads"; return false; }
         base = (char*)m;
-        s.data = base; s.size = 0; s.map = m; s.mapLen = reserved; s.stream = &stream;
+        src.data = base; src.size = 0; src.map = m; src.mapLen = reserved; src.stream = &stream;
         th = std::thread([this, device]() {
             std::string e;
             size_t len = 0;
@@ -112,35 +145,42 @@ struct Inflater : Ht2zOut {
         });
         return true;
     }
-    // waits for the inflate; HT2GPU_OK when all of it is there and verified
-    int verified(std::string& err)
+    // HT2GPU_OK when the text is all there and every member verified (wait: for the inflate to finish), or while
+    // the inflate runs (!wait)
+    int verify(std::string& err, bool wait = true)
     {
+        if (!gzip || !started) return HT2GPU_OK;
         std::unique_lock<std::mutex> lk(stream.mu);
-        stream.cv.wait(lk, [&] { return stream.done; });
-        if (stream.rc) err = stream.err;
-        return stream.rc;
+        if (wait) stream.cv.wait(lk, [&] { return stream.done; });
+        if (stream.done && stream.rc) err = stream.err;
+        return stream.done ? stream.rc : HT2GPU_OK;
     }
-    void join() { if (th.joinable()) { stop = true; th.join(); } ht2_source_close(comp); }
-    ~Inflater() { join(); }
+    void release(ht2gpu_gunzip_stats_t& gzStats)
+    {
+        if (released) return;
+        if (th.joinable()) { stop = true; th.join(); }
+        if (gzip && started) addGunzipStats(gzStats, st);
+        ht2_source_close(comp);
+        ht2_source_close(src);
+        released = true;
+    }
 };
-
-void addGunzipStats(ht2gpu_gunzip_stats_t& acc, const ht2gpu_gunzip_stats_t& g)
-{
-    acc.in_bytes += g.in_bytes; acc.out_bytes += g.out_bytes; acc.members += g.members; acc.blocks += g.blocks; acc.chunks += g.chunks;
-    acc.chunks_confirmed += g.chunks_confirmed; acc.chunks_merged_no_candidate += g.chunks_merged_no_candidate;
-    acc.chunks_merged_false_positive += g.chunks_merged_false_positive; acc.windows += g.windows; acc.decode_rounds += g.decode_rounds;
-    acc.peak_device_bytes += g.peak_device_bytes;   // the mate files are inflated at the same time
-    acc.windows_cut += g.windows_cut;
-    acc.chunk_bytes = g.chunk_bytes;
-    acc.ms_find += g.ms_find; acc.ms_decode += g.ms_decode; acc.ms_window += g.ms_window; acc.ms_replace += g.ms_replace;
-    acc.ms_crc += g.ms_crc; acc.ms_copy += g.ms_copy;
-}
 // ht2gpu_parse_reads / ht2gpu_route_reads are host-only: compressed input is refused, not inflated on the CPU
 bool refuseCompressed(const Ht2ReadSource& s, std::string& err)
 {
     if (isBzip2(s)) { err = kBzip2Msg; return true; }
     if (isGzip(s)) { err = "gzip-compressed reads: this call is host-only; inflate them with ht2gpu_gunzip first"; return true; }
     return false;
+}
+unsigned threadCount(const ht2gpu_reads_input_t* in)
+{
+    const unsigned n = in->threads > 0 ? (unsigned)in->threads : std::thread::hardware_concurrency();
+    return n < 1 ? 1 : n > 64 ? 64 : n;
+}
+Ht2ReadsOpts readsOpts(const ht2gpu_reads_input_t* in)
+{
+    Ht2ReadsOpts ro; ro.fastq = in->format == 1; ro.trim5 = in->trim5; ro.trim3 = in->trim3; ro.phred64 = in->phred64 != 0; ro.seed = in->seed;
+    return ro;
 }
 
 // Routes records to the read files of ht2gpu_read_routes_t by their units' outcomes.  Each of the nine streams
@@ -210,336 +250,328 @@ extern "C" int ht2gpu_run_reads_multi(ht2gpu_handle_t** hs, int nDev, const ht2g
 }
 
 namespace {
-// One input of a stream: a file (or memory range), its record index, and its inflate when it is gzip.
-struct InFile {
-    Ht2ReadSource src;
-    std::unique_ptr<Inflater> gz;        // gzip input: created when opened, started when the producer comes near it
-    bool started = false;                // plain, or inflate started: src holds the text
-    bool verified = false;               // consumer: every gzip member checked
-    bool closed = false;
-    std::atomic<bool> exhausted{false};  // producer: moved past its last record, never touches it again
-    std::atomic<int64_t> lastBatch{-1};  // the last batch holding records of it
-};
-// The reads of one kind: pairs (f[0] the -1 files, f[1] the -2 files) or unpaired reads (f[0]).  Record k of the
-// stream is record k of its files back to back; the mates of a pair have the same ordinal, wherever the files end.
+// The reads of one kind: pairs (files[0] the -1 files, files[1] the -2 files) or unpaired reads (files[0]).  Record k
+// of the stream is record k of its files back to back; the mates of a pair have the same ordinal, wherever the files end.
+struct StreamSpec { bool paired; std::vector<InputSpec> files[2]; };
+
 struct Stream {
     bool paired = false;
     std::vector<std::unique_ptr<InFile> > f[2];
-};
-struct InputSpec { const char* path; const char* data; size_t len; };
-
-// The pipeline over a run's streams, in order (pairs before unpaired reads).  rdid, -s and -u count per stream, as
-// the reference's per-source read counters do (pat.h:224, hisat2.cpp:1959-1964, 3319); the read loop ends for good at
-// the first unit with rdid >= skip + upto (hisat2.cpp:3634), so a later stream is read only if the earlier one ended
-// before that.  A batch never holds units of two streams.
-int runStreams(ht2gpu_handle_t** hs, int nDev, const std::vector<InputSpec>* specs, int nStreams, bool pairedFirst,
-               const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx, ht2gpu_read_routes_t* routes, ht2gpu_run_stats_t* st)
-{
-    ht2gpu_handle_t* h = hs[0];
-    const bool route = routes && routes->mask;
-    if (route && !routes->write) return HT2GPU_ERR_ARG;
-    if (routes) { routes->n_spans = 0; routes->bytes = 0; routes->s_route = 0; }
-    for (int i = 1; i < nDev; i++)
-        if (!ht2_same_sam_output(h, hs[i])) { ht2gpu_set_error(h, "ht2gpu_run_reads_multi: the handles' SAM output settings differ"); return HT2GPU_ERR_ARG; }
-    ht2gpu_run_stats_t S; memset(&S, 0, sizeof(S));
-    const double t0 = nowS();
-    unsigned nth = in->threads > 0 ? (unsigned)in->threads : std::thread::hardware_concurrency();
-    if (nth < 1) nth = 1;
-    if (nth > 64) nth = 64;
-    const int perDev = ht2gpu_sam_slots(h);
-    const int nSlots = perDev * nDev;          // stage k: device k % nDev, device slot k / nDev
-    PipeCtx* C = ctxOf(h, nth, nSlots);
-    std::lock_guard<std::mutex> runLock(C->mu);
-    Ht2ThreadPool& pool = *C->pool;
-    std::vector<Ht2HostBatch>& stage = C->stage;
-    std::string err;
-    const int device = ht2_handle_device(h);
-    std::vector<Stream> streams((size_t)nStreams);
-    auto eachFile = [&](const std::function<void(InFile&)>& fn) { for (auto& s : streams) for (auto& v : s.f) for (auto& F : v) fn(*F); };
-    memset(&C->gz, 0, sizeof(C->gz));
-    auto closeFile = [&](InFile& F) {   // the producer is done with it
-        if (F.closed) return;
-        if (F.gz) { F.gz->join(); if (F.started) addGunzipStats(C->gz, F.gz->st); }
-        ht2_source_close(F.src);
-        F.closed = true;
-    };
-    auto fail = [&](int rc, const std::string& m) { ht2gpu_set_error(h, m.c_str()); eachFile(closeFile); if (st) *st = S; return rc; };
-    if (route) for (int i = 0; i < nDev; i++) { const int rc = ht2gpu_record_outcomes(hs[i], 1); if (rc) return fail(rc, ht2gpu_last_error(hs[i])); }
-    // every file is opened (mapped) up front, so that a missing one fails the run before anything is aligned
-    for (int s = 0; s < nStreams; s++) {
-        streams[s].paired = pairedFirst && s == 0;
-        for (int k = 0; k < (streams[s].paired ? 2 : 1); k++)
-            for (const InputSpec& sp : specs[s * 2 + k]) {
-                streams[s].f[k].emplace_back(new InFile());
-                InFile& F = *streams[s].f[k].back();
-                if (sp.path) { if (!ht2_source_open(F.src, sp.path, err)) return fail(HT2GPU_ERR_ARG, err); }
-                else ht2_source_memory(F.src, sp.data, sp.len);
-            }
+    // a gzip file is inflated from the time the producer reaches the file before it (or the run starts), so that the
+    // next file's text is landing while the current one is read
+    bool startAhead(int k, size_t fi, int device, std::string& e)
+    {
+        for (size_t j = fi; j < fi + 2 && j < f[k].size(); j++) if (!f[k][j]->startInflate(device, e)) return false;
+        return true;
     }
-    for (int s = 0; s < nStreams; s++)
-        for (auto& v : streams[s].f)
-            for (auto& F : v) {
-                if (isBzip2(F->src)) return fail(HT2GPU_ERR_ARG, kBzip2Msg);
-                if (isGzip(F->src)) F->gz.reset(new Inflater()); else F->started = true;
-            }
-    // a gzip file is inflated from the time the producer reaches the file before it (or the run starts), so that
-    // the next file's text is landing while the current one is read
-    auto startFile = [&](Stream& S, int k, size_t fi, std::string& e) {
-        for (size_t j = fi; j < fi + 2 && j < S.f[k].size(); j++) {
-            InFile& F = *S.f[k][j];
-            if (!F.started) { F.started = true; if (!F.gz->start(F.src, device, e)) return false; }
+};
+// A submitted batch as the consumer needs it after its wait: its pieces and, per piece and mate, the file and, when
+// routing, a copy of the record starts rec[ra .. ra + n] (the producer keeps appending to the files' indexes meanwhile).
+struct RecPiece { InFile* f[2]; std::vector<uint64_t> rec[2]; };
+struct SlotBatch { std::vector<Ht2BatchPiece> pcs; std::vector<RecPiece> recs; };
+
+// The producer's place in a stream: per mate, the file (cf) and the record in that file (cp) of the next unit.
+struct StreamCursor {
+    Stream& S;
+    Stream* after;   // the next stream: its first file starts inflating when this stream reaches its last one
+    const int device;
+    const bool fastq;
+    Ht2ThreadPool& pool;
+    size_t cf[2];
+    uint64_t cp[2];
+    int nm() const { return S.paired ? 2 : 1; }
+    // the n units [r, r + want) that are there (0 at the end of the stream); a pair with only one mate is an error
+    bool next(uint64_t r, uint64_t want, uint64_t rEnd, uint64_t& n, std::string& e)
+    {
+        uint64_t av[2] = {0, 0}; bool ended[2] = {false, false};
+        n = ~(uint64_t)0;
+        for (int k = 0; k < nm(); k++) { if (!indexAhead(k, want, av[k], ended[k], e)) return false; if (av[k] < n) n = av[k]; }
+        if (S.paired && av[0] != av[1] && ended[av[0] < av[1] ? 0 : 1] && r + n < rEnd) {
+            e = av[0] < av[1] ? "fewer reads in file specified with -1 than in file specified with -2"
+                              : "fewer reads in file specified with -2 than in file specified with -1";
+            return false;
         }
         return true;
-    };
-    for (int k = 0; k < 2 && nStreams > 0; k++) if (!startFile(streams[0], k, 0, err)) return fail(HT2GPU_ERR_ARG, err);
-    const bool fastq = in->format == 1;
-    // -s / -u (hisat2.cpp:1959-1964, 3319): records [skip, skip + upto) of each stream
-    const uint64_t r0 = in->skip;
-    const uint64_t rEnd = in->upto ? r0 + in->upto : ~(uint64_t)0;
-    const uint64_t perRead = in->batch_reads ? in->batch_reads : 4000000;   // large batches amortise the drain of the pool kernel's last reads
-    Ht2ReadsOpts ro; ro.fastq = fastq; ro.trim5 = in->trim5; ro.trim3 = in->trim3; ro.phred64 = in->phred64 != 0; ro.seed = in->seed;
+    }
+    // Moves past units [rdid, rdid + n) of batch bi, cut into the pieces in which every mate stays in one file (b ==
+    // NULL: skipped records).  A file's last batch is set before the file is marked exhausted, so that the consumer
+    // never lets go of a file this batch still has to parse.
+    bool take(uint64_t rdid, uint64_t n, SlotBatch* b, int64_t bi, bool route, std::string& e)
+    {
+        size_t q = 0;
+        if (b) b->pcs.clear();
+        for (uint64_t u = 0; u < n;) {
+            uint64_t m = n - u;
+            bool moved = false;
+            for (int k = 0; k < nm() && !moved; k++) {
+                if (cf[k] >= S.f[k].size()) { e = "read front end: a batch ran past the end of its input"; return false; }
+                InFile& F = *S.f[k][cf[k]];
+                const uint64_t rem = F.src.nRecords() - cp[k];
+                if (rem == 0 && F.src.scanDone) { F.exhausted = true; cf[k]++; cp[k] = 0; moved = true; }
+                else if (rem < m) m = rem;
+            }
+            if (moved) continue;
+            if (b) {
+                if (q == b->recs.size()) b->recs.emplace_back();
+                RecPiece& rp = b->recs[q++];
+                for (int k = 0; k < 2; k++) {
+                    InFile* F = rp.f[k] = k < nm() ? S.f[k][cf[k]].get() : NULL;
+                    if (F) F->lastBatch = bi;
+                    if (F && route) rp.rec[k].assign(F->src.rec.begin() + (ptrdiff_t)cp[k], F->src.rec.begin() + (ptrdiff_t)(cp[k] + m) + 1);
+                }
+                b->pcs.push_back({&rp.f[0]->src, rp.f[1] ? &rp.f[1]->src : NULL, cp[0], rp.f[1] ? cp[1] : 0, m, rdid + u});
+            }
+            for (int k = 0; k < nm(); k++) cp[k] += m;
+            u += m;
+        }
+        if (b) b->recs.resize(q);
+        for (int k = 0; k < nm(); k++)   // a file read to its end is let go at once
+            while (cf[k] < S.f[k].size() && S.f[k][cf[k]]->src.scanDone && cp[k] == S.f[k][cf[k]]->src.nRecords()) {
+                S.f[k][cf[k]]->exhausted = true; cf[k]++; cp[k] = 0;
+            }
+        return true;
+    }
+    // Index mate k's files from the cursor on until `want` records are known, the files end (ended), or a file still
+    // being inflated holds a quarter of them, so that the first batches are aligned while the rest is decoded.  have:
+    // the number of records known, at most want.
+    bool indexAhead(int k, uint64_t want, uint64_t& have, bool& ended, std::string& e)
+    {
+        size_t fi = cf[k]; uint64_t pos = cp[k];
+        have = 0;
+        for (;;) {
+            if (fi >= S.f[k].size()) { ended = true; return true; }
+            if (!S.startAhead(k, fi, device, e)) return false;
+            if (fi + 1 == S.f[k].size() && after && !after->startAhead(0, 0, device, e)) return false;
+            Ht2ReadSource& src = S.f[k][fi]->src;
+            while (!src.scanDone && src.nRecords() < pos + (want - have) && !(src.stream && have + src.nRecords() - pos >= (want + 3) / 4))
+                if (!ht2_source_scan(src, fastq, pool, (size_t)256 << 20, e)) return false;
+            have += src.nRecords() - pos < want - have ? src.nRecords() - pos : want - have;
+            if (have == want || !src.scanDone) return true;
+            fi++; pos = 0;
+        }
+    }
+};
 
-    // slot states: 0 free, 1 submitted
-    std::mutex mu; std::condition_variable cv;
-    std::vector<int> state((size_t)nSlots, 0);
-    uint64_t submitted = 0;
-    int prodRc = HT2GPU_OK; std::string prodErr; bool prodDone = false;
-    double parseS = 0, submitS = 0, waitS = 0, sinkS = 0, indexS = 0;
-    // the pieces of each submitted batch, with their record starts when routing (the producer keeps appending to the
-    // sources' indexes meanwhile)
-    struct RecPiece { InFile* fa; InFile* fb; const char* da; const char* db; uint64_t ra, rb, n; std::vector<uint64_t> a, b; };
-    struct SlotRecs { bool paired; std::vector<RecPiece> pcs; };
-    std::vector<SlotRecs> recs((size_t)nSlots);
+// One call of the pipeline over a run's streams, in order (pairs before unpaired reads).  rdid, -s and -u count per
+// stream, as the reference's per-source read counters do (pat.h:224, hisat2.cpp:1959-1964, 3319); the read loop ends
+// for good at the first unit with rdid >= skip + upto (hisat2.cpp:3634), so a later stream is read only if the earlier
+// one ended before that.  A batch never holds units of two streams.  The producer thread indexes, parses and submits
+// batches; the caller's thread waits for them in order.  What the two share is under mu, the run's first failure too.
+struct Run {
+    Run(ht2gpu_handle_t** hs, int nDev, const ht2gpu_reads_input_t* in, ht2gpu_sink_fn sink, void* ctx, ht2gpu_read_routes_t* routes)
+        : hs(hs), nDev(nDev), in(in), sink(sink), ctx(ctx), routes(routes), route(routes && routes->mask), ro(readsOpts(in)),
+          r0(in->skip), rEnd(in->upto ? in->skip + in->upto : ~(uint64_t)0),
+          perRead(in->batch_reads ? in->batch_reads : 4000000),   // large batches amortise the drain of the pool kernel's last reads
+          router(routes, ro.fastq) { memset(&S, 0, sizeof(S)); }
+    int exec(const std::vector<StreamSpec>& specs, ht2gpu_run_stats_t* st)
+    {
+        if (route && !routes->write) return HT2GPU_ERR_ARG;
+        if (routes) { routes->n_spans = 0; routes->bytes = 0; routes->s_route = 0; }
+        for (int i = 1; i < nDev; i++)
+            if (!ht2_same_sam_output(hs[0], hs[i])) { ht2gpu_set_error(hs[0], "ht2gpu_run_reads_multi: the handles' SAM output settings differ"); return HT2GPU_ERR_ARG; }
+        const double t0 = nowS();
+        nSlots = ht2gpu_sam_slots(hs[0]) * nDev;   // stage k: device k % nDev, device slot k / nDev
+        C = ctxOf(hs[0], threadCount(in), nSlots);
+        std::lock_guard<std::mutex> runLock(C->mu);
+        memset(&C->gz, 0, sizeof(C->gz));
+        device = ht2_handle_device(hs[0]);
+        state.assign((size_t)nSlots, 0);
+        batches.resize((size_t)nSlots);
+        if (open(specs)) {
+            std::thread producer([this] { produce(); std::lock_guard<std::mutex> lk(mu); prodDone = true; cv.notify_all(); });
+            consume();
+            producer.join();
+        }
+        return finish(t0, st);
+    }
+    ht2gpu_handle_t** const hs;
+    const int nDev;
+    const ht2gpu_reads_input_t* const in;
+    const ht2gpu_sink_fn sink; void* const ctx;
+    ht2gpu_read_routes_t* const routes; const bool route;
+    const Ht2ReadsOpts ro;
+    const uint64_t r0, rEnd, perRead;   // -s / -u (hisat2.cpp:1959-1964, 3319): records [skip, skip + upto) of each stream
+    int nSlots = 0, device = 0;
+    PipeCtx* C = NULL;
+    std::vector<Stream> streams;
+    std::vector<InFile*> files;          // every file of every stream, in order
+    std::vector<SlotBatch> batches;      // per slot
+    Router router;                       // consumer
+    ht2gpu_run_stats_t S;                // consumer
+    double parseS = 0, submitS = 0, indexS = 0, waitS = 0, sinkS = 0, routeS = 0;
+    std::mutex mu;
+    std::condition_variable cv;
+    std::vector<int> state;              // per slot: 0 free, 1 submitted
+    uint64_t submitted = 0; bool prodDone = false;
+    int rc = HT2GPU_OK;                  // the first failure of either thread
+    std::string err;
+
+    // Keeps the first failure and wakes both threads; returns false.
+    bool fail(int code, const std::string& m)
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        if (rc == HT2GPU_OK) { rc = code; err = m; }
+        cv.notify_all();
+        return false;
+    }
+
+    // Every file is opened (mapped) up front, so that a missing one fails the run before anything is aligned.
+    bool open(const std::vector<StreamSpec>& specs)
+    {
+        std::string e;
+        for (int i = 0; i < nDev && route; i++) { const int orc = ht2gpu_record_outcomes(hs[i], 1); if (orc) return fail(orc, ht2gpu_last_error(hs[i])); }
+        streams.resize(specs.size());
+        for (size_t s = 0; s < specs.size(); s++) {
+            streams[s].paired = specs[s].paired;
+            for (int k = 0; k < (specs[s].paired ? 2 : 1); k++)
+                for (const InputSpec& sp : specs[s].files[k]) {
+                    streams[s].f[k].emplace_back(new InFile());
+                    files.push_back(streams[s].f[k].back().get());
+                    if (!files.back()->open(sp, e)) return fail(HT2GPU_ERR_ARG, e);
+                }
+        }
+        for (InFile* F : files) if (!F->detect(e)) return fail(HT2GPU_ERR_ARG, e);
+        for (int k = 0; k < 2 && !streams.empty(); k++) if (!streams[0].startAhead(k, 0, device, e)) return fail(HT2GPU_ERR_ARG, e);
+        return true;
+    }
+
+    bool index(StreamCursor& cur, uint64_t r, uint64_t want, uint64_t& n)
+    {
+        const double ti = nowS();
+        std::string e;
+        const bool ok = cur.next(r, want, rEnd, n, e);
+        indexS += nowS() - ti;
+        return ok || fail(HT2GPU_ERR_ARG, e);
+    }
 
     // The producer indexes the input only as far ahead as the next batch needs (so that indexing overlaps the device
     // work), parses the batch on all threads and submits it.  The first batch is a quarter of the others: the device
     // starts early, the later batches are large.
-    std::thread producer([&]() {
-        uint64_t i = 0;
-        int rc = HT2GPU_OK;
+    void produce()
+    {
+        uint64_t i = 0, n = 0;
         std::string e;
-        std::vector<Ht2BatchPiece> pcs;
-        for (int s = 0; s < nStreams && rc == HT2GPU_OK; s++) {
-            Stream& SM = streams[s];
-            const int nm = SM.paired ? 2 : 1;
-            uint64_t perBatch = SM.paired ? (perRead + 1) / 2 : perRead;   // batch_reads counts reads, a unit here may be a pair
-            if (perBatch < 1) perBatch = 1;
-            size_t cf[2] = {0, 0}; uint64_t cp[2] = {0, 0};   // per mate: the cursor's file and its record in that file
-            // Index mate k's files from the cursor on until `want` records are known, the files end (ended), or a
-            // file still being inflated holds a quarter of them, so that the first batches are aligned while the rest
-            // is decoded.  Returns the number of records known, at most want.
-            auto indexAhead = [&](int k, uint64_t want, bool& ended) -> uint64_t {
-                uint64_t have = 0; size_t fi = cf[k]; uint64_t pos = cp[k];
-                ended = false;
-                for (;;) {
-                    if (fi >= SM.f[k].size()) { ended = true; break; }
-                    if (!startFile(SM, k, fi, e)) { rc = HT2GPU_ERR_ARG; break; }
-                    if (fi + 1 == SM.f[k].size() && s + 1 < nStreams && !startFile(streams[s + 1], 0, 0, e)) { rc = HT2GPU_ERR_ARG; break; }
-                    Ht2ReadSource& src = SM.f[k][fi]->src;
-                    while (!src.scanDone && src.nRecords() < pos + (want - have) && !(src.stream && have + src.nRecords() - pos >= (want + 3) / 4))
-                        if (!ht2_source_scan(src, fastq, pool, (size_t)256 << 20, e)) { rc = HT2GPU_ERR_ARG; break; }
-                    if (rc != HT2GPU_OK) break;
-                    const uint64_t got = src.nRecords() - pos < want - have ? src.nRecords() - pos : want - have;
-                    have += got;
-                    if (have == want || !src.scanDone) break;
-                    fi++; pos = 0;
-                }
-                return have;
-            };
-            // Units [r, r + n) of batch bi: the pieces in which every mate stays in one file (pieces == NULL: skipped
-            // records).  A file's last batch is set before the file is marked exhausted, so that the consumer never
-            // lets go of a file this batch still has to parse.
-            auto take = [&](uint64_t r, uint64_t n, std::vector<Ht2BatchPiece>* pieces, uint64_t bi) {
-                for (uint64_t u = 0; u < n;) {
-                    uint64_t m = n - u;
-                    bool moved = false;
-                        for (int k = 0; k < nm; k++) {
-                        if (cf[k] >= SM.f[k].size()) { rc = HT2GPU_ERR_ARG; e = "read front end: a batch ran past the end of its input"; return; }
-                        InFile& F = *SM.f[k][cf[k]];
-                        const uint64_t rem = F.src.nRecords() - cp[k];
-                        if (rem == 0 && F.src.scanDone) { F.exhausted = true; cf[k]++; cp[k] = 0; moved = true; break; }
-                        if (rem < m) m = rem;
-                    }
-                    if (moved) continue;
-                    if (pieces) {
-                        InFile* fb = SM.paired ? SM.f[1][cf[1]].get() : NULL;
-                        SM.f[0][cf[0]]->lastBatch = (int64_t)bi;
-                        if (fb) fb->lastBatch = (int64_t)bi;
-                        Ht2BatchPiece pc = {&SM.f[0][cf[0]]->src, fb ? &fb->src : NULL, cp[0], SM.paired ? cp[1] : 0, m, r + u};
-                        pieces->push_back(pc);
-                    }
-                    for (int k = 0; k < nm; k++) cp[k] += m;
-                    u += m;
-                }
-                for (int k = 0; k < nm; k++)   // a file read to its end is let go at once
-                    while (cf[k] < SM.f[k].size() && SM.f[k][cf[k]]->src.scanDone && cp[k] == SM.f[k][cf[k]]->src.nRecords()) {
-                        SM.f[k][cf[k]]->exhausted = true; cf[k]++; cp[k] = 0;
-                    }
-            };
-            // the units [r, r + want) that are there, or 0 at the end of the stream; a pair with only one mate is an error
-            auto next = [&](uint64_t r, uint64_t want) -> uint64_t {
-                const double ti = nowS();
-                uint64_t n = ~(uint64_t)0, av[2] = {0, 0}; bool ended[2] = {false, false};
-                for (int k = 0; k < nm && rc == HT2GPU_OK; k++) { av[k] = indexAhead(k, want, ended[k]); if (av[k] < n) n = av[k]; }
-                indexS += nowS() - ti;
-                if (rc != HT2GPU_OK) return 0;
-                if (SM.paired && av[0] != av[1] && ended[av[0] < av[1] ? 0 : 1] && r + n < rEnd) {
-                    rc = HT2GPU_ERR_ARG;
-                    e = av[0] < av[1] ? "fewer reads in file specified with -1 than in file specified with -2"
-                                      : "fewer reads in file specified with -2 than in file specified with -1";
-                    return 0;
-                }
-                return n;
-            };
+        for (size_t s = 0; s < streams.size(); s++) {
+            StreamCursor cur{streams[s], s + 1 < streams.size() ? &streams[s + 1] : NULL, device, ro.fastq, *C->pool, {0, 0}, {0, 0}};
+            const uint64_t perBatch = streams[s].paired ? (perRead + 1) / 2 : perRead;   // batch_reads counts reads, a unit here may be a pair
             uint64_t r = 0;
-            while (r < r0 && rc == HT2GPU_OK) {   // -s: the skipped records are indexed, not parsed
-                const uint64_t want = r0 - r < perBatch ? r0 - r : perBatch;
-                const uint64_t n = next(r, want);
+            while (r < r0) {   // -s: the skipped records are indexed, not parsed
+                if (!index(cur, r, r0 - r < perBatch ? r0 - r : perBatch, n)) return;
                 if (n == 0) break;
-                take(r, n, NULL, 0);
+                if (!cur.take(r, n, NULL, 0, false, e)) { fail(HT2GPU_ERR_ARG, e); return; }
                 r += n;
             }
             bool more = true;   // the stream has units left
-            while (rc == HT2GPU_OK && r >= r0) {
+            while (r >= r0) {
                 const int slot = (int)(i % (uint64_t)nSlots);
-                { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return state[slot] == 0 || prodRc != HT2GPU_OK; }); if (prodRc != HT2GPU_OK) { rc = prodRc; break; } }
+                { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return state[slot] == 0 || rc != HT2GPU_OK; }); if (rc != HT2GPU_OK) return; }
                 uint64_t want = (i == 0 && perBatch >= 8) ? perBatch / 4 : perBatch;
                 if (r + want > rEnd) want = rEnd > r ? rEnd - r : 0;
-                const uint64_t n = want ? next(r, want) : 0;
-                if (rc != HT2GPU_OK) break;
+                n = 0;
+                if (want && !index(cur, r, want, n)) return;
                 if (n == 0) { more = want == 0; break; }   // cut by -u, or nothing left
-                pcs.clear();
-                take(r, n, &pcs, i);
-                if (rc == HT2GPU_OK) {
-                    const double tp = nowS();
-                    if (!ht2_parse_pieces(pcs.data(), pcs.size(), ro, stage[slot], pool, C->scratch, e)) rc = HT2GPU_ERR_ARG;
-                    parseS += nowS() - tp;
-                }
-                if (rc == HT2GPU_OK) {
-                    SlotRecs& sr = recs[slot];
-                    sr.paired = SM.paired;
-                    sr.pcs.resize(pcs.size());
-                    // the cursor has moved past these records: find each piece's files again from the sources
-                    for (size_t q = 0; q < pcs.size(); q++) {
-                        RecPiece& rp = sr.pcs[q];
-                        rp.fa = rp.fb = NULL;
-                        for (int k = 0; k < nm; k++)
-                            for (auto& F : SM.f[k]) if (&F->src == (k ? pcs[q].b : pcs[q].a)) { (k ? rp.fb : rp.fa) = F.get(); break; }
-                        rp.da = pcs[q].a->data; rp.db = pcs[q].b ? pcs[q].b->data : NULL;
-                        rp.ra = pcs[q].ra; rp.rb = pcs[q].rb; rp.n = pcs[q].n;
-                        if (route) {
-                            rp.a.assign(pcs[q].a->rec.begin() + (ptrdiff_t)rp.ra, pcs[q].a->rec.begin() + (ptrdiff_t)(rp.ra + rp.n) + 1);
-                            if (pcs[q].b) rp.b.assign(pcs[q].b->rec.begin() + (ptrdiff_t)rp.rb, pcs[q].b->rec.begin() + (ptrdiff_t)(rp.rb + rp.n) + 1);
-                        }
-                    }
-                }
-                if (rc == HT2GPU_OK) {
-                    Ht2HostBatch& hb = stage[slot];
-                    ht2gpu_read_batch_t rb; memset(&rb, 0, sizeof(rb));
-                    rb.n_reads = hb.n_reads; rb.paired = SM.paired ? 1 : 0; rb.seq = hb.seq; rb.qual = hb.haveQual ? hb.qual : NULL; rb.offs = hb.offs; rb.seeds = hb.seeds;
-                    const double ts = nowS();
-                    rc = ht2gpu_submit_sam(hs[slot % nDev], slot / nDev, &rb, hb.names, hb.nameOffs, hb.namesBytes);
-                    submitS += nowS() - ts;
-                    if (rc != HT2GPU_OK) e = ht2gpu_last_error(hs[slot % nDev]);
-                }
-                if (rc != HT2GPU_OK) break;
-                std::lock_guard<std::mutex> lk(mu);
-                state[slot] = 1; submitted = ++i;
+                SlotBatch& b = batches[slot];
+                if (!cur.take(r, n, &b, (int64_t)i, route, e)) { fail(HT2GPU_ERR_ARG, e); return; }
+                Ht2HostBatch& hb = C->stage[slot];
+                const double tp = nowS();
+                const bool parsed = ht2_parse_pieces(b.pcs.data(), b.pcs.size(), ro, hb, *C->pool, C->scratch, e);
+                parseS += nowS() - tp;
+                if (!parsed) { fail(HT2GPU_ERR_ARG, e); return; }
+                ht2gpu_read_batch_t rb; memset(&rb, 0, sizeof(rb));
+                rb.n_reads = hb.n_reads; rb.paired = streams[s].paired ? 1 : 0; rb.seq = hb.seq; rb.qual = hb.haveQual ? hb.qual : NULL; rb.offs = hb.offs; rb.seeds = hb.seeds;
+                const double ts = nowS();
+                const int src = ht2gpu_submit_sam(hs[slot % nDev], slot / nDev, &rb, hb.names, hb.nameOffs, hb.namesBytes);
+                submitS += nowS() - ts;
+                if (src != HT2GPU_OK) { fail(src, ht2gpu_last_error(hs[slot % nDev])); return; }
+                { std::lock_guard<std::mutex> lk(mu); state[slot] = 1; submitted = ++i; cv.notify_all(); }
                 r += n;
-                cv.notify_all();
             }
             // cut by -u: the read loop ends at the first unit with rdid >= skip + upto, if there is one
-            if (rc == HT2GPU_OK && more && s + 1 < nStreams && next(r, 1) > 0) break;
+            if (more && s + 1 < streams.size() && (!index(cur, r, 1, n) || n > 0)) return;
         }
-        std::lock_guard<std::mutex> lk(mu);
-        if (rc != HT2GPU_OK && prodRc == HT2GPU_OK) { prodRc = rc; prodErr = e; }
-        prodDone = true;
-        cv.notify_all();
-    });
+    }
 
-    int rc = HT2GPU_OK;
-    double routeS = 0;
-    Router router(routes, fastq);
-    for (uint64_t i = 0; ; i++) {
-        const int slot = (int)(i % (uint64_t)nSlots);
-        {
-            std::unique_lock<std::mutex> lk(mu);
-            cv.wait(lk, [&] { return submitted > i || prodRc != HT2GPU_OK || prodDone; });
-            if (submitted <= i) { rc = prodRc; break; }   // the producer has finished (or failed)
-        }
-        ht2gpu_sam_result_t r;
-        const double tw = nowS();
-        rc = ht2gpu_wait_sam(hs[slot % nDev], slot / nDev, &r);
-        waitS += nowS() - tw;
-        if (rc != HT2GPU_OK) { prodErr = ht2gpu_last_error(hs[slot % nDev]); break; }
-        S.n_batches++; S.n_units += r.n_units; S.n_reads += stage[slot].n_reads; S.sam_bytes += r.sam_len; S.n_err_reads += r.n_err_reads;
-        S.ms_align += r.ms_align; S.ms_sam += r.ms_sam; S.ms_h2d += r.ms_h2d; S.ms_d2h += r.ms_d2h;
-        S.h2d_bytes += r.h2d_bytes; S.d2h_bytes += r.d2h_bytes; S.n_launches += r.n_launches;
-        const SlotRecs& sr = recs[slot];
-        for (const RecPiece& rp : sr.pcs)   // nothing of a gzip file leaves the run before the file is verified
-            for (InFile* F : {rp.fa, rp.fb})
-                if (F && F->gz && !F->verified && rc == HT2GPU_OK) { rc = F->gz->verified(prodErr); F->verified = rc == HT2GPU_OK; }
-        const double tk = nowS();
-        if (rc == HT2GPU_OK && sink && r.sam_len) { if (sink(ctx, r.sam, r.sam_len) != 0) { rc = HT2GPU_ERR_ARG; prodErr = "the SAM sink reported an error"; } }
-        sinkS += nowS() - tk;
-        if (route && rc == HT2GPU_OK) {
-            const double tr = nowS();
-            const uint8_t* ob = NULL; uint32_t nu = 0;
-            rc = ht2gpu_unit_outcomes(hs[slot % nDev], slot / nDev, &ob, &nu);
-            if (rc != HT2GPU_OK) prodErr = ht2gpu_last_error(hs[slot % nDev]);
-            else {
-                uint64_t u = 0;
-                for (const RecPiece& rp : sr.pcs) {
-                    if (u + rp.n > nu) break;
-                    router.batch(rp.da, rp.a.data(), rp.ra, rp.db, sr.paired ? rp.b.data() : NULL, rp.rb, rp.n, ob + u);
-                    u += rp.n;
-                }
-                if (router.rc) { rc = HT2GPU_ERR_ARG; prodErr = "the read-file writer reported an error"; }
+    // The caller's thread waits for the batches in order, hands their SAM to the sink (nothing of a gzip file before
+    // the file is verified), routes their records and lets go of the files the producer has left.
+    void consume()
+    {
+        for (uint64_t i = 0; ; i++) {
+            const int slot = (int)(i % (uint64_t)nSlots);
+            ht2gpu_handle_t* hd = hs[slot % nDev];
+            {
+                std::unique_lock<std::mutex> lk(mu);
+                cv.wait(lk, [&] { return submitted > i || rc != HT2GPU_OK || prodDone; });
+                if (submitted <= i) return;   // the producer has finished (or failed)
             }
+            ht2gpu_sam_result_t r;
+            const double tw = nowS();
+            const int wrc = ht2gpu_wait_sam(hd, slot / nDev, &r);
+            waitS += nowS() - tw;
+            if (wrc != HT2GPU_OK) { fail(wrc, ht2gpu_last_error(hd)); return; }
+            S.n_batches++; S.n_units += r.n_units; S.n_reads += C->stage[slot].n_reads; S.sam_bytes += r.sam_len; S.n_err_reads += r.n_err_reads;
+            S.ms_align += r.ms_align; S.ms_sam += r.ms_sam; S.ms_h2d += r.ms_h2d; S.ms_d2h += r.ms_d2h;
+            S.h2d_bytes += r.h2d_bytes; S.d2h_bytes += r.d2h_bytes; S.n_launches += r.n_launches;
+            const SlotBatch& b = batches[slot];
+            bool ok = true;
+            std::string e;
+            for (const RecPiece& rp : b.recs)
+                for (InFile* F : rp.f) { const int v = ok && F ? F->verify(e) : HT2GPU_OK; if (v) ok = fail(v, e); }
+            const double tk = nowS();
+            if (ok && sink && r.sam_len && sink(ctx, r.sam, r.sam_len) != 0) ok = fail(HT2GPU_ERR_ARG, "the SAM sink reported an error");
+            sinkS += nowS() - tk;
+            if (route && ok) {
+                const double tr = nowS();
+                const uint8_t* ob = NULL; uint32_t nu = 0;
+                const int orc = ht2gpu_unit_outcomes(hd, slot / nDev, &ob, &nu);
+                if (orc != HT2GPU_OK) ok = fail(orc, ht2gpu_last_error(hd));
+                for (uint64_t q = 0, u = 0; ok && q < b.pcs.size() && u + b.pcs[q].n <= nu; u += b.pcs[q++].n) {
+                    const Ht2BatchPiece& pc = b.pcs[q];
+                    router.batch(pc.a->data, b.recs[q].rec[0].data(), pc.ra, pc.b ? pc.b->data : NULL, pc.b ? b.recs[q].rec[1].data() : NULL,
+                                 pc.rb, pc.n, ob + u);
+                }
+                if (ok && router.rc) ok = fail(HT2GPU_ERR_ARG, "the read-file writer reported an error");
+                routeS += nowS() - tr;
+            }
+            // files the producer has left whose last batch is done: their text (and address space) is let go
+            bool flushed = false;
+            for (InFile* F : files)
+                if (!F->released && F->exhausted && F->lastBatch <= (int64_t)i) {
+                    if (route && !flushed) { router.finish(); flushed = true; }   // no pending span may point into it
+                    F->release(C->gz);
+                }
+            { std::lock_guard<std::mutex> lk(mu); state[slot] = 0; cv.notify_all(); }
+            if (!ok) return;
+        }
+    }
+
+    // After both threads: the gzip files read from are verified, the router finished, the batches still in flight
+    // after an error drained, every file let go and the stats filled.
+    int finish(double t0, ht2gpu_run_stats_t* st)
+    {
+        std::string e;
+        // a gzip file that was read from (or read to its end) is verified before the run succeeds; one whose records
+        // were never needed (-u) is stopped
+        for (InFile* F : files)
+            if (rc == HT2GPU_OK && !F->released && (F->exhausted || F->lastBatch >= 0)) { const int v = F->verify(e); if (v) fail(v, e); }
+        if (rc != HT2GPU_OK)   // a failed inflate explains a failed run better than what the parser made of its bytes
+            for (InFile* F : files) { const int z = F->verify(e, false); if (z) { std::lock_guard<std::mutex> lk(mu); rc = z; err = e; } }
+        if (route) {
+            const double tr = nowS();
+            router.finish();
+            if (router.rc) fail(HT2GPU_ERR_ARG, "the read-file writer reported an error");
             routeS += nowS() - tr;
+            routes->s_route = routeS;
+            for (int i = 0; i < nDev; i++) ht2gpu_record_outcomes(hs[i], 0);
         }
-        // files the producer has left whose last batch is done: their text (and address space) is let go
-        bool flushed = false;
-        for (auto& sm : streams)
-            for (auto& v : sm.f)
-                for (auto& F : v)
-                    if (!F->closed && F->exhausted && F->lastBatch <= (int64_t)i) {
-                        if (route && !flushed) { router.finish(); flushed = true; }   // no pending span may point into it
-                        closeFile(*F);
-                    }
-        { std::lock_guard<std::mutex> lk(mu); state[slot] = 0; if (rc != HT2GPU_OK) prodRc = rc; cv.notify_all(); }
-        if (rc != HT2GPU_OK) break;
+        if (rc != HT2GPU_OK)   // drain the batches still in flight
+            for (int s = 0; s < nSlots; s++) if (state[s] == 1) { ht2gpu_sam_result_t r; ht2gpu_wait_sam(hs[s % nDev], s / nDev, &r); }
+        for (InFile* F : files) F->release(C->gz);
+        S.s_index = indexS; S.s_parse = parseS; S.s_submit = submitS; S.s_wait = waitS; S.s_sink = sinkS; S.s_total = nowS() - t0;
+        if (st) *st = S;
+        if (rc != HT2GPU_OK) ht2gpu_set_error(hs[0], err.empty() ? "ht2gpu_run_reads failed" : err.c_str());
+        return rc;
     }
-    { std::lock_guard<std::mutex> lk(mu); if (rc != HT2GPU_OK && prodRc == HT2GPU_OK) prodRc = rc; cv.notify_all(); }
-    producer.join();
-    if (rc == HT2GPU_OK && prodRc != HT2GPU_OK) { rc = prodRc; }
-    // a gzip file that was read from (or read to its end) is verified before the run succeeds; one whose records were
-    // never needed (-u) is stopped
-    eachFile([&](InFile& F) {
-        if (rc == HT2GPU_OK && F.gz && F.started && !F.closed && !F.verified && (F.exhausted || F.lastBatch >= 0)) rc = F.gz->verified(prodErr);
-    });
-    eachFile([&](InFile& F) {   // a failed inflate explains a failed run better than what the parser made of its bytes
-        if (F.gz && F.started && rc != HT2GPU_OK) {
-            std::lock_guard<std::mutex> lk(F.gz->stream.mu);
-            if (F.gz->stream.done && F.gz->stream.rc) { rc = F.gz->stream.rc; prodErr = F.gz->stream.err; }
-        }
-    });
-    if (route) {
-        const double tr = nowS();
-        router.finish();
-        if (router.rc && rc == HT2GPU_OK) { rc = HT2GPU_ERR_ARG; prodErr = "the read-file writer reported an error"; }
-        routeS += nowS() - tr;
-        routes->s_route = routeS;
-        for (int i = 0; i < nDev; i++) ht2gpu_record_outcomes(hs[i], 0);
-    }
-    // drain anything still in flight after an error
-    if (rc != HT2GPU_OK) for (int s = 0; s < nSlots; s++) if (state[s] == 1) { ht2gpu_sam_result_t r; ht2gpu_wait_sam(hs[s % nDev], s / nDev, &r); }
-    eachFile(closeFile);
-    S.s_index = indexS; S.s_parse = parseS; S.s_submit = submitS; S.s_wait = waitS; S.s_sink = sinkS; S.s_total = nowS() - t0;
-    if (st) *st = S;
-    if (rc != HT2GPU_OK) ht2gpu_set_error(h, prodErr.empty() ? "ht2gpu_run_reads failed" : prodErr.c_str());
-    return rc;
-}
+};
 }
 
 // The same pipeline over several devices of one process (hisat2-b200 --gpus N): batch i goes to handle i % n,
@@ -552,10 +584,11 @@ extern "C" int ht2gpu_run_reads_routed(ht2gpu_handle_t** hs, int nDev, const ht2
     if (!hs || nDev < 1 || !in) return HT2GPU_ERR_ARG;
     for (int i = 0; i < nDev; i++) if (!hs[i]) return HT2GPU_ERR_ARG;
     if (!in->path1 && !in->data1) { ht2gpu_set_error(hs[0], "ht2gpu_run_reads: no input"); return HT2GPU_ERR_ARG; }
-    std::vector<InputSpec> sp[2];
-    sp[0].push_back({in->path1, in->data1, in->len1});
-    if (in->path2 || in->data2) sp[1].push_back({in->path2, in->data2, in->len2});
-    return runStreams(hs, nDev, sp, 1, !sp[1].empty(), in, sink, ctx, routes, st);
+    std::vector<StreamSpec> ss(1);
+    ss[0].paired = in->path2 || in->data2;
+    ss[0].files[0].push_back({in->path1, in->data1, in->len1});
+    if (ss[0].paired) ss[0].files[1].push_back({in->path2, in->data2, in->len2});
+    return Run(hs, nDev, in, sink, ctx, routes).exec(ss, st);
 }
 
 // Read-file lists: every -1 / -2 file back to back as one paired stream, then every -U file as one unpaired stream.
@@ -570,7 +603,9 @@ extern "C" int ht2gpu_run_reads_files(ht2gpu_handle_t** hs, int nDev, const ht2g
         return refuse(std::to_string(files->n1) + " mate files/sequences were specified with -1, but " + std::to_string(files->n2) +
                       "\nmate files/sequences were specified with -2.  The same number of mate files/\nsequences must be specified with -1 and -2.");
     if (files->n1 + files->n_u == 0) return refuse("ht2gpu_run_reads_files: no input");
-    std::vector<InputSpec> sp[4];
+    std::vector<StreamSpec> ss;
+    if (files->n1) ss.push_back(StreamSpec{true, {}});
+    if (files->n_u) ss.push_back(StreamSpec{false, {}});
     int stdinUses = 0;
     const char* const* lists[3] = {files->paths1, files->paths2, files->paths_u};
     const uint32_t counts[3] = {files->n1, files->n2, files->n_u};
@@ -580,10 +615,38 @@ extern "C" int ht2gpu_run_reads_files(ht2gpu_handle_t** hs, int nDev, const ht2g
             const char* p = lists[l][j];
             if (!p || !*p) return refuse("ht2gpu_run_reads_files: an empty read file name");
             if (strcmp(p, "-") == 0 && ++stdinUses > 1) return refuse("standard input ('-') can be read only once");
-            sp[files->n1 ? l : 0].push_back({p, NULL, 0});
+            (l < 2 ? ss[0].files[l] : ss.back().files[0]).push_back({p, NULL, 0});
         }
     }
-    return runStreams(hs, nDev, sp, (files->n1 ? 1 : 0) + (files->n_u ? 1 : 0), files->n1 != 0, in, sink, ctx, routes, st);
+    return Run(hs, nDev, in, sink, ctx, routes).exec(ss, st);
+}
+
+namespace {
+// The whole input of the host-only calls: opened, indexed, mate counts checked, and the units [r0, r1) after -s / -u.
+struct WholeInput {
+    Ht2ThreadPool pool;
+    Ht2ReadSource a, b;
+    const bool paired;
+    uint64_t r0 = 0, r1 = 0;
+    explicit WholeInput(const ht2gpu_reads_input_t* in) : pool(threadCount(in)), paired(in->path2 != NULL || in->data2 != NULL) {}
+    ~WholeInput() { ht2_source_close(a); ht2_source_close(b); }
+    bool open(const ht2gpu_reads_input_t* in, std::string& err)
+    {
+        if (!in->path1 && !in->data1) { err = "no input"; return false; }
+        if (!openSpec(a, {in->path1, in->data1, in->len1}, err) || (paired && !openSpec(b, {in->path2, in->data2, in->len2}, err))) return false;
+        if (refuseCompressed(a, err) || refuseCompressed(b, err)) return false;
+        if (!ht2_source_index(a, in->format == 1, pool, err) || (paired && !ht2_source_index(b, in->format == 1, pool, err))) return false;
+        if (paired && a.nRecords() != b.nRecords()) { err = "mate files have different numbers of reads"; return false; }
+        r0 = in->skip < a.nRecords() ? in->skip : a.nRecords(); r1 = a.nRecords();
+        if (in->upto && r0 + in->upto < r1) r1 = r0 + in->upto;
+        return true;
+    }
+};
+int errOut(char* errbuf, size_t errbuf_len, const std::string& m)
+{
+    if (errbuf && errbuf_len) { strncpy(errbuf, m.c_str(), errbuf_len - 1); errbuf[errbuf_len - 1] = 0; }
+    return HT2GPU_ERR_ARG;
+}
 }
 
 // Host-only: parse a whole input into ONE batch (malloc'ed buffers).  No device is touched: this is the read
@@ -592,35 +655,13 @@ extern "C" int ht2gpu_parse_reads(const ht2gpu_reads_input_t* in, ht2gpu_parsed_
 {
     if (!in || !out) return HT2GPU_ERR_ARG;
     memset(out, 0, sizeof(*out));
-    auto fail = [&](const std::string& m) { if (errbuf && errbuf_len) { strncpy(errbuf, m.c_str(), errbuf_len - 1); errbuf[errbuf_len - 1] = 0; } return HT2GPU_ERR_ARG; };
-    unsigned nth = in->threads > 0 ? (unsigned)in->threads : std::thread::hardware_concurrency();
-    if (nth < 1) nth = 1;
-    if (nth > 64) nth = 64;
-    Ht2ThreadPool pool(nth);
-    Ht2ReadSource a, b;
+    WholeInput w(in);
     std::string err;
-    const bool paired = in->path2 != NULL || in->data2 != NULL;
-    if (in->path1) { if (!ht2_source_open(a, in->path1, err)) return fail(err); }
-    else if (in->data1) ht2_source_memory(a, in->data1, in->len1);
-    else return fail("no input");
-    if (in->path2) { if (!ht2_source_open(b, in->path2, err)) { ht2_source_close(a); return fail(err); } }
-    else if (in->data2) ht2_source_memory(b, in->data2, in->len2);
-    if (refuseCompressed(a, err) || refuseCompressed(b, err)) { ht2_source_close(a); ht2_source_close(b); return fail(err); }
-    const bool fastq = in->format == 1;
-    bool ok = ht2_source_index(a, fastq, pool, err) && (!paired || ht2_source_index(b, fastq, pool, err));
-    if (ok && paired && a.nRecords() != b.nRecords()) { ok = false; err = "mate files have different numbers of reads"; }
+    if (!w.open(in, err)) return errOut(errbuf, errbuf_len, err);
     Ht2HostBatch* hb = new Ht2HostBatch();
-    if (ok) {
-        uint64_t r0 = in->skip, r1 = a.nRecords();
-        if (r0 > r1) r0 = r1;
-        if (in->upto && r0 + in->upto < r1) r1 = r0 + in->upto;
-        Ht2ReadsOpts ro; ro.fastq = fastq; ro.trim5 = in->trim5; ro.trim3 = in->trim3; ro.phred64 = in->phred64 != 0; ro.seed = in->seed;
-        Ht2ParseScratch scratch;
-        ok = ht2_parse_batch(a, paired ? &b : NULL, r0, r1, ro, *hb, pool, scratch, err);
-    }
-    ht2_source_close(a); ht2_source_close(b);
-    if (!ok) { hb->freeAll(); delete hb; return fail(err); }
-    out->batch.n_reads = hb->n_reads; out->batch.paired = paired ? 1 : 0; out->batch.seq = hb->seq; out->batch.qual = hb->haveQual ? hb->qual : NULL;
+    Ht2ParseScratch scratch;
+    if (!ht2_parse_batch(w.a, w.paired ? &w.b : NULL, w.r0, w.r1, readsOpts(in), *hb, w.pool, scratch, err)) { hb->freeAll(); delete hb; return errOut(errbuf, errbuf_len, err); }
+    out->batch.n_reads = hb->n_reads; out->batch.paired = w.paired ? 1 : 0; out->batch.seq = hb->seq; out->batch.qual = hb->haveQual ? hb->qual : NULL;
     out->batch.offs = hb->offs; out->batch.seeds = hb->seeds;
     out->names = hb->names; out->name_offs = hb->nameOffs; out->names_bytes = hb->namesBytes; out->priv = hb;
     return HT2GPU_OK;
@@ -631,40 +672,19 @@ extern "C" int ht2gpu_route_reads(const ht2gpu_reads_input_t* in, const uint8_t*
 {
     if (!in || !routes || (n_units && !outcomes) || (routes->mask && !routes->write)) return HT2GPU_ERR_ARG;
     routes->n_spans = 0; routes->bytes = 0; routes->s_route = 0;
-    auto fail = [&](const std::string& m) { if (errbuf && errbuf_len) { strncpy(errbuf, m.c_str(), errbuf_len - 1); errbuf[errbuf_len - 1] = 0; } return HT2GPU_ERR_ARG; };
     const double t0 = nowS();
-    unsigned nth = in->threads > 0 ? (unsigned)in->threads : std::thread::hardware_concurrency();
-    if (nth < 1) nth = 1;
-    if (nth > 64) nth = 64;
-    Ht2ThreadPool pool(nth);
-    Ht2ReadSource a, b;
+    WholeInput w(in);
     std::string err;
-    const bool paired = in->path2 != NULL || in->data2 != NULL;
-    if (in->path1) { if (!ht2_source_open(a, in->path1, err)) return fail(err); }
-    else if (in->data1) ht2_source_memory(a, in->data1, in->len1);
-    else return fail("no input");
-    if (in->path2) { if (!ht2_source_open(b, in->path2, err)) { ht2_source_close(a); return fail(err); } }
-    else if (in->data2) ht2_source_memory(b, in->data2, in->len2);
-    if (refuseCompressed(a, err) || refuseCompressed(b, err)) { ht2_source_close(a); ht2_source_close(b); return fail(err); }
-    const bool fastq = in->format == 1;
-    bool ok = ht2_source_index(a, fastq, pool, err) && (!paired || ht2_source_index(b, fastq, pool, err));
-    if (ok && paired && a.nRecords() != b.nRecords()) { ok = false; err = "mate files have different numbers of reads"; }
-    uint64_t r0 = in->skip, r1 = a.nRecords();
-    if (r0 > r1) r0 = r1;
-    if (in->upto && r0 + in->upto < r1) r1 = r0 + in->upto;
-    if (ok && r1 - r0 != n_units) { ok = false; err = "the outcomes do not cover the input's " + std::to_string(r1 - r0) + " units"; }
-    int rc = HT2GPU_OK;
+    bool ok = w.open(in, err);
+    if (ok && w.r1 - w.r0 != n_units) { ok = false; err = "the outcomes do not cover the input's " + std::to_string(w.r1 - w.r0) + " units"; }
     if (ok && routes->mask) {
-        Router router(routes, fastq);
-        router.batch(a.data, a.rec.data() + r0, r0, b.data, paired ? b.rec.data() + r0 : NULL, r0, r1 - r0, outcomes);
+        Router router(routes, in->format == 1);
+        router.batch(w.a.data, w.a.rec.data() + w.r0, w.r0, w.b.data, w.paired ? w.b.rec.data() + w.r0 : NULL, w.r0, w.r1 - w.r0, outcomes);
         router.finish();
-        if (router.rc) { rc = HT2GPU_ERR_ARG; err = "the read-file writer reported an error"; }
+        if (router.rc) { ok = false; err = "the read-file writer reported an error"; }
     }
-    ht2_source_close(a); ht2_source_close(b);
     routes->s_route = nowS() - t0;
-    if (!ok) return fail(err);
-    if (rc) return fail(err);
-    return HT2GPU_OK;
+    return ok ? HT2GPU_OK : errOut(errbuf, errbuf_len, err);
 }
 
 extern "C" void ht2gpu_free_parsed(ht2gpu_parsed_reads_t* p)
