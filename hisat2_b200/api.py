@@ -26,7 +26,12 @@ class Options(C.Structure):
         "ignore_quals", "nofw", "norc", "min_frag", "max_frag", "no_mixed", "no_discordant")] + [
         ("seed", C.c_uint32), ("threads_per_block", C.c_int32), ("blocks_per_sm", C.c_int32), ("slots_per_lane", C.c_int32), ("warp_per_read", C.c_int32),
         ("bowtie2_dp", C.c_int32), ("gbar", C.c_int32), ("score_min_type", C.c_int32),
-        ("score_min_const", C.c_double), ("score_min_coeff", C.c_double)]
+        ("score_min_const", C.c_double), ("score_min_coeff", C.c_double), ("chr_names", C.c_int32)]
+
+# Index(chr_names=...): the reference names of --remove-chrname / --add-chrname (ht2gpu_options_t.chr_names)
+CHR_NAMES = {None: 0, "remove": 1, "add": 2}
+# set_sam_output(rna_strandness=...): --rna-strandness, numbered as ht2gpu_sam_output_t.rna_strandness
+RNA_STRANDNESS = {None: 0, "F": 1, "R": 2, "FR": 3, "RF": 4}
 
 
 class CReadBatch(C.Structure):
@@ -165,7 +170,8 @@ def route_reads(outcomes, path1=None, path2=None, data1=None, data2=None, fastq=
 
 class CSamOutput(C.Structure):
     _fields_ = [("no_unal", C.c_int32), ("omit_sec_seq", C.c_int32), ("no_sq", C.c_int32), ("rg_id", C.c_char_p),
-                ("rg", C.POINTER(C.c_char_p)), ("n_rg", C.c_int32)]
+                ("rg", C.POINTER(C.c_char_p)), ("n_rg", C.c_int32), ("rna_strandness", C.c_int32),
+                ("no_qname_trunc", C.c_int32), ("no_templatelen_adjustment", C.c_int32)]
 
 
 # ReportingMetrics of ht2gpu_align_counts_t, in its field order
@@ -597,17 +603,29 @@ class SeedResult(object):
             pass
 
 
+def _options(lib, opts):
+    """ht2gpu_options_t: the defaults, then opts (chr_names by name, see CHR_NAMES)."""
+    o = Options()
+    lib.ht2gpu_default_options(C.byref(o))
+    for k, v in opts.items():
+        if k == "chr_names":
+            if v not in CHR_NAMES:
+                raise ValueError("chr_names must be 'remove', 'add' or None, not %r" % (v,))
+            v = CHR_NAMES[v]
+        setattr(o, k, v)
+    return o
+
+
 class Index(object):
     """Device-resident HISAT2 index + alignment entry points."""
 
     def __init__(self, base=None, image=None, device_image=None, device=0, **opts):
+        """opts: the fields of ht2gpu_options_t; chr_names is "remove" (--remove-chrname), "add" (--add-chrname) or
+        None (the index's names)."""
         self._lib = load_library()
         self._opts = dict(opts)
-        o = Options()
-        self._lib.ht2gpu_default_options(C.byref(o))
+        o = _options(self._lib, opts)
         o.device = device
-        for k, v in opts.items():
-            setattr(o, k, v)
         self._h = C.c_void_p()
         if base is not None:
             rc = self._lib.ht2gpu_open(os.fsencode(base), C.byref(o), C.byref(self._h))
@@ -698,15 +716,22 @@ class Index(object):
         self._check(self._lib.ht2gpu_write_novel_splicesites(hs, 1 + len(peers), path.encode(), C.byref(n)), "ht2gpu_write_novel_splicesites")
         return int(n.value)
 
-    def set_sam_output(self, no_unal=False, omit_sec_seq=False, no_sq=False, rg_id=None, rg=()):
+    def set_sam_output(self, no_unal=False, omit_sec_seq=False, no_sq=False, rg_id=None, rg=(), rna_strandness=None,
+                       no_qname_trunc=False, no_templatelen_adjustment=False):
         """ht2gpu_set_sam_output: --no-unal, --omit-sec-seq, --no-sq, --rg-id and the extra --rg fields of the @RG
-        line (printed only with an rg_id).  Applies to the batches that follow and to sam_header()."""
+        line (printed only with an rg_id), --rna-strandness ("F", "R", "FR", "RF" or None), --sam-no-qname-trunc and
+        --no-templatelen-adjustment.  Applies to the batches that follow and to sam_header()."""
+        if rna_strandness not in RNA_STRANDNESS:
+            raise ValueError("rna_strandness must be one of F, R, FR, RF or None, not %r" % (rna_strandness,))
         rg = [r.encode() if isinstance(r, str) else bytes(r) for r in rg]
         arr = (C.c_char_p * max(1, len(rg)))(*rg)
         cfg = CSamOutput(int(bool(no_unal)), int(bool(omit_sec_seq)), int(bool(no_sq)),
-                         (rg_id.encode() if isinstance(rg_id, str) else rg_id) if rg_id else None, arr, len(rg))
+                         (rg_id.encode() if isinstance(rg_id, str) else rg_id) if rg_id else None, arr, len(rg),
+                         RNA_STRANDNESS[rna_strandness], int(bool(no_qname_trunc)), int(bool(no_templatelen_adjustment)))
         self._check(self._lib.ht2gpu_set_sam_output(self._h, C.byref(cfg)), "ht2gpu_set_sam_output")
-        self._sam_output = dict(no_unal=no_unal, omit_sec_seq=omit_sec_seq, no_sq=no_sq, rg_id=rg_id, rg=tuple(rg))
+        self._sam_output = dict(no_unal=no_unal, omit_sec_seq=omit_sec_seq, no_sq=no_sq, rg_id=rg_id, rg=tuple(rg),
+                                rna_strandness=rna_strandness, no_qname_trunc=no_qname_trunc,
+                                no_templatelen_adjustment=no_templatelen_adjustment)
 
     def align_counts(self, peers=(), reset=False):
         """ht2gpu_align_counts: the per-read outcome counts (ReportingMetrics) of every batch formatted on the device
@@ -718,10 +743,7 @@ class Index(object):
 
     def peer(self, device):
         """ht2gpu_open_peer: a replica of this index on another device of this process (device-to-device copy)."""
-        o = Options()
-        self._lib.ht2gpu_default_options(C.byref(o))
-        for k, v in self._opts.items():
-            setattr(o, k, v)
+        o = _options(self._lib, self._opts)
         o.device = device
         other = Index.__new__(Index)
         other._lib = self._lib

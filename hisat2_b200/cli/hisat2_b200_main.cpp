@@ -79,6 +79,8 @@ static void usage() {
                     "            [--known-splicesite-infile F] [--novel-splicesite-infile F] [--novel-splicesite-outfile F]\n"
                     "            [--bowtie2-dp 0|1|2] [--score-min F,C,L] [--gbar N] [--sensitive] [--very-sensitive] [--fast]\n"
                     "            [--no-unal] [--omit-sec-seq] [--no-hd] [--no-sq] [--rg-id ID] [--rg TEXT]...\n"
+                    "            [--rna-strandness F|R|FR|RF] [--remove-chrname|--add-chrname] [--no-templatelen-adjustment]\n"
+                    "            [--sam-no-qname-trunc]\n"
                     "            [--summary-file F] [--new-summary] [--quiet]\n"
                     "            [--un P] [--al P] [--un-conc P] [--al-conc P] [--al-conc-disc P], each also as --<opt>-gz\n"
                     "            and --<opt>-bz2: write unpaired reads that did not / did align, pairs that did not / did align\n"
@@ -114,7 +116,7 @@ int main(int argc, char** argv)
     // SAM output (hisat2.cpp:601-623, 1342-1343, 1389-1407): --no-hd prints no header at all (no @PG either,
     // hisat2.cpp:4127-4131); --rg ID:<x> sets the read-group id like --rg-id <x>, any other --rg text is an @RG field
     bool noHd = false, newSummary = false, quiet = false;
-    int32_t noUnal = 0, omitSecSeq = 0, noSq = 0;
+    int32_t noUnal = 0, omitSecSeq = 0, noSq = 0, rnaStrandness = 0, noQnameTrunc = 0, noTlenAdj = 0;
     std::string rgId; std::vector<std::string> rgFields;
     const char* summaryFile = NULL;
     ReadFiles rfs;
@@ -163,6 +165,13 @@ int main(int argc, char** argv)
             std::string v = next();
             if (v.compare(0, 3, "ID:") == 0) rgId = v.substr(3); else rgFields.push_back(v);
         }
+        else if (a == "--rna-strandness") {   // hisat2.cpp:1694-1705; read.h:30-36 numbering
+            const std::string v = next();
+            if (v == "F") rnaStrandness = 1; else if (v == "R") rnaStrandness = 2; else if (v == "FR") rnaStrandness = 3; else if (v == "RF") rnaStrandness = 4;
+            else { fprintf(stderr, "Error: should be one of F, R, FR, or RF \n"); return 1; }
+        }
+        else if (a == "--remove-chrname") o.chr_names |= HT2GPU_CHR_NAMES_REMOVE; else if (a == "--add-chrname") o.chr_names |= HT2GPU_CHR_NAMES_ADD;
+        else if (a == "--no-templatelen-adjustment") noTlenAdj = 1; else if (a == "--sam-no-qname-trunc") noQnameTrunc = 1;
         else if (a == "--summary-file") summaryFile = next(); else if (a == "--new-summary") newSummary = true;
         else if (a == "--quiet") quiet = true;   // no alignment summary (hisat2.cpp:4165)
         else if (a.compare(0, 2, "--") == 0 && [&]() {
@@ -223,6 +232,7 @@ int main(int argc, char** argv)
     ht2gpu_sam_output_t so; memset(&so, 0, sizeof(so));
     so.no_unal = noUnal; so.omit_sec_seq = omitSecSeq; so.no_sq = noSq;
     so.rg_id = rgId.empty() ? NULL : rgId.c_str(); so.rg = rgPtrs.data(); so.n_rg = (int32_t)rgPtrs.size();
+    so.rna_strandness = rnaStrandness; so.no_qname_trunc = noQnameTrunc; so.no_templatelen_adjustment = noTlenAdj;
     if (ht2gpu_set_sam_output(h, &so) != HT2GPU_OK) { fprintf(stderr, "Error: %s\n", ht2gpu_last_error(h)); return 1; }
     if (!noHd) {
         char* hd; size_t hl; ht2gpu_sam_header(h, &hd, &hl); fwrite(hd, 1, hl, fo); ht2gpu_free_text(hd);

@@ -699,6 +699,8 @@ struct ht2gpu_handle {
     uint8_t*       dBlob;
     bool           ownBlob;
     size_t         blobBytes;
+    Ht2RefNames    refNames;   // the reference names of opt.chr_names (SAM, splice-site files) ...
+    uint8_t*       dRefNames;  // ... and their copy on the device, next to the index image
     Ht2Params      P;
     ht2gpu_options_t opt;
     int            device;
@@ -815,6 +817,9 @@ static int finishOpen(ht2gpu_handle* h)
     }
 #endif
     h->graph = !H->global.linearFM;   // graph (SNP) indexes: ALT-aware aligner instantiation, graph seed kernel
+    h->refNames.build(*h->img, h->opt.chr_names);
+    CK(cudaMalloc(&h->dRefNames, h->refNames.blob.size()));
+    CK(cudaMemcpy(h->dRefNames, h->refNames.blob.data(), h->refNames.blob.size(), cudaMemcpyHostToDevice));
     applyOptions(h->P, *h->img, h->opt);
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, h->device));
@@ -912,8 +917,12 @@ static ht2gpu_handle* newHandle(const ht2gpu_options_t* opt)
     return h;
 }
 
-static int selectDevice(ht2gpu_handle* h)
+// Every ht2gpu_open*: refuse the options that need no device to refuse, then select the handle's device
+static int startOpen(ht2gpu_handle* h)
 {
+    const int32_t cn = h->opt.chr_names;
+    if (cn == (HT2GPU_CHR_NAMES_REMOVE | HT2GPU_CHR_NAMES_ADD)) { h->err = "--remove-chrname and --add-chrname cannot be used at the same time"; return HT2GPU_ERR_ARG; }
+    if (cn != HT2GPU_CHR_NAMES_INDEX && cn != HT2GPU_CHR_NAMES_REMOVE && cn != HT2GPU_CHR_NAMES_ADD) { h->err = "chr_names must be 0, 1 (remove) or 2 (add)"; return HT2GPU_ERR_ARG; }
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n <= 0) {
@@ -945,7 +954,7 @@ extern "C" int ht2gpu_open_image(const void* image, size_t bytes, const ht2gpu_o
     if (!image || !out || bytes < sizeof(Ht2ImageHeader)) return HT2GPU_ERR_ARG;
     ht2gpu_handle* h = newHandle(opt);
     *out = h;
-    int rc = selectDevice(h);
+    int rc = startOpen(h);
     if (rc) return rc;
     h->img = new Ht2Image();
     h->img->blob.assign((const uint8_t*)image, (const uint8_t*)image + bytes);
@@ -962,7 +971,7 @@ extern "C" int ht2gpu_open_device_image(const void* dev_image, size_t bytes, con
     if (!dev_image || !out || !host_prefix || prefix_bytes < sizeof(Ht2ImageHeader)) return HT2GPU_ERR_ARG;
     ht2gpu_handle* h = newHandle(opt);
     *out = h;
-    int rc = selectDevice(h);
+    int rc = startOpen(h);
     if (rc) return rc;
     h->img = new Ht2Image();
     // host copy is needed for reference names / lengths (SAM) -- fetch it from the device
@@ -978,8 +987,9 @@ extern "C" int ht2gpu_open_peer(const ht2gpu_handle_t* src, const ht2gpu_options
 {
     if (!src || !out || !src->dBlob || !src->img) return HT2GPU_ERR_ARG;
     ht2gpu_handle* h = newHandle(opt ? opt : &src->opt);
+    h->opt.chr_names = src->opt.chr_names;   // one run prints one set of names
     *out = h;
-    int rc = selectDevice(h);
+    int rc = startOpen(h);
     if (rc) return rc;
     h->img = new Ht2Image();
     h->img->blob = src->img->blob;            // host copy: reference names / lengths for SAM
@@ -1001,7 +1011,7 @@ extern "C" int ht2gpu_open(const char* index_base, const ht2gpu_options_t* opt, 
     if (!index_base || !out) return HT2GPU_ERR_ARG;
     ht2gpu_handle* h = newHandle(opt);
     *out = h;
-    int rc = selectDevice(h);
+    int rc = startOpen(h);
     if (rc) return rc;
     h->img = ht2_image_load(index_base, h->err);
     if (!h->img) return HT2GPU_ERR_INDEX;
@@ -1047,6 +1057,7 @@ extern "C" int ht2gpu_close(ht2gpu_handle_t* h)
     if (h->dSplT) cudaFree(h->dSplT);
     if (h->dSsT) cudaFree(h->dSsT);
     if (h->dRgTag) cudaFree(h->dRgTag);
+    if (h->dRefNames) cudaFree(h->dRefNames);
     cudaFree(h->dStats);
     for (int k = 0; k < HT2GPU_N_SLOTS; k++) {
         SamSlot& S = h->slots[k];
@@ -1337,13 +1348,15 @@ extern "C" void ht2gpu_free_results(ht2gpu_result_batch_t* res)
 static Ht2SamIn samIn(const ht2gpu_handle* h, const SamSlot& S)
 {
     Ht2SamIn in;
-    in.blob = h->dBlob; in.minscTab = h->dMinsc;
+    in.blob = h->dBlob; in.refNames = h->dRefNames; in.minscTab = h->dMinsc;
     in.seq = S.dSeq; in.qual = S.batch.qual ? S.dQual : NULL; in.offs = S.dOffs; in.names = S.dNames; in.nameOffs = S.dNameOffs;
     in.n_reads = S.batch.n_reads; in.paired = S.batch.paired;
     in.reads = S.dReads; in.alns = S.dAlns; in.edits = S.dEdits; in.pairs = S.dPairs;
-    in.khits = h->P.khits; in.secondary = h->P.secondary; in.mixed = h->P.mixed; in.discord = h->P.discord; in.ssT = h->dSsT;
+    in.khits = h->P.khits; in.secondary = h->P.secondary; in.mixed = h->P.mixed; in.discord = h->P.discord;
+    in.ssT = h->samOut.noTlenAdj ? NULL : h->dSsT;
     in.colCount = h->collectSs ? S.dCounters + 6 : NULL; in.colRecs = S.dColRecs; in.colCap = (uint32_t)S.capCol;
     in.noUnal = h->samOut.noUnal; in.omitSecSeq = h->samOut.omitSecSeq; in.rgTag = h->dRgTag;
+    in.rnaStrandness = h->samOut.rnaStrandness; in.noQnameTrunc = h->samOut.noQnameTrunc;
     in.unitOut = h->recordOut ? S.dOut : NULL;
     return in;
 }
@@ -1422,9 +1435,11 @@ extern "C" int ht2gpu_submit_sam(ht2gpu_handle_t* h, int slot, const ht2gpu_read
     rc = ensureOut(h, S, S.units, (size_t)b->n_reads * 2 + 1024, (size_t)b->n_reads * 4 + 4096, (size_t)S.units * 2 + 1024);
     if (rc) return rc;
     // SAM text: ~2.2 bytes per base + ~170 per record at one record per read; grown from the measured size if short
-    // (+ "\tRG:Z:<id>" per record with a read group)
+    // (+ "\tRG:Z:<id>" per record with a read group, + "\tXS:A:<c>" under a known strandness; every name is counted
+    // whole)
     const size_t rgBytes = h->samOut.rgId.empty() ? 0 : h->samOut.rgTag().size() + 1;
-    const size_t est = (size_t)((double)b->offs[b->n_reads] * 2.6) + (size_t)b->n_reads * (260 + rgBytes) + names_bytes + 4096;
+    const size_t xsBytes = h->samOut.rnaStrandness ? 7 : 0;
+    const size_t est = (size_t)((double)b->offs[b->n_reads] * 2.6) + (size_t)b->n_reads * (260 + rgBytes + xsBytes) + names_bytes + 4096;
     if (est > S.capSam) CK(growBuf(S.dSam, S.capSam, est, 1, 1));
     return enqueueKernels(h, S, true);
 }
@@ -1819,7 +1834,7 @@ extern "C" int ht2gpu_sam_header(ht2gpu_handle_t* h, char** out, size_t* out_len
 {
     if (!h || !out) return HT2GPU_ERR_ARG;
     std::string s;
-    ht2_sam_header(s, *h->img, &h->samOut);
+    ht2_sam_header(s, *h->img, &h->samOut, &h->refNames);
     char* p = (char*)malloc(s.size() + 1);
     memcpy(p, s.data(), s.size()); p[s.size()] = 0;
     *out = p; if (out_len) *out_len = s.size();
@@ -1843,7 +1858,7 @@ extern "C" int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_pat
     if (files.empty()) return HT2GPU_OK;
     for (const Ht2SsFile& f : files) { FILE* t = fopen(f.path.c_str(), "rb"); if (!t) { h->err = "ht2gpu: cannot open " + f.path; return HT2GPU_ERR_INDEX; } fclose(t); }
     std::string err; uint32_t ns = 0;
-    if (!ht2_ssdb_build(*h->img, files, h->ssBlob, ns, err)) { h->err = err; h->ssBlob.clear(); return HT2GPU_ERR_INDEX; }
+    if (!ht2_ssdb_build(*h->img, files, h->ssBlob, ns, err, &h->refNames)) { h->err = err; h->ssBlob.clear(); return HT2GPU_ERR_INDEX; }
     CK(cudaSetDevice(h->device));
     CK(cudaMalloc(&h->dSsT, h->ssBlob.size()));
     CK(cudaMemcpy(h->dSsT, h->ssBlob.data(), h->ssBlob.size(), cudaMemcpyHostToDevice));
@@ -1875,7 +1890,7 @@ extern "C" int ht2gpu_write_novel_splicesites(ht2gpu_handle_t** hs, int n, const
     Ht2NovelSites all;
     for (int i = 0; i < n; i++) { if (!hs[i]) return HT2GPU_ERR_ARG; std::lock_guard<std::mutex> lk(hs[i]->novelMu); all.merge(hs[i]->novel); }
     std::string err;
-    if (!all.write(*hs[0]->img, path, n_written, err)) { hs[0]->err = err; return HT2GPU_ERR_INDEX; }
+    if (!all.write(*hs[0]->img, path, n_written, err, &hs[0]->refNames)) { hs[0]->err = err; return HT2GPU_ERR_INDEX; }
     return HT2GPU_OK;
 }
 
@@ -1886,7 +1901,7 @@ extern "C" int ht2gpu_format_sam(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* 
     unsigned nth = std::thread::hardware_concurrency();
     if (const char* e = getenv("HT2GPU_THREADS")) nth = (unsigned)atoi(e);
     return ht2_format_batch(*h->img, h->P, b, names, res, out, out_len, nth, h->ssBlob.empty() ? NULL : h->ssBlob.data(),
-                            NULL, NULL, 0, &h->samOut) ? HT2GPU_OK : HT2GPU_ERR_ARG;
+                            NULL, NULL, 0, &h->samOut, NULL, NULL, &h->refNames) ? HT2GPU_OK : HT2GPU_ERR_ARG;
 }
 
 // Read outcomes for --un / --al / --un-conc / --al-conc / --al-conc-disc (ht2gpu.h): the counting pass stores them
@@ -1913,15 +1928,18 @@ extern "C" int ht2gpu_unit_outcomes(ht2gpu_handle_t* h, int slot, const uint8_t*
     return HT2GPU_OK;
 }
 
-// SAM output settings (--no-unal, --omit-sec-seq, --no-sq, --rg-id / --rg).  The read group's "RG:Z:<id>" is uploaded
-// once here; the SAM kernels print it from device memory.
+// SAM output settings (--no-unal, --omit-sec-seq, --no-sq, --rg-id / --rg, --rna-strandness, --sam-no-qname-trunc,
+// --no-templatelen-adjustment).  The read group's "RG:Z:<id>" is uploaded once here; the SAM kernels print it from
+// device memory.
 extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output_t* cfg)
 {
     if (!h || !cfg || cfg->n_rg < 0 || (cfg->n_rg > 0 && !cfg->rg)) return HT2GPU_ERR_ARG;
+    if (cfg->rna_strandness < 0 || cfg->rna_strandness > 4) { h->err = "ht2gpu_set_sam_output: rna_strandness must be 0 (unknown) .. 4 (RF)"; return HT2GPU_ERR_ARG; }
     for (int k = 0; k < HT2GPU_N_SLOTS; k++)
         if (h->slots[k].pending) { h->err = "ht2gpu_set_sam_output: a batch is in flight (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
     Ht2SamOutput so;
     so.noUnal = cfg->no_unal != 0; so.omitSecSeq = cfg->omit_sec_seq != 0; so.noSq = cfg->no_sq != 0;
+    so.rnaStrandness = (uint32_t)cfg->rna_strandness; so.noQnameTrunc = cfg->no_qname_trunc != 0; so.noTlenAdj = cfg->no_templatelen_adjustment != 0;
     if (cfg->rg_id) so.rgId = cfg->rg_id;
     for (int i = 0; i < cfg->n_rg; i++) { if (!cfg->rg[i]) return HT2GPU_ERR_ARG; so.rg.push_back(cfg->rg[i]); }
     CK(cudaSetDevice(h->device));
@@ -1936,8 +1954,9 @@ extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output
     return HT2GPU_OK;
 }
 
-// The output settings of two handles are the same (ht2gpu_run_reads_multi: one run prints one kind of record)
-bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b) { return a->samOut == b->samOut; }
+// The output settings and reference names of two handles are the same (ht2gpu_run_reads_multi: one run prints one
+// kind of record)
+bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b) { return a->samOut == b->samOut && a->opt.chr_names == b->opt.chr_names; }
 int ht2_handle_device(const ht2gpu_handle_t* h) { return h->device; }
 
 extern "C" int ht2gpu_align_counts(ht2gpu_handle_t** hs, int n, int reset, ht2gpu_align_counts_t* out)

@@ -264,14 +264,15 @@ bool ht2_read_reads(const char* path, std::vector<Ht2HostRead>& out, int mate, s
 // SAM back end
 // ---------------------------------------------------------------------------
 // SamConfig::printHeader (sam.h:446-463) without @PG: @HD, @SQ unless --no-sq, @RG when a read-group id is set
-void ht2_sam_header(std::string& o, const Ht2Image& img, const Ht2SamOutput* so)
+void ht2_sam_header(std::string& o, const Ht2Image& img, const Ht2SamOutput* so, const Ht2RefNames* refNames)
 {
     o += "@HD\tVN:1.0\tSO:unsorted\n";
     const Ht2ImageHeader* H = img.header();
+    Ht2RefNames own;
+    if (!refNames) { own.build(img, HT2GPU_CHR_NAMES_INDEX); refNames = &own; }
     for (uint32_t i = 0; !(so && so->noSq) && i < H->nRefs; i++) {
         o += "@SQ\tSN:";
-        const char* nm = img.refName(i);
-        for (const char* c = nm; *c && !isspace((unsigned char)*c); c++) o.push_back(*c);
+        o += refNames->token(i);
         o += "\tLN:";
         appendInt(o, img.refPlen(i));
         o += "\n";
@@ -371,9 +372,11 @@ extern "C" int ht2gpu_format_align_summary(const ht2gpu_align_counts_t* c, int n
 // over the ranges, a writing pass straight into the output (records in read order = --reorder).
 bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read_batch_t* b, const char* names,
                       const ht2gpu_result_batch_t* res, char** out, size_t* out_len, unsigned nth, const uint8_t* ssT, uint32_t* colCount, Ht2SsRec* colRecs, uint32_t colCap,
-                      const Ht2SamOutput* so, ht2gpu_align_counts_t* counts, uint8_t* unitOut)
+                      const Ht2SamOutput* so, ht2gpu_align_counts_t* counts, uint8_t* unitOut, const Ht2RefNames* refNames)
 {
     const std::string rgTag = so ? so->rgTag() : std::string();
+    Ht2RefNames own;
+    if (!refNames) { own.build(img, HT2GPU_CHR_NAMES_INDEX); refNames = &own; }
     const uint32_t units = b->paired ? b->n_reads / 2 : b->n_reads;
     std::vector<uint32_t> nameOffs((size_t)b->n_reads + 1);
     {
@@ -382,12 +385,14 @@ bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read
         nameOffs[b->n_reads] = (uint32_t)at;
     }
     Ht2SamIn in;
-    in.blob = img.blob.data(); in.minscTab = P.minscTab;
+    in.blob = img.blob.data(); in.refNames = refNames->blob.data(); in.minscTab = P.minscTab;
     in.seq = b->seq; in.qual = b->qual; in.offs = b->offs; in.names = names; in.nameOffs = nameOffs.data();
     in.n_reads = b->n_reads; in.paired = b->paired;
     in.reads = res->reads; in.alns = res->alns; in.edits = res->edits; in.pairs = res->pairs;
-    in.khits = P.khits; in.secondary = P.secondary; in.mixed = P.mixed; in.discord = P.discord; in.ssT = ssT; in.colCount = colCount; in.colRecs = colRecs; in.colCap = colCap;
+    in.khits = P.khits; in.secondary = P.secondary; in.mixed = P.mixed; in.discord = P.discord;
+    in.ssT = so && so->noTlenAdj ? NULL : ssT; in.colCount = colCount; in.colRecs = colRecs; in.colCap = colCap;
     in.noUnal = so && so->noUnal; in.omitSecSeq = so && so->omitSecSeq; in.rgTag = rgTag.empty() ? NULL : rgTag.c_str();
+    in.rnaStrandness = so ? so->rnaStrandness : 0; in.noQnameTrunc = so && so->noQnameTrunc;
     in.unitOut = unitOut;
     Ht2SamFmt F; F.bind(&in);
     if (nth > 64) nth = 64;

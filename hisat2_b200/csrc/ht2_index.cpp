@@ -521,16 +521,38 @@ Ht2Image* ht2_image_load(const char* base_c, std::string& err)
 #include <algorithm>
 #include <set>
 #include <tuple>
-bool ht2_ssdb_build(const Ht2Image& img, const std::vector<Ht2SsFile>& files, std::vector<uint8_t>& blob, uint32_t& nSites, std::string& err)
+// the reference-name table of a handle (ht2_index.h): the splice-site DB matches and prints its names
+void Ht2RefNames::build(const Ht2Image& img, int chrNames)
 {
     const uint32_t nRefs = img.header()->nRefs;
-    std::vector<std::string> names(nRefs);
+    blob.assign((size_t)nRefs * 4, 0);
     for (uint32_t r = 0; r < nRefs; r++) {
-        const char* n = img.refName(r);
-        size_t i = 0;
-        while (n[i] && !isspace((unsigned char)n[i])) i++;
-        names[r].assign(n, i);
+        std::string n = img.refName(r);
+        const bool chr = n.compare(0, 3, "chr") == 0;
+        if (chrNames == HT2GPU_CHR_NAMES_REMOVE && chr) n = n.substr(3);
+        else if (chrNames == HT2GPU_CHR_NAMES_ADD && !chr) n = "chr" + n;
+        const uint32_t at = (uint32_t)blob.size();
+        memcpy(blob.data() + (size_t)r * 4, &at, 4);
+        blob.insert(blob.end(), n.c_str(), n.c_str() + n.size() + 1);
     }
+}
+
+std::string Ht2RefNames::token(uint32_t i) const
+{
+    const char* n = (*this)[i];
+    size_t k = 0;
+    while (n[k] && !isspace((unsigned char)n[k])) k++;
+    return std::string(n, k);
+}
+
+bool ht2_ssdb_build(const Ht2Image& img, const std::vector<Ht2SsFile>& files, std::vector<uint8_t>& blob, uint32_t& nSites, std::string& err,
+                    const Ht2RefNames* refNames)
+{
+    const uint32_t nRefs = img.header()->nRefs;
+    Ht2RefNames own;
+    if (!refNames) { own.build(img, HT2GPU_CHR_NAMES_INDEX); refNames = &own; }
+    std::vector<std::string> names(nRefs);
+    for (uint32_t r = 0; r < nRefs; r++) names[r] = refNames->token(r);
     std::vector<std::vector<Ht2SsSite>> per(nRefs);
     std::vector<std::set<std::tuple<uint32_t, uint32_t, uint32_t>>> seen(nRefs);
     for (const Ht2SsFile& f : files) {
@@ -590,8 +612,10 @@ void Ht2NovelSites::merge(const Ht2NovelSites& o)
         else { it->second.first += kv.second.first; if (kv.second.second < it->second.second) it->second.second = kv.second.second; }
     }
 }
-bool Ht2NovelSites::write(const Ht2Image& img, const char* path, uint64_t* nWritten, std::string& err) const
+bool Ht2NovelSites::write(const Ht2Image& img, const char* path, uint64_t* nWritten, std::string& err, const Ht2RefNames* names) const
 {
+    Ht2RefNames own;
+    if (!names) { own.build(img, HT2GPU_CHR_NAMES_INDEX); names = &own; }
     FILE* f = fopen(path, "wb");
     if (!f) { err = std::string("ht2: cannot write ") + path; return false; }
     // calculate_splicesite_read_dist (splice_site.cpp:528-563): smallest read count whose cumulative share of the sites exceeds 0.7
@@ -604,7 +628,6 @@ bool Ht2NovelSites::write(const Ht2Image& img, const char* path, uint64_t* nWrit
     struct S { uint32_t ref, left, right, dir, numreads; };
     std::vector<S> list;
     uint64_t nw = 0;
-    auto name = [&](uint32_t ref) { const char* n = img.refName(ref); size_t i = 0; while (n[i] && !isspace((unsigned char)n[i])) i++; return std::string(n, i); };
     auto impl = [&](const S* ss) {   // print_impl (splice_site.cpp:605-651)
         size_t i = 0;
         while (i < list.size()) {
@@ -620,7 +643,7 @@ bool Ht2NovelSites::write(const Ht2Image& img, const char* path, uint64_t* nWrit
             }
             if (!do_print) { i++; continue; }
             const char c = (tmp.dir == HT2_SPL_FW || tmp.dir == HT2_SPL_SEMI_FW) ? '+' : ((tmp.dir == HT2_SPL_RC || tmp.dir == HT2_SPL_SEMI_RC) ? '-' : '.');
-            fprintf(f, "%s\t%u\t%u\t%c\n", name(tmp.ref).c_str(), tmp.left, tmp.right, c);
+            fprintf(f, "%s\t%u\t%u\t%c\n", names->token(tmp.ref).c_str(), tmp.left, tmp.right, c);
             nw++;
             list.erase(list.begin() + i);
         }

@@ -25,7 +25,8 @@
 
 // Everything one batch's formatter reads; all pointers live in the memory space the caller runs in.
 struct Ht2SamIn {
-    const uint8_t*  blob;        // index image (reference names, ALT table + names)
+    const uint8_t*  blob;        // index image (ALT table + names)
+    const uint8_t*  refNames;    // the handle's reference names (Ht2RefNames::blob, ht2_index.h): RNAME, RNEXT
     const int32_t*  minscTab;    // --score-min per read length (Ht2Params::minscTab)
     const uint8_t*  seq;         // read batch (ht2gpu_read_batch_t)
     const uint8_t*  qual;        // NULL = all 'I'
@@ -39,7 +40,8 @@ struct Ht2SamIn {
     const ht2gpu_edit_t*        edits;
     const uint16_t*             pairs;
     uint32_t khits, secondary, mixed, discord;
-    const uint8_t*  ssT;         // the run's splice-site DB (ht2_ssdb.h) or NULL: template-length adjustment of concordant pairs
+    const uint8_t*  ssT;         // the run's splice-site DB (ht2_ssdb.h) or NULL: template-length adjustment of concordant
+                                 // pairs (NULL under --no-templatelen-adjustment)
     uint32_t*       colCount;    // --novel-splicesite-outfile: junctions of the printed alignments (write pass only), or NULL
     Ht2SsRec*       colRecs;
     uint32_t        colCap;
@@ -47,6 +49,8 @@ struct Ht2SamIn {
     uint32_t        noUnal;      // --no-unal: appendMate prints nothing for rs == NULL (aln_sink.h:3040)
     uint32_t        omitSecSeq;  // --omit-sec-seq: SEQ / QUAL '*' in non-primary records (aln_sink.h:3190-3215)
     const char*     rgTag;       // "RG:Z:<id>" or NULL (sam.h:780, 1102)
+    uint32_t        rnaStrandness;   // --rna-strandness: 0 unknown, 1 F, 2 R, 3 FR, 4 RF (read.h:30-36)
+    uint32_t        noQnameTrunc;    // --sam-no-qname-trunc: QNAME up to the '\0' (sam.h:238-256)
     uint8_t*        unitOut;     // ht2gpu_record_outcomes: the counting pass stores each unit's HT2GPU_OUTCOME_* bits here, or NULL
 };
 
@@ -101,18 +105,19 @@ __device__ __forceinline__ uint32_t ht2_sam_ld4(const char* p) {
 }
 #endif
 
-// Length of s up to its first '\0' or white space; atEnd = it stopped at the '\0'.  The device reads aligned words
-// (no word past the one holding the stop byte, so nothing outside the string's allocation granule).
-HT2_HD uint32_t ht2_sam_token(const char* s, bool& atEnd) {
+// Length of s up to its first '\0' or (stopAtSpace) white space; atEnd = it stopped at the '\0'.  The device reads
+// aligned words (no word past the one holding the stop byte, so nothing outside the string's allocation granule).
+HT2_HD uint32_t ht2_sam_token(const char* s, bool& atEnd, bool stopAtSpace) {
 #ifdef __CUDA_ARCH__
     const uintptr_t a = (uintptr_t)s;
     const uint32_t* w = (const uint32_t*)(a & ~(uintptr_t)3);
     const uint32_t head = (uint32_t)(a & 3);
     const uint32_t before = (1u << (8 * head)) - 1u;        // bytes ahead of s read as 'A'
+    const uint32_t spaces = stopAtSpace ? 0xffffffffu : 0u;
     uint32_t x = (w[0] & ~before) | (0x41414141u & before);
     for (uint32_t k = 0;; k += 4) {
         const uint32_t z = __vcmpeq4(x, 0u);
-        const uint32_t st = z | __vcmpeq4(x, 0x20202020u) | (__vcmpgeu4(x, 0x09090909u) & __vcmpleu4(x, 0x0d0d0d0du));
+        const uint32_t st = z | ((__vcmpeq4(x, 0x20202020u) | (__vcmpgeu4(x, 0x09090909u) & __vcmpleu4(x, 0x0d0d0d0du))) & spaces);
         if (st) {
             const uint32_t b = (uint32_t)(__ffs(st) - 1) >> 3;
             atEnd = (z >> (8 * b)) & 1u;
@@ -122,7 +127,7 @@ HT2_HD uint32_t ht2_sam_token(const char* s, bool& atEnd) {
     }
 #else
     uint32_t i = 0;
-    while (s[i] && !ht2_sam_isspace(s[i])) i++;
+    while (s[i] && !(stopAtSpace && ht2_sam_isspace(s[i]))) i++;
     atEnd = !s[i];
     return i;
 #endif
@@ -138,12 +143,13 @@ HT2_HD void ht2_sam_copy(char* d, const char* s, uint32_t len) {
     for (; i < len; i++) d[i] = s[i];
 }
 
-// A read or reference name up to its first white space, at most cap bytes; with omitSlashMate a trailing /1, /2
-// or /3 of the whole name is dropped.  White space cannot come after the '/'
-// of such a suffix, so the suffix only matters when the name ends at its terminator.
-template <bool WRITE> HT2_NI uint32_t ht2_sam_name(char* d, const char* name, bool omitSlashMate, uint32_t cap) {
+// A read or reference name up to its first white space, at most cap bytes (trunc; without it the whole name, as
+// --sam-no-qname-trunc prints QNAME); with omitSlashMate a trailing /1, /2 or /3 of the whole name is dropped.
+// White space cannot come after the '/' of such a suffix, so the suffix only matters when the name ends at its
+// terminator.
+template <bool WRITE> HT2_NI uint32_t ht2_sam_name(char* d, const char* name, bool omitSlashMate, uint32_t cap, bool trunc) {
     bool atEnd;
-    uint32_t len = ht2_sam_token(name, atEnd);
+    uint32_t len = ht2_sam_token(name, atEnd, trunc);
     if (atEnd && omitSlashMate && len >= 2 && name[len - 2] == '/' &&
         (name[len - 1] == '1' || name[len - 1] == '2' || name[len - 1] == '3')) len -= 2;
     if (len > cap) len = cap;
@@ -176,7 +182,7 @@ struct Ht2SamCur {
     }
     HT2_HD void str(const char* z) { n += ht2_sam_str<WRITE>(at(), z); }
     HT2_HD void i64(int64_t v) { n += ht2_sam_i64<WRITE>(at(), v); }
-    HT2_HD void name(const char* z, bool omitSlashMate, uint32_t cap) { n += ht2_sam_name<WRITE>(at(), z, omitSlashMate, cap); }
+    HT2_HD void name(const char* z, bool omitSlashMate, uint32_t cap, bool trunc) { n += ht2_sam_name<WRITE>(at(), z, omitSlashMate, cap, trunc); }
     // cnt bytes, byte i = byteAt(i); once the destination is 4-byte aligned, bytes i..i+3 = word4(i), one store (SEQ / QUAL)
     template <typename F, typename G> HT2_HD void run(uint32_t cnt, F byteAt, G word4) {
         if (WRITE) {
@@ -238,10 +244,7 @@ struct Ht2SamFmt {
     HT2_HD void bind(const Ht2SamIn* i) {
         in = i; IH = (const Ht2ImageHeader*)i->blob; nAlts = IH->nAlts; altTab = (const Ht2Alt*)(i->blob + IH->o_alts);
     }
-    HT2_HD const char* refName(uint32_t tidx) const {
-        const uint32_t* no = (const uint32_t*)(in->blob + IH->o_nameOffs);
-        return (const char*)in->blob + IH->o_names + no[tidx];
-    }
+    HT2_HD const char* refName(uint32_t tidx) const { return (const char*)in->refNames + ((const uint32_t*)in->refNames)[tidx]; }
     HT2_HD const char* altName(uint32_t si) const {
         const uint32_t* no = (const uint32_t*)(in->blob + IH->o_altNameOffs);
         return (const char*)in->blob + IH->o_altNames + no[si];
@@ -476,7 +479,7 @@ struct Ht2SamFmt {
         return fraglen;
     }
 
-    template <bool W> HT2_HD void putRefName(Ht2SamCur<W>& o, uint32_t tidx) const { o.name(refName(tidx), false, 0xffffffffu); }
+    template <bool W> HT2_HD void putRefName(Ht2SamCur<W>& o, uint32_t tidx) const { o.name(refName(tidx), false, 0xffffffffu, true); }
     template <bool W> HT2_HD void putSeqQual(Ht2SamCur<W>& o, const Ht2SamRead& rd, bool fw) const {
         const uint32_t n = rd.len;
         if (n == 0) { o.s("*\t*"); return; }   // aln_sink.h:3194, 3210
@@ -721,6 +724,19 @@ struct Ht2SamFmt {
         return o.n;
     }
 
+    // XS:A of every aligned record under a known --rna-strandness (sam.h:938-963): '-' where the alignment's strand
+    // is the opposite of the transcript's.  mate1 = AlnRes::readMate1 (aligner_result.h:1549): mate 1 of a pair or an
+    // unpaired read (ALN_RES_TYPE_UNPAIRED_MATE1, aln_sink.h:2368).  Every strandness goes with every read layout;
+    // mate 2 under F or R gets '+', as in the reference.
+    HT2_HD char xsStrand(bool mate1, bool fw) const {
+        enum { F = 1, R, FR, RF };
+        const uint32_t s = in->rnaStrandness;
+        bool minus;
+        if (mate1) minus = fw ? (s == R || s == RF) : (s == F || s == FR);
+        else minus = fw ? s == FR : s == RF;
+        return minus ? '-' : '+';
+    }
+
 #ifdef HT2_ENABLE_SPLICED
     // XS:A of a spliced alignment: AlnRes::spliced_whichsense_transcript (aligner_result.h:1288-1318, sam.h:925-937);
     // '+', '-' or 0 for none
@@ -793,7 +809,8 @@ struct Ht2SamFmt {
                                const Ht2SamSumm& summ, const Ht2SamFlags& fl, bool fraglenSet, int64_t fraglen, bool haveOscore) const {
         if (rs == NULL && in->noUnal) return 0;
         Ht2SamCur<W> o = {d, 0};
-        o.name(rd.name, fl.partOfPair(), 255);
+        const bool trunc = !in->noQnameTrunc;
+        o.name(rd.name, fl.partOfPair(), trunc ? 255 : 0xffffffffu, trunc);
         o.c('\t');
         int flag = 0;
         if (fl.partOfPair()) {
@@ -885,8 +902,9 @@ struct Ht2SamFmt {
         putYT(o, fl);
         putYF(o, rd);
         putRG(o);
+        if (in->rnaStrandness) { o.s("\tXS:A:"); o.c(xsStrand(rd.mate < 2, rs->fw != 0)); }
 #ifdef HT2_ENABLE_SPLICED
-        if (spliced) { const char xs = xsSense(ed, ned); if (xs) { o.s("\tXS:A:"); o.c(xs); } }
+        else if (spliced) { const char xs = xsSense(ed, ned); if (xs) { o.s("\tXS:A:"); o.c(xs); } }
 #else
         (void)spliced;
 #endif

@@ -73,7 +73,16 @@ typedef struct {
     int32_t  score_min_type;         /* --score-min <type>,<const>,<coeff>: 'C', 'L', 'S' (sqrt) or 'G' (log); default L,0,-0.2 */
     double   score_min_const;
     double   score_min_coeff;
+    /* The reference names the handle prints (@SQ, RNAME, RNEXT) and matches splice-site files against
+     * (ht2gpu_load_splicesites, ht2gpu_write_novel_splicesites), hisat2.cpp:3957-3976: HT2GPU_CHR_NAMES_INDEX (0) as in
+     * the index, _REMOVE (--remove-chrname) drops a leading "chr", _ADD (--add-chrname) puts "chr" before every name
+     * that does not start with it.  Both flags together, or any other value, is HT2GPU_ERR_ARG before a device is
+     * used (both: the reference's "--remove-chrname and --add-chrname cannot be used at the same time").
+     * ht2gpu_open_peer takes the source handle's setting.  ht2gpu_ref_name and the ht2_* compatibility calls keep the
+     * index's own names, as the reference's hisat2lib does: it has no such option. */
+    int32_t  chr_names;
 } ht2gpu_options_t;
+enum { HT2GPU_CHR_NAMES_INDEX = 0, HT2GPU_CHR_NAMES_REMOVE = 1, HT2GPU_CHR_NAMES_ADD = 2 };
 
 /* A batch of reads, structure-of-arrays, host memory.  Read i occupies
  * seq[offs[i] .. offs[i+1]).  Bases are codes 0..4 (A,C,G,T,N) exactly as
@@ -430,12 +439,22 @@ void ht2gpu_free_text(char* p);
  *   no_sq         --no-sq: ht2gpu_sam_header prints no @SQ lines
  *   rg_id         --rg-id: "@RG\tID:<rg_id>" (+ "\t<rg[i]>" for every --rg field) in the header, "RG:Z:<rg_id>" in
  *                 every record; NULL or "" = no read group (the rg fields are then not printed either)
+ *   rna_strandness  --rna-strandness: 0 unknown, 1 F, 2 R, 3 FR, 4 RF (read.h:30-36).  When known, every aligned
+ *                 record gets XS:A:+ or - from the library's strand, the mate and the alignment's orientation
+ *                 (sam.h:938-963); it replaces the splice-motif sense of spliced records.  Single-end reads and
+ *                 mate 1 take the mate-1 rule, mate 2 the mate-2 rule, whatever the read layout (F or R on pairs
+ *                 prints '+' for every mate 2, as the reference does)
+ *   no_qname_trunc  --sam-no-qname-trunc: QNAME is the whole name line, not cut at white space or at 255 characters
+ *                 (sam.h:238-256); a trailing /1 or /2 of a mate is still left out
+ *   no_templatelen_adjustment  --no-templatelen-adjustment: the TLEN of concordant pairs is not shortened by a known
+ *                 intron between the mates (aln_sink.h:2068-2076)
  * All off by default.  Set between batches, like ht2gpu_load_splicesites (refused while a batch is in flight). */
 typedef struct {
     int32_t no_unal, omit_sec_seq, no_sq;
     const char* rg_id;
     const char* const* rg;
     int32_t n_rg;
+    int32_t rna_strandness, no_qname_trunc, no_templatelen_adjustment;
 } ht2gpu_sam_output_t;
 int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output_t* cfg);
 
@@ -456,7 +475,7 @@ int ht2gpu_align_counts(ht2gpu_handle_t** hs, int n, int reset, ht2gpu_align_cou
 int ht2gpu_format_align_summary(const ht2gpu_align_counts_t* c, int new_style, int discordant, int mixed,
                                 char** out, size_t* out_len);
 
-/* Reference-sequence names and lengths (ht2_index_getrefnames, ht2.h:108). */
+/* Reference-sequence names and lengths (ht2_index_getrefnames, ht2.h:108): the index's own names, whatever chr_names. */
 uint32_t ht2gpu_num_refs(const ht2gpu_handle_t* h);
 const char* ht2gpu_ref_name(const ht2gpu_handle_t* h, uint32_t i);
 uint32_t ht2gpu_ref_len(const ht2gpu_handle_t* h, uint32_t i);
