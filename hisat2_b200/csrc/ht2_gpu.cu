@@ -12,6 +12,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <string>
@@ -640,6 +642,32 @@ ht2_sam_scan_kernel(unsigned long long* blk, uint32_t nBlk)
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
+// Device memory (cudaMalloc) or pinned host memory (cudaHostAlloc) with one owner: freed when the owner goes.
+// Capacities count elements; contents are not kept when a buffer is allocated again.  A failed allocation is
+// returned and cleared from cudaGetLastError(), so that the check after a later kernel launch does not find it.
+template <typename T, bool Pinned = false>
+struct CudaBuf {
+    T*     p = NULL;
+    size_t cap = 0;
+    CudaBuf() = default;
+    CudaBuf(const CudaBuf&) = delete; void operator=(const CudaBuf&) = delete;
+    ~CudaBuf() { release(); }
+    operator T*() const { return p; }
+    void release() { if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); } p = NULL; cap = 0; }
+    cudaError_t alloc(size_t n)   // exactly n elements
+    {
+        release();
+        const cudaError_t e = Pinned ? cudaHostAlloc((void**)&p, n * sizeof(T), cudaHostAllocPortable) : cudaMalloc((void**)&p, n * sizeof(T));
+        if (e != cudaSuccess) { p = NULL; cudaGetLastError(); } else cap = n;
+        return e;
+    }
+    // room for need elements; a new allocation holds need * num / den and 16 (device) or 4096 (pinned) more
+    cudaError_t reserve(size_t need, size_t num = Pinned ? 9 : 5, size_t den = Pinned ? 8 : 4) { return need <= cap && p ? cudaSuccess : alloc(need * num / den + (Pinned ? 4096 : 16)); }
+    cudaError_t upload(const void* src, size_t n) { const cudaError_t e = alloc(n); return e ? e : cudaMemcpy(p, src, n * sizeof(T), cudaMemcpyHostToDevice); }   // of n host elements
+};
+template <typename T> using DevBuf = CudaBuf<T, false>;
+template <typename T> using PinBuf = CudaBuf<T, true>;
+
 // One in-flight batch of the SAM path (ht2gpu_submit_sam / ht2gpu_wait_sam): its own stream, device input
 // buffers, device result pools, device SAM text and pinned host output, so that the H2D copy of batch i+1 and
 // the D2H copy of batch i-1 overlap the kernels of batch i.  The alignment workspaces (dWork) are shared by all
@@ -649,29 +677,40 @@ ht2_sam_scan_kernel(unsigned long long* blk, uint32_t nBlk)
 // device memory a handle leaves free beside its workspace pool: slot buffers of 4 M-read batches, the per-thread
 // stack of the pool kernel, and headroom for other work on the device
 #define HT2_MEM_RESERVE ((size_t)10 << 30)
+// The points a slot's events mark on its stream.  EV_ALIGN_START comes after the waits for the kernels before it.
+// The SAM path records every one; ht2gpu_align_batch has no upload mark (its H2D time runs to the kernel start) and no
+// SAM pass; ht2gpu_seed_search brackets each seed kernel with the align pair.
+enum SlotEvent { EV_START, EV_UPLOADED, EV_ALIGN_START, EV_ALIGN_END, EV_SAM_END, EV_COPIED, EV_N };
 struct SamSlot {
-    bool         init;
-    cudaStream_t stream;
-    cudaEvent_t  ev[6];            // start, h2d done, kernel start, align done, sam done, d2h done
-    cudaEvent_t  evSplit[3];       // HT2GPU_SAM_SPLIT=1: before the counting pass, after it, after the block scan
-    uint8_t *dSeq, *dQual; uint64_t* dOffs; uint32_t* dSeeds; char* dNames; uint32_t* dNameOffs;
-    size_t capSeq, capQual, capOffs, capSeeds, capNames, capNameOffs;
-    ht2gpu_read_result_t* dReads; ht2gpu_aln_t* dAlns; ht2gpu_edit_t* dEdits; uint16_t* dPairs; unsigned int* dCounters;
-    size_t capUnits, capAlns, capEdits, capPairs;
-    uint32_t* dSamLen; size_t capSamLen;          // bytes of SAM text per unit
-    unsigned long long* dBlk; size_t capBlk;      // per-block sums, then exclusive block offsets; [nBlk] = total
-    char* dSam; size_t capSam;
-    Ht2SsRec* dColRecs; size_t capCol;            // --novel-splicesite-outfile: junction records of the batch (count in dCounters[6])
-    unsigned long long* dTally;                   // ReportingMetrics of the batch (HT2_T_N counters, ht2_sam.h), zeroed per SAM pass
-    uint8_t* dOut; size_t capOut;                 // ht2gpu_record_outcomes: one HT2GPU_OUTCOME_* byte per unit (counting pass)
-    uint8_t* hOut; size_t capHOut;                // ... copied back with the meta (pinned)
-    bool outValid;                                // hOut holds the outcomes of the batch the last ht2gpu_wait_sam returned
-    char* hSam; size_t capHSam;                   // pinned
-    unsigned long long* hMeta;                    // pinned: [0] total SAM bytes, [1..4] result counters, [5] reads with errors,
-                                                  //         [HT2_META_TALLY ..] the batch's ReportingMetrics
+    bool         init = false;
+    cudaStream_t stream = NULL;
+    cudaEvent_t  ev[EV_N] = {};
+    cudaEvent_t  evSplit[3] = {};  // HT2GPU_SAM_SPLIT=1: before the counting pass, after it, after the block scan
+    DevBuf<uint8_t> dSeq, dQual; DevBuf<uint64_t> dOffs; DevBuf<uint32_t> dSeeds; DevBuf<char> dNames; DevBuf<uint32_t> dNameOffs;
+    DevBuf<ht2gpu_read_result_t> dReads; DevBuf<ht2gpu_aln_t> dAlns; DevBuf<ht2gpu_edit_t> dEdits;
+    DevBuf<uint32_t> dPairs;                      // one pair: the two uint16_t alignment indexes of ht2gpu_result_batch_t.pairs
+    DevBuf<unsigned int> dCounters;
+    DevBuf<uint32_t> dSamLen;                     // bytes of SAM text per unit
+    DevBuf<unsigned long long> dBlk;              // per-block sums, then exclusive block offsets; [nBlk] = total
+    DevBuf<char> dSam;
+    DevBuf<Ht2SsRec> dColRecs;                    // --novel-splicesite-outfile: junction records of the batch (count in dCounters[6])
+    DevBuf<unsigned long long> dTally;            // ReportingMetrics of the batch (HT2_T_N counters, ht2_sam.h), zeroed per SAM pass
+    DevBuf<uint8_t> dOut;                         // ht2gpu_record_outcomes: one HT2GPU_OUTCOME_* byte per unit (counting pass)
+    PinBuf<uint8_t> hOut;                         // ... copied back with the meta
+    bool outValid = false;                        // hOut holds the outcomes of the batch the last ht2gpu_wait_sam returned
+    PinBuf<char> hSam;
+    PinBuf<unsigned long long> hMeta;             // [0] total SAM bytes, [1..4] result counters, [5] reads with errors,
+                                                  // [HT2_META_TALLY ..] the batch's ReportingMetrics
     // the submitted batch (for a re-run after a pool overflow)
-    ht2gpu_read_batch_t batch; uint32_t units; size_t namesBytes; uint64_t h2dBytes; uint32_t nLaunch;
-    bool pending;
+    ht2gpu_read_batch_t batch = {}; uint32_t units = 0; size_t namesBytes = 0; uint64_t h2dBytes = 0; uint32_t nLaunch = 0;
+    bool pending = false;
+
+    ~SamSlot()   // the buffers are freed after the stream's work is done
+    {
+        if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : evSplit) if (e) cudaEventDestroy(e);
+    }
 };
 
 // Alignment workspaces are a property of the DEVICE, not of an index handle: every handle of the process that runs
@@ -682,54 +721,59 @@ struct SamSlot {
 struct WorkPool {
     int            device;
     size_t         nWork;
-    Ht2Work*       dWork;
-    cudaEvent_t    evDone;        // recorded after the latest kernels of a batch (alignment + SAM)
-    Ht2SwScratch*  dSw;           // --bowtie2-dp scratch per launched thread (allocated on first use)
-    uint32_t*      dSwPool;
-    size_t         swThreads;     // launched threads dSw / dSwPool hold: geometries of equal nWork differ in grid size
-    std::mutex     mu;            // [wait, launches, record] of one batch are one critical section
-    int            refs;
+    DevBuf<Ht2Work> dWork;
+    cudaEvent_t    evDone = NULL;  // recorded after the latest kernels of a batch (alignment + SAM)
+    DevBuf<Ht2SwScratch> dSw;      // --bowtie2-dp scratch per launched thread (allocated on first use)
+    DevBuf<uint32_t> dSwPool;
+    size_t         swThreads = 0;  // launched threads dSw / dSwPool hold: geometries of equal nWork differ in grid size
+    std::mutex     mu;             // [wait, launches, record] of one batch are one critical section
+    int            refs = 0;
+
+    // The whole pool (zeroed workspaces, evDone recorded), or e != cudaSuccess
+    WorkPool(int dev, size_t n, cudaError_t& e) : device(dev), nWork(n)
+    {
+        if ((e = dWork.alloc(nWork)) || (e = cudaMemset(dWork, 0, nWork * sizeof(Ht2Work))) ||
+            (e = cudaEventCreateWithFlags(&evDone, cudaEventDisableTiming)) || (e = cudaEventRecord(evDone, 0))) return;
+        e = cudaDeviceSynchronize();
+    }
+    ~WorkPool() { cudaSetDevice(device); cudaDeviceSynchronize(); if (evDone) cudaEventDestroy(evDone); }   // its kernels are done first
 };
 static std::mutex gPoolMu;
 static std::vector<WorkPool*> gPools;
 
 struct ht2gpu_handle {
-    WorkPool*      pool;
-    Ht2Image*      img;        // host copy (may hold only the header prefix when adopting a device image)
-    uint8_t*       dBlob;
-    bool           ownBlob;
-    size_t         blobBytes;
+    WorkPool*      pool = NULL;
+    std::unique_ptr<Ht2Image> img;   // host copy of the index image (all of it)
+    uint8_t*       dBlob = NULL;     // the image on the device: blobCopy, or the caller's (ht2gpu_open_device_image)
+    DevBuf<uint8_t> blobCopy;
     Ht2RefNames    refNames;   // the reference names of opt.chr_names (SAM, splice-site files) ...
-    uint8_t*       dRefNames;  // ... and their copy on the device, next to the index image
+    DevBuf<uint8_t> dRefNames; // ... and their copy on the device, next to the index image
     Ht2Params      P;
     ht2gpu_options_t opt;
-    int            device;
-    int            nSM;
-    int            tpb, bpsm;
-    uint32_t       samStage;  // bytes of the SAM writing pass's staging buffer (dynamic shared memory per block)
-    bool           graph;
-    int            poolWarps;
-    int            rgK;
-    int32_t*       dMinsc;   // --score-min table on the device (Ht2Params::minscTab)
-    void*          dSplT;    // spliced builds: Ht2SplTables on the device
-    uint8_t*       dSsT;     // the run's splice-site DB on the device (ht2gpu_load_splicesites) or NULL
-    bool           collectSs; // --novel-splicesite-outfile: collect the junctions of printed alignments
-    bool           recordOut; // ht2gpu_record_outcomes: the SAM counting pass stores each unit's outcome byte
+    int            device = 0;
+    int            nSM = 0;
+    int            tpb = 0, bpsm = 0;
+    uint32_t       samStage = 0;  // bytes of the SAM writing pass's staging buffer (dynamic shared memory per block)
+    bool           graph = false;
+    int            poolWarps = 0;
+    int            rgK = 0;
+    DevBuf<int32_t> dMinsc;  // --score-min table on the device (Ht2Params::minscTab)
+    DevBuf<uint8_t> dSplT;   // spliced mode: Ht2SplTables on the device
+    DevBuf<uint8_t> dSsT;    // the run's splice-site DB on the device (ht2gpu_load_splicesites) or NULL
+    bool           collectSs = false; // --novel-splicesite-outfile: collect the junctions of printed alignments
+    bool           recordOut = false; // ht2gpu_record_outcomes: the SAM counting pass stores each unit's outcome byte
     Ht2NovelSites  novel;     // ... aggregated here (ht2gpu_wait_sam), written by ht2gpu_write_novel_splicesites
     std::mutex     novelMu;
     std::vector<uint8_t> ssBlob;   // ... and its host copy (host formatter)
     Ht2SamOutput   samOut;    // SAM output settings (ht2gpu_set_sam_output)
-    char*          dRgTag;    // ... its "RG:Z:<id>" on the device, or NULL
-    ht2gpu_align_counts_t counts;   // ReportingMetrics of every batch ht2gpu_wait_sam returned (ht2gpu_align_counts)
+    DevBuf<char>   dRgTag;    // ... its "RG:Z:<id>" on the device, or NULL
+    ht2gpu_align_counts_t counts = {};   // ReportingMetrics of every batch ht2gpu_wait_sam returned (ht2gpu_align_counts)
     std::mutex     countMu;
-    size_t         nWork;
-    cudaStream_t   stream;
-    cudaEvent_t    ev[4];
     std::string    err;
-    unsigned long long* dStats;   // HT2GPU_STATS=1: per-state round statistics of the pool kernel
+    DevBuf<unsigned long long> dStats;   // HT2GPU_STATS=1: per-state round statistics of the pool kernel
     SamSlot        slots[HT2GPU_N_SLOTS];
-    void*          pipeCtx;       // ht2_pipeline.cpp's per-handle context
-    void         (*pipeCtxFree)(void*);
+    void*          pipeCtx = NULL;       // ht2_pipeline.cpp's per-handle context
+    void         (*pipeCtxFree)(void*) = NULL;
 };
 
 // Results live in ONE pinned host buffer per batch (D2H at PCIe speed instead of
@@ -800,124 +844,132 @@ static void applyOptions(Ht2Params& P, const Ht2Image& img, const ht2gpu_options
     if (o.score_min_type != 0) ht2_set_score_min(P, (char)o.score_min_type, o.score_min_const, o.score_min_coeff);
 }
 
-static int finishOpen(ht2gpu_handle* h)
+// ---- ht2gpu_open*: the steps after the host image and the device blob have arrived -------------------------------
+static int checkImage(ht2gpu_handle* h)
 {
     const Ht2ImageHeader* H = h->img->header();
     if (H->magic != HT2_MAGIC || H->version != HT2_IMAGE_VERSION) { h->err = "bad index image"; return HT2GPU_ERR_INDEX; }
-    if (H->totalBytes != h->blobBytes) { h->err = "index image is truncated (header.totalBytes differs from the bytes given)"; return HT2GPU_ERR_INDEX; }
+    if (H->totalBytes != h->img->blob.size()) { h->err = "index image is truncated (header.totalBytes differs from the bytes given)"; return HT2GPU_ERR_INDEX; }
 #ifndef HT2_ENABLE_SPLICED
     if (!h->opt.no_spliced_alignment) { h->err = "spliced alignment is not implemented in this build; pass --no-spliced-alignment"; return HT2GPU_ERR_UNSUPPORTED; }
-#else
+#endif
+    return HT2GPU_OK;
+}
+
+static int loadNamesAndParams(ht2gpu_handle* h)
+{
+#ifdef HT2_ENABLE_SPLICED
     // spliced mode (the default build; HT2_NO_SPLICED=1 leaves it out) == the reference's --no-temp-splicesite: the
     // splice-site DB holds only the sites loaded with ht2gpu_load_splicesites, never junctions of earlier reads
-    if (!h->opt.no_spliced_alignment) {
-        const Ht2SplTables& T = ht2_spl_tables();
-        CK(cudaMalloc(&h->dSplT, sizeof(Ht2SplTables)));
-        CK(cudaMemcpy(h->dSplT, &T, sizeof(Ht2SplTables), cudaMemcpyHostToDevice));
-    }
+    if (!h->opt.no_spliced_alignment) CK(h->dSplT.upload(&ht2_spl_tables(), sizeof(Ht2SplTables)));
 #endif
-    h->graph = !H->global.linearFM;   // graph (SNP) indexes: ALT-aware aligner instantiation, graph seed kernel
+    h->graph = !h->img->header()->global.linearFM;   // graph (SNP) indexes: ALT-aware aligner instantiation, graph seed kernel
     h->refNames.build(*h->img, h->opt.chr_names);
-    CK(cudaMalloc(&h->dRefNames, h->refNames.blob.size()));
-    CK(cudaMemcpy(h->dRefNames, h->refNames.blob.data(), h->refNames.blob.size(), cudaMemcpyHostToDevice));
+    CK(h->dRefNames.upload(h->refNames.blob.data(), h->refNames.blob.size()));
     applyOptions(h->P, *h->img, h->opt);
+    CK(h->dMinsc.upload(h->P.minscTab, sizeof(h->P.minscTab) / sizeof(h->P.minscTab[0])));
+    return HT2GPU_OK;
+}
+
+// The pool kernel: one block of poolWarps warps per SM, rgK read slots per lane (DESIGN.md 4)
+static int chooseGeometry(ht2gpu_handle* h)
+{
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, h->device));
     h->nSM = prop.multiProcessorCount;
-    // the pool kernel: one block of poolWarps warps per SM, rgK read slots per lane (DESIGN.md 4)
     h->poolWarps = (h->opt.threads_per_block == 128 && !h->graph) ? 4 : 8;
     h->tpb = 32 * h->poolWarps;
     h->bpsm = (h->opt.blocks_per_sm > 0 && !h->graph) ? h->opt.blocks_per_sm : 1;
     h->rgK = (h->opt.slots_per_lane > 0 && !h->graph) ? h->opt.slots_per_lane : 4;
     if (h->rgK != 2 && h->rgK != 4 && !(h->poolWarps == 4 && h->rgK == 8)) h->rgK = 4;
     if (h->poolWarps == 16) { h->poolWarps = 8; h->tpb = 256; }   // the 16-warp variant was slower and is no longer built
-    h->nWork = (size_t)h->nSM * h->bpsm * h->poolWarps * 32 * h->rgK;
-    CK(cudaMalloc(&h->dMinsc, sizeof(h->P.minscTab)));
-    CK(cudaMemcpy(h->dMinsc, h->P.minscTab, sizeof(h->P.minscTab), cudaMemcpyHostToDevice));
-    {   // the device's workspace pool for this launch geometry
-        std::lock_guard<std::mutex> lk(gPoolMu);
-        auto findPool = [&](size_t n) { WorkPool* r = NULL; for (WorkPool* q : gPools) if (q->device == h->device && q->nWork == n) r = q; return r; };
-        const size_t nThreads = (size_t)h->nSM * h->bpsm * (size_t)h->tpb;
-        const size_t dpBytes = nThreads * (sizeof(Ht2SwScratch) + (size_t)HT2_SW_POOL_WORDS * sizeof(uint32_t));
-        WorkPool* wp = findPool(h->nWork);
-        if (!wp && h->opt.slots_per_lane <= 0 && !h->graph && h->poolWarps == 8 && h->rgK == 4) {
-            // The default geometry's workspace (370 kB per slot, ~50 GB on an H100) must leave room for what else the
-            // process and the device need: the DP scratch of this handle, slot buffers, stack, other processes.  Where
-            // it does not, or where the process already has the half-size pool, linear indexes run with 2 slots per
-            // lane: half the memory, about 12 % less kernel throughput (DESIGN.md 3).  Graph indexes have one geometry.
-            size_t freeB = 0, totalB = 0;
-            CK(cudaMemGetInfo(&freeB, &totalB));
-            WorkPool* half = findPool(h->nWork / 2);
-            const size_t need = h->nWork * sizeof(Ht2Work) + (h->P.bowtie2Dp ? dpBytes : 0) + HT2_MEM_RESERVE;
-            if (half || need > freeB) { h->rgK = 2; h->nWork /= 2; wp = half; }
-        }
-        if (!wp) {
-            wp = new WorkPool();
-            wp->device = h->device; wp->nWork = h->nWork; wp->refs = 0;
-            wp->dWork = NULL; wp->dSw = NULL; wp->dSwPool = NULL; wp->swThreads = 0;
-            CK(cudaMalloc(&wp->dWork, wp->nWork * sizeof(Ht2Work)));
-            CK(cudaMemset(wp->dWork, 0, wp->nWork * sizeof(Ht2Work)));
-            CK(cudaEventCreateWithFlags(&wp->evDone, cudaEventDisableTiming));
-            CK(cudaEventRecord(wp->evDone, 0));
-            CK(cudaDeviceSynchronize());
-            gPools.push_back(wp);
-        }
-        if (h->P.bowtie2Dp && wp->swThreads < nThreads) {
-            // dynamic-programming scratch (ht2_sw.h): per executing thread, not per read slot.  Geometries with the same
-            // nWork share the pool but not the grid (8x4 and blocks_per_sm=2 x 2 slots: twice the threads), so the
-            // scratch grows to the largest grid once the pool's kernels are done.
-            std::lock_guard<std::mutex> lw(wp->mu);
-            CK(cudaEventSynchronize(wp->evDone));
-            cudaFree(wp->dSw); cudaFree(wp->dSwPool);
-            wp->dSw = NULL; wp->dSwPool = NULL; wp->swThreads = 0;
-            CK(cudaMalloc(&wp->dSw, nThreads * sizeof(Ht2SwScratch)));
-            CK(cudaMalloc(&wp->dSwPool, nThreads * (size_t)HT2_SW_POOL_WORDS * sizeof(uint32_t)));
-            wp->swThreads = nThreads;
-        }
-        wp->refs++;
-        h->pool = wp;
-    }
-    {   // per-thread stack: what the kernels of this index type need, not a blanket value (the limit is
-        // context-wide and the driver backs it for every resident thread).  Linear indexes have a statically
-        // known call tree; graph indexes recurse through alignWithALTs (ht2_alt.h, depth <= HT2_ALT_MAXDEP).
-        size_t need = 0;
-        cudaFuncAttributes fa;
-        if (h->graph) { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, true, false, true>)); need = fa.localSizeBytes + 36 * 1024; }
-        else { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, false, false, true>)); need = fa.localSizeBytes + 4 * 1024; }
-        CK(cudaFuncGetAttributes(&fa, ht2_sam_kernel<true>));
-        if (fa.localSizeBytes + 2048 > need) need = fa.localSizeBytes + 2048;
-        // the writing pass's staging buffer: what leaves room for HT2_SAM_STAGE_BLOCKS blocks per SM (1 KB of every
-        // block's shared memory is reserved by the system)
-        int smemSM = 0, smemBlk = 0;
-        CK(cudaDeviceGetAttribute(&smemSM, cudaDevAttrMaxSharedMemoryPerMultiprocessor, h->device));
-        CK(cudaDeviceGetAttribute(&smemBlk, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-        size_t stage = (size_t)smemSM / HT2_SAM_STAGE_BLOCKS - 1024 - fa.sharedSizeBytes;
-        if (stage > (size_t)smemBlk - fa.sharedSizeBytes) stage = (size_t)smemBlk - fa.sharedSizeBytes;
-        h->samStage = (uint32_t)(stage & ~(size_t)15);
-        CK(cudaFuncSetAttribute(ht2_sam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->samStage));
-        size_t cur = 0;
-        CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
-        if (cur < need) CK(cudaDeviceSetLimit(cudaLimitStackSize, need));
-    }
-    CK(cudaStreamCreate(&h->stream));
-    for (int i = 0; i < 4; i++) CK(cudaEventCreate(&h->ev[i]));
     return HT2GPU_OK;
 }
 
-static ht2gpu_handle* newHandle(const ht2gpu_options_t* opt)
+static WorkPool* findPool(int device, size_t nWork)   // the caller holds gPoolMu
 {
-    ht2gpu_handle* h = new ht2gpu_handle();
-    h->img = NULL; h->dBlob = NULL; h->ownBlob = false; h->blobBytes = 0; h->pool = NULL; h->nWork = 0; h->dMinsc = NULL; h->dSplT = NULL; h->dSsT = NULL; h->collectSs = false; h->recordOut = false;
-    h->stream = 0;
-    h->dStats = NULL;
-    memset((void*)h->slots, 0, sizeof(h->slots));
-    h->pipeCtx = NULL; h->pipeCtxFree = NULL;
-    if (opt) h->opt = *opt; else ht2gpu_default_options(&h->opt);
-    h->device = h->opt.device;
-    return h;
+    for (WorkPool* q : gPools) if (q->device == device && q->nWork == nWork) return q;
+    return NULL;
 }
 
-// Every ht2gpu_open*: refuse the options that need no device to refuse, then select the handle's device
+// The device's workspace pool for the handle's launch geometry: found or created, and counted.  releasePool drops
+// the count and frees the pool with its last handle.
+static int acquirePool(ht2gpu_handle* h)
+{
+    std::lock_guard<std::mutex> lk(gPoolMu);
+    size_t nWork = (size_t)h->nSM * h->bpsm * h->poolWarps * 32 * h->rgK;
+    const size_t nThreads = (size_t)h->nSM * h->bpsm * (size_t)h->tpb;
+    const size_t dpBytes = nThreads * (sizeof(Ht2SwScratch) + (size_t)HT2_SW_POOL_WORDS * sizeof(uint32_t));
+    WorkPool* wp = findPool(h->device, nWork);
+    if (!wp && h->opt.slots_per_lane <= 0 && !h->graph && h->poolWarps == 8 && h->rgK == 4) {
+        // The default geometry's workspace (370 kB per slot, ~50 GB on an H100) must leave room for what else the
+        // process and the device need: the DP scratch of this handle, slot buffers, stack, other processes.  Where
+        // it does not, or where the process already has the half-size pool, linear indexes run with 2 slots per
+        // lane: half the memory, about 12 % less kernel throughput (DESIGN.md 3).  Graph indexes have one geometry.
+        size_t freeB = 0, totalB = 0;
+        CK(cudaMemGetInfo(&freeB, &totalB));
+        WorkPool* half = findPool(h->device, nWork / 2);
+        const size_t need = nWork * sizeof(Ht2Work) + (h->P.bowtie2Dp ? dpBytes : 0) + HT2_MEM_RESERVE;
+        if (half || need > freeB) { h->rgK = 2; nWork /= 2; wp = half; }
+    }
+    if (!wp) {
+        cudaError_t e;
+        wp = new WorkPool(h->device, nWork, e);
+        if (e != cudaSuccess) { delete wp; h->err = std::string("the workspace pool: ") + cudaGetErrorString(e); return HT2GPU_ERR_CUDA; }
+        gPools.push_back(wp);
+    }
+    wp->refs++;
+    h->pool = wp;
+    if (h->P.bowtie2Dp && wp->swThreads < nThreads) {
+        // dynamic-programming scratch (ht2_sw.h): per executing thread, not per read slot.  Geometries with the same
+        // nWork share the pool but not the grid (8x4 and blocks_per_sm=2 x 2 slots: twice the threads), so the
+        // scratch grows to the largest grid once the pool's kernels are done.
+        std::lock_guard<std::mutex> lw(wp->mu);
+        CK(cudaEventSynchronize(wp->evDone));
+        wp->dSw.release(); wp->dSwPool.release(); wp->swThreads = 0;
+        CK(wp->dSw.alloc(nThreads));
+        CK(wp->dSwPool.alloc(nThreads * (size_t)HT2_SW_POOL_WORDS));
+        wp->swThreads = nThreads;
+    }
+    return HT2GPU_OK;
+}
+
+static void releasePool(WorkPool* wp)
+{
+    if (!wp) return;
+    std::lock_guard<std::mutex> lk(gPoolMu);
+    if (--wp->refs > 0) return;
+    gPools.erase(std::find(gPools.begin(), gPools.end(), wp));
+    delete wp;
+}
+
+// Per-thread stack: what the kernels of this index type need, not a blanket value (the limit is context-wide and the
+// driver backs it for every resident thread).  Linear indexes have a statically known call tree; graph indexes
+// recurse through alignWithALTs (ht2_alt.h, depth <= HT2_ALT_MAXDEP).  And the SAM writing pass's staging buffer.
+static int setKernelLimits(ht2gpu_handle* h)
+{
+    size_t need = 0;
+    cudaFuncAttributes fa;
+    if (h->graph) { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, true, false, true>)); need = fa.localSizeBytes + 36 * 1024; }
+    else { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, false, false, true>)); need = fa.localSizeBytes + 4 * 1024; }
+    CK(cudaFuncGetAttributes(&fa, ht2_sam_kernel<true>));
+    if (fa.localSizeBytes + 2048 > need) need = fa.localSizeBytes + 2048;
+    // the writing pass's staging buffer: what leaves room for HT2_SAM_STAGE_BLOCKS blocks per SM (1 KB of every
+    // block's shared memory is reserved by the system)
+    int smemSM = 0, smemBlk = 0;
+    CK(cudaDeviceGetAttribute(&smemSM, cudaDevAttrMaxSharedMemoryPerMultiprocessor, h->device));
+    CK(cudaDeviceGetAttribute(&smemBlk, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    size_t stage = (size_t)smemSM / HT2_SAM_STAGE_BLOCKS - 1024 - fa.sharedSizeBytes;
+    if (stage > (size_t)smemBlk - fa.sharedSizeBytes) stage = (size_t)smemBlk - fa.sharedSizeBytes;
+    h->samStage = (uint32_t)(stage & ~(size_t)15);
+    CK(cudaFuncSetAttribute(ht2_sam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->samStage));
+    size_t cur = 0;
+    CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
+    if (cur < need) CK(cudaDeviceSetLimit(cudaLimitStackSize, need));
+    return HT2GPU_OK;
+}
+
+// Refuse the options that need no device to refuse, then select the handle's device
 static int startOpen(ht2gpu_handle* h)
 {
     const int32_t cn = h->opt.chr_names;
@@ -931,6 +983,26 @@ static int startOpen(ht2gpu_handle* h)
     }
     CK(cudaSetDevice(h->device));
     return HT2GPU_OK;
+}
+
+// Every ht2gpu_open*.  load(h) brings the host image (h->img) and the device blob (h->dBlob).  *out
+// holds the handle from the start: after a failure, ht2gpu_last_error explains it and ht2gpu_close frees the handle.
+template <typename Load>
+static int openHandle(const ht2gpu_options_t* opt, ht2gpu_handle_t** out, Load load)
+{
+    ht2gpu_handle* h = new ht2gpu_handle();
+    if (opt) h->opt = *opt; else ht2gpu_default_options(&h->opt);
+    h->device = h->opt.device;
+    *out = h;
+    int rc = startOpen(h);
+    if (!rc) rc = load(h);
+    if (!rc && !h->dBlob) h->dBlob = h->blobCopy;   // the handle's own copy, unless it borrows the caller's
+    if (!rc) rc = checkImage(h);
+    if (!rc) rc = loadNamesAndParams(h);
+    if (!rc) rc = chooseGeometry(h);
+    if (!rc) rc = acquirePool(h);
+    if (!rc) rc = setKernelLimits(h);
+    return rc;
 }
 
 extern "C" int ht2gpu_build_image(const char* index_base, void** image, size_t* bytes, char* errbuf, size_t errbuf_len)
@@ -952,78 +1024,62 @@ extern "C" void ht2gpu_free_image(void* image) { free(image); }
 extern "C" int ht2gpu_open_image(const void* image, size_t bytes, const ht2gpu_options_t* opt, ht2gpu_handle_t** out)
 {
     if (!image || !out || bytes < sizeof(Ht2ImageHeader)) return HT2GPU_ERR_ARG;
-    ht2gpu_handle* h = newHandle(opt);
-    *out = h;
-    int rc = startOpen(h);
-    if (rc) return rc;
-    h->img = new Ht2Image();
-    h->img->blob.assign((const uint8_t*)image, (const uint8_t*)image + bytes);
-    h->blobBytes = bytes;
-    CK(cudaMalloc(&h->dBlob, bytes));
-    h->ownBlob = true;
-    CK(cudaMemcpy(h->dBlob, image, bytes, cudaMemcpyHostToDevice));
-    return finishOpen(h);
+    return openHandle(opt, out, [&](ht2gpu_handle* h) -> int {
+        h->img.reset(new Ht2Image());
+        h->img->blob.assign((const uint8_t*)image, (const uint8_t*)image + bytes);
+        CK(h->blobCopy.upload(image, bytes));
+        return HT2GPU_OK;
+    });
 }
 
 extern "C" int ht2gpu_open_device_image(const void* dev_image, size_t bytes, const void* host_prefix, size_t prefix_bytes,
                                         const ht2gpu_options_t* opt, ht2gpu_handle_t** out)
 {
     if (!dev_image || !out || !host_prefix || prefix_bytes < sizeof(Ht2ImageHeader)) return HT2GPU_ERR_ARG;
-    ht2gpu_handle* h = newHandle(opt);
-    *out = h;
-    int rc = startOpen(h);
-    if (rc) return rc;
-    h->img = new Ht2Image();
-    // host copy is needed for reference names / lengths (SAM) -- fetch it from the device
-    h->img->blob.resize(bytes);
-    CK(cudaMemcpy(h->img->blob.data(), dev_image, bytes, cudaMemcpyDeviceToHost));
-    h->blobBytes = bytes;
-    h->dBlob = (uint8_t*)dev_image;
-    h->ownBlob = false;
-    return finishOpen(h);
+    return openHandle(opt, out, [&](ht2gpu_handle* h) -> int {
+        // host copy is needed for reference names / lengths (SAM) -- fetch it from the device; the blob stays the caller's
+        h->img.reset(new Ht2Image());
+        h->img->blob.resize(bytes);
+        CK(cudaMemcpy(h->img->blob.data(), dev_image, bytes, cudaMemcpyDeviceToHost));
+        h->dBlob = (uint8_t*)dev_image;
+        return HT2GPU_OK;
+    });
 }
 
 extern "C" int ht2gpu_open_peer(const ht2gpu_handle_t* src, const ht2gpu_options_t* opt, ht2gpu_handle_t** out)
 {
     if (!src || !out || !src->dBlob || !src->img) return HT2GPU_ERR_ARG;
-    ht2gpu_handle* h = newHandle(opt ? opt : &src->opt);
-    h->opt.chr_names = src->opt.chr_names;   // one run prints one set of names
-    *out = h;
-    int rc = startOpen(h);
-    if (rc) return rc;
-    h->img = new Ht2Image();
-    h->img->blob = src->img->blob;            // host copy: reference names / lengths for SAM
-    h->blobBytes = src->blobBytes;
-    CK(cudaMalloc(&h->dBlob, h->blobBytes));
-    h->ownBlob = true;
-    if (h->device == src->device) CK(cudaMemcpy(h->dBlob, src->dBlob, h->blobBytes, cudaMemcpyDeviceToDevice));
-    else {
-        int can = 0;
-        cudaDeviceCanAccessPeer(&can, h->device, src->device);
-        if (can) { cudaError_t e = cudaDeviceEnablePeerAccess(src->device, 0); if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e); cudaGetLastError(); }
-        CK(cudaMemcpyPeer(h->dBlob, h->device, src->dBlob, src->device, h->blobBytes));
-    }
-    return finishOpen(h);
+    ht2gpu_options_t o = opt ? *opt : src->opt;
+    o.chr_names = src->opt.chr_names;   // one run prints one set of names
+    return openHandle(&o, out, [&](ht2gpu_handle* h) -> int {
+        h->img.reset(new Ht2Image());
+        h->img->blob = src->img->blob;            // host copy: reference names / lengths for SAM
+        const size_t bytes = h->img->blob.size();
+        CK(h->blobCopy.alloc(bytes));
+        if (h->device == src->device) CK(cudaMemcpy(h->blobCopy, src->dBlob, bytes, cudaMemcpyDeviceToDevice));
+        else {
+            int can = 0;
+            cudaDeviceCanAccessPeer(&can, h->device, src->device);
+            if (can) { cudaError_t e = cudaDeviceEnablePeerAccess(src->device, 0); if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e); cudaGetLastError(); }
+            CK(cudaMemcpyPeer(h->blobCopy, h->device, src->dBlob, src->device, bytes));
+        }
+        return HT2GPU_OK;
+    });
 }
 
 extern "C" int ht2gpu_open(const char* index_base, const ht2gpu_options_t* opt, ht2gpu_handle_t** out)
 {
     if (!index_base || !out) return HT2GPU_ERR_ARG;
-    ht2gpu_handle* h = newHandle(opt);
-    *out = h;
-    int rc = startOpen(h);
-    if (rc) return rc;
-    h->img = ht2_image_load(index_base, h->err);
-    if (!h->img) return HT2GPU_ERR_INDEX;
-    h->blobBytes = h->img->blob.size();
-    CK(cudaMalloc(&h->dBlob, h->blobBytes));
-    h->ownBlob = true;
-    CK(cudaMemcpy(h->dBlob, h->img->blob.data(), h->blobBytes, cudaMemcpyHostToDevice));
-    return finishOpen(h);
+    return openHandle(opt, out, [&](ht2gpu_handle* h) -> int {
+        h->img.reset(ht2_image_load(index_base, h->err));
+        if (!h->img) return HT2GPU_ERR_INDEX;
+        CK(h->blobCopy.upload(h->img->blob.data(), h->img->blob.size()));
+        return HT2GPU_OK;
+    });
 }
 
 extern "C" const void* ht2gpu_image_data(const ht2gpu_handle_t* h) { return h && h->img ? h->img->blob.data() : NULL; }
-extern "C" size_t ht2gpu_image_bytes(const ht2gpu_handle_t* h) { return h ? h->blobBytes : 0; }
+extern "C" size_t ht2gpu_image_bytes(const ht2gpu_handle_t* h) { return h && h->img ? h->img->blob.size() : 0; }
 extern "C" const void* ht2gpu_device_image(const ht2gpu_handle_t* h) { return h ? h->dBlob : NULL; }
 extern "C" const char* ht2gpu_last_error(const ht2gpu_handle_t* h) { return h ? h->err.c_str() : "null handle"; }
 extern "C" int ht2gpu_launch_geometry(const ht2gpu_handle_t* h, int32_t out[3])
@@ -1036,45 +1092,12 @@ extern "C" uint32_t ht2gpu_num_refs(const ht2gpu_handle_t* h) { return h && h->i
 extern "C" const char* ht2gpu_ref_name(const ht2gpu_handle_t* h, uint32_t i) { return h->img->refName(i); }
 extern "C" uint32_t ht2gpu_ref_len(const ht2gpu_handle_t* h, uint32_t i) { return h->img->refPlen(i); }
 
+// The handle's buffers, slots (each synchronized first) and image go with it
 extern "C" int ht2gpu_close(ht2gpu_handle_t* h)
 {
     if (!h) return HT2GPU_OK;
     if (h->pipeCtx && h->pipeCtxFree) h->pipeCtxFree(h->pipeCtx);
-    if (h->dBlob && h->ownBlob) cudaFree(h->dBlob);
-    if (h->pool) {   // the last handle of a pool frees the workspaces
-        std::lock_guard<std::mutex> lk(gPoolMu);
-        WorkPool* wp = h->pool;
-        if (--wp->refs == 0) {
-            cudaSetDevice(wp->device);
-            cudaDeviceSynchronize();
-            cudaFree(wp->dWork); cudaFree(wp->dSw); cudaFree(wp->dSwPool); cudaEventDestroy(wp->evDone);
-            for (size_t i = 0; i < gPools.size(); i++) if (gPools[i] == wp) { gPools.erase(gPools.begin() + i); break; }
-            delete wp;
-        }
-        h->pool = NULL;
-    }
-    if (h->dMinsc) cudaFree(h->dMinsc);
-    if (h->dSplT) cudaFree(h->dSplT);
-    if (h->dSsT) cudaFree(h->dSsT);
-    if (h->dRgTag) cudaFree(h->dRgTag);
-    if (h->dRefNames) cudaFree(h->dRefNames);
-    cudaFree(h->dStats);
-    for (int k = 0; k < HT2GPU_N_SLOTS; k++) {
-        SamSlot& S = h->slots[k];
-        if (!S.init) continue;
-        cudaStreamSynchronize(S.stream);
-        cudaFree(S.dSeq); cudaFree(S.dQual); cudaFree(S.dOffs); cudaFree(S.dSeeds); cudaFree(S.dNames); cudaFree(S.dNameOffs);
-        cudaFree(S.dReads); cudaFree(S.dAlns); cudaFree(S.dEdits); cudaFree(S.dPairs); cudaFree(S.dCounters);
-        cudaFree(S.dSamLen); cudaFree(S.dBlk); cudaFree(S.dSam); cudaFree(S.dColRecs); cudaFree(S.dTally); cudaFree(S.dOut);
-        if (S.hSam) cudaFreeHost(S.hSam);
-        if (S.hOut) cudaFreeHost(S.hOut);
-        if (S.hMeta) cudaFreeHost(S.hMeta);
-        cudaStreamDestroy(S.stream);
-        for (int i = 0; i < 6; i++) cudaEventDestroy(S.ev[i]);
-        for (int i = 0; i < 3; i++) if (S.evSplit[i]) cudaEventDestroy(S.evSplit[i]);
-    }
-    if (h->stream) { cudaStreamDestroy(h->stream); for (int i = 0; i < 4; i++) cudaEventDestroy(h->ev[i]); }
-    delete h->img;
+    releasePool(h->pool);
     delete h;
     return HT2GPU_OK;
 }
@@ -1088,27 +1111,15 @@ extern "C" uint32_t ht2gpu_read_seed(const uint8_t* seq, const uint8_t* qual, ui
     return ht2_gen_rand_seed(r, global_seed);
 }
 
-template <typename T>
-static cudaError_t growBuf(T*& p, size_t& cap, size_t need, size_t slackNum = 5, size_t slackDen = 4)
-{
-    if (need <= cap && p) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = NULL;
-    size_t ncap = need * slackNum / slackDen + 16;
-    cudaError_t e = cudaMalloc(&p, ncap * sizeof(T));
-    cap = (e == cudaSuccess) ? ncap : 0;
-    return e;
-}
-
 static int slotInit(ht2gpu_handle* h, SamSlot& S)
 {
     if (S.init) return HT2GPU_OK;
     CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 6; i++) CK(cudaEventCreate(&S.ev[i]));
-    if (getenv("HT2GPU_SAM_SPLIT")) for (int i = 0; i < 3; i++) CK(cudaEventCreate(&S.evSplit[i]));
-    CK(cudaMalloc(&S.dCounters, 8 * sizeof(unsigned int)));
-    CK(cudaMalloc(&S.dTally, HT2_T_N * sizeof(unsigned long long)));
-    CK(cudaHostAlloc(&S.hMeta, (HT2_META_TALLY + HT2_T_N) * sizeof(unsigned long long), cudaHostAllocPortable));
+    for (cudaEvent_t& e : S.ev) CK(cudaEventCreate(&e));
+    if (getenv("HT2GPU_SAM_SPLIT")) for (cudaEvent_t& e : S.evSplit) CK(cudaEventCreate(&e));
+    CK(S.dCounters.alloc(8));
+    CK(S.dTally.alloc(HT2_T_N));
+    CK(S.hMeta.alloc(HT2_META_TALLY + HT2_T_N));
     S.init = true;
     return HT2GPU_OK;
 }
@@ -1120,18 +1131,18 @@ static int uploadBatch(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* 
 {
     const uint32_t n = b->n_reads;
     const uint64_t nb = b->offs[n];
-    CK(growBuf(S.dSeq, S.capSeq, nb + 8));
-    if (b->qual) CK(growBuf(S.dQual, S.capQual, nb + 8));
-    CK(growBuf(S.dOffs, S.capOffs, (size_t)n + 1));
-    CK(growBuf(S.dSeeds, S.capSeeds, (size_t)n + 1));
+    CK(S.dSeq.reserve(nb + 8));
+    if (b->qual) CK(S.dQual.reserve(nb + 8));
+    CK(S.dOffs.reserve((size_t)n + 1));
+    CK(S.dSeeds.reserve((size_t)n + 1));
     CK(cudaMemcpyAsync(S.dSeq, b->seq, nb, cudaMemcpyHostToDevice, S.stream));
     if (b->qual) CK(cudaMemcpyAsync(S.dQual, b->qual, nb, cudaMemcpyHostToDevice, S.stream));
     CK(cudaMemcpyAsync(S.dOffs, b->offs, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, S.stream));
     CK(cudaMemcpyAsync(S.dSeeds, b->seeds, (size_t)n * 4, cudaMemcpyHostToDevice, S.stream));
     h2dBytes = nb * (b->qual ? 2 : 1) + ((size_t)n + 1) * 8 + (size_t)n * 4;
     if (names) {
-        CK(growBuf(S.dNames, S.capNames, namesBytes + 8));
-        CK(growBuf(S.dNameOffs, S.capNameOffs, (size_t)n + 1));
+        CK(S.dNames.reserve(namesBytes + 8));
+        CK(S.dNameOffs.reserve((size_t)n + 1));
         CK(cudaMemcpyAsync(S.dNames, names, namesBytes, cudaMemcpyHostToDevice, S.stream));
         CK(cudaMemcpyAsync(S.dNameOffs, nameOffs, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, S.stream));
         h2dBytes += namesBytes + ((size_t)n + 1) * 4;
@@ -1141,13 +1152,12 @@ static int uploadBatch(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* 
 
 static int ensureOut(ht2gpu_handle* h, SamSlot& S, uint32_t units, size_t alns, size_t edits, size_t pairs)
 {
-    CK(growBuf(S.dReads, S.capUnits, units));
-    CK(growBuf(S.dAlns, S.capAlns, alns));
-    CK(growBuf(S.dEdits, S.capEdits, edits));
-    size_t pc = S.capPairs * 2, need = pairs * 2;
-    if (need > pc || !S.dPairs) { CK(growBuf(S.dPairs, pc, need)); S.capPairs = pc / 2; }
+    CK(S.dReads.reserve(units));
+    CK(S.dAlns.reserve(alns));
+    CK(S.dEdits.reserve(edits));
+    CK(S.dPairs.reserve(pairs));
     if (!h->dStats && getenv("HT2GPU_STATS")) {
-        CK(cudaMalloc(&h->dStats, (1024 + 256 * 12) * sizeof(unsigned long long)));
+        CK(h->dStats.alloc(1024 + 256 * 12));
         CK(cudaMemset(h->dStats, 0, (1024 + 256 * 12) * sizeof(unsigned long long)));
     }
     return HT2GPU_OK;
@@ -1164,15 +1174,15 @@ static int launchAlign(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* 
         return HT2GPU_ERR_ARG;
     }
     DevBatch db;
-    db.seq = S.dSeq; db.qual = b->qual ? S.dQual : NULL; db.offs = S.dOffs; db.seeds = S.dSeeds;
-    db.n_units = units; db.paired = b->paired; db.sw = h->P.bowtie2Dp ? wp->dSw : NULL; db.swPool = h->P.bowtie2Dp ? wp->dSwPool : NULL; db.minscTab = h->dMinsc;
+    db.seq = S.dSeq; db.qual = b->qual ? S.dQual.p : NULL; db.offs = S.dOffs; db.seeds = S.dSeeds;
+    db.n_units = units; db.paired = b->paired; db.sw = h->P.bowtie2Dp ? wp->dSw.p : NULL; db.swPool = h->P.bowtie2Dp ? wp->dSwPool.p : NULL; db.minscTab = h->dMinsc;
     { static const int e = getenv("HT2GPU_ELECT") ? atoi(getenv("HT2GPU_ELECT")) : 8; db.elect = (uint32_t)(e < 1 ? 1 : (e > 32 ? 32 : e)); }
 #ifdef HT2_ENABLE_SPLICED
-    db.splT = (const Ht2SplTables*)h->dSplT; db.ssT = h->dSsT;
+    db.splT = (const Ht2SplTables*)h->dSplT.p; db.ssT = h->dSsT;
 #endif
     DevOut o;
-    o.reads = S.dReads; o.alns = S.dAlns; o.edits = S.dEdits; o.pairs = S.dPairs;
-    o.capAlns = (uint32_t)S.capAlns; o.capEdits = (uint32_t)S.capEdits; o.capPairs = (uint32_t)S.capPairs;
+    o.reads = S.dReads; o.alns = S.dAlns; o.edits = S.dEdits; o.pairs = (uint16_t*)S.dPairs.p;
+    o.capAlns = (uint32_t)S.dAlns.cap; o.capEdits = (uint32_t)S.dEdits.cap; o.capPairs = (uint32_t)S.dPairs.cap;
     o.counters = S.dCounters;
     o.stats = h->dStats;
     CK(cudaMemsetAsync(S.dCounters, 0, 8 * sizeof(unsigned int), S.stream));
@@ -1263,7 +1273,7 @@ static int runBatch(ht2gpu_handle* h, const ht2gpu_read_batch_t* b, int iters, h
     if (rc) return rc;
     const uint32_t units = b->paired ? b->n_reads / 2 : b->n_reads;
     uint64_t h2d = 0;
-    CK(cudaEventRecord(S.ev[0], S.stream));
+    CK(cudaEventRecord(S.ev[EV_START], S.stream));
     rc = uploadBatch(h, S, b, NULL, NULL, 0, h2d);
     if (rc) return rc;
     size_t capA = (size_t)b->n_reads * 2 + 1024, capE = (size_t)b->n_reads * 4 + 4096, capP = (size_t)units * 2 + 1024;
@@ -1276,14 +1286,14 @@ static int runBatch(ht2gpu_handle* h, const ht2gpu_read_batch_t* b, int iters, h
         {
             std::lock_guard<std::mutex> lk(h->pool->mu);
             CK(cudaStreamWaitEvent(S.stream, h->pool->evDone, 0));
-            for (int it = 0; it < iters; it++) { rc = launchAlign(h, S, b, units, it == 0 ? S.ev[1] : NULL); if (rc) return rc; nLaunch++; }
-            CK(cudaEventRecord(S.ev[2], S.stream));
+            for (int it = 0; it < iters; it++) { rc = launchAlign(h, S, b, units, it == 0 ? S.ev[EV_ALIGN_START] : NULL); if (rc) return rc; nLaunch++; }
+            CK(cudaEventRecord(S.ev[EV_ALIGN_END], S.stream));
             CK(cudaEventRecord(h->pool->evDone, S.stream));
         }
         CK(cudaMemcpyAsync(counters, S.dCounters, sizeof(counters), cudaMemcpyDeviceToHost, S.stream));
         CK(cudaStreamSynchronize(S.stream));
-        CK(cudaEventElapsedTime(&msKernel, S.ev[1], S.ev[2]));
-        if (counters[0] <= S.capAlns && counters[1] <= S.capEdits && counters[2] <= S.capPairs) break;
+        CK(cudaEventElapsedTime(&msKernel, S.ev[EV_ALIGN_START], S.ev[EV_ALIGN_END]));
+        if (counters[0] <= S.dAlns.cap && counters[1] <= S.dEdits.cap && counters[2] <= S.dPairs.cap) break;
         // result pools were too small: grow and re-run (results are deterministic)
         capA = counters[0] + 1024; capE = counters[1] + 4096; capP = counters[2] + 1024;
     }
@@ -1303,11 +1313,11 @@ static int runBatch(ht2gpu_handle* h, const ht2gpu_read_batch_t* b, int iters, h
     if (counters[0]) CK(cudaMemcpyAsync(hAlns, S.dAlns, (size_t)counters[0] * sizeof(ht2gpu_aln_t), cudaMemcpyDeviceToHost, S.stream));
     if (counters[1]) CK(cudaMemcpyAsync(hEdits, S.dEdits, (size_t)counters[1] * sizeof(ht2gpu_edit_t), cudaMemcpyDeviceToHost, S.stream));
     if (counters[2]) CK(cudaMemcpyAsync(hPairs, S.dPairs, (size_t)counters[2] * 4, cudaMemcpyDeviceToHost, S.stream));
-    CK(cudaEventRecord(S.ev[3], S.stream));
+    CK(cudaEventRecord(S.ev[EV_COPIED], S.stream));
     CK(cudaStreamSynchronize(S.stream));
     float msH2d = 0, msD2h = 0;
-    CK(cudaEventElapsedTime(&msH2d, S.ev[0], S.ev[1]));
-    CK(cudaEventElapsedTime(&msD2h, S.ev[2], S.ev[3]));
+    CK(cudaEventElapsedTime(&msH2d, S.ev[EV_START], S.ev[EV_ALIGN_START]));
+    CK(cudaEventElapsedTime(&msD2h, S.ev[EV_ALIGN_END], S.ev[EV_COPIED]));
     res->n_reads = units; res->reads = hReads;
     res->n_alns = counters[0]; res->alns = hAlns;
     res->n_edits = counters[1]; res->edits = hEdits;
@@ -1349,15 +1359,15 @@ static Ht2SamIn samIn(const ht2gpu_handle* h, const SamSlot& S)
 {
     Ht2SamIn in;
     in.blob = h->dBlob; in.refNames = h->dRefNames; in.minscTab = h->dMinsc;
-    in.seq = S.dSeq; in.qual = S.batch.qual ? S.dQual : NULL; in.offs = S.dOffs; in.names = S.dNames; in.nameOffs = S.dNameOffs;
+    in.seq = S.dSeq; in.qual = S.batch.qual ? S.dQual.p : NULL; in.offs = S.dOffs; in.names = S.dNames; in.nameOffs = S.dNameOffs;
     in.n_reads = S.batch.n_reads; in.paired = S.batch.paired;
-    in.reads = S.dReads; in.alns = S.dAlns; in.edits = S.dEdits; in.pairs = S.dPairs;
+    in.reads = S.dReads; in.alns = S.dAlns; in.edits = S.dEdits; in.pairs = (const uint16_t*)S.dPairs.p;
     in.khits = h->P.khits; in.secondary = h->P.secondary; in.mixed = h->P.mixed; in.discord = h->P.discord;
-    in.ssT = h->samOut.noTlenAdj ? NULL : h->dSsT;
-    in.colCount = h->collectSs ? S.dCounters + 6 : NULL; in.colRecs = S.dColRecs; in.colCap = (uint32_t)S.capCol;
+    in.ssT = h->samOut.noTlenAdj ? NULL : h->dSsT.p;
+    in.colCount = h->collectSs ? S.dCounters + 6 : NULL; in.colRecs = S.dColRecs; in.colCap = (uint32_t)S.dColRecs.cap;
     in.noUnal = h->samOut.noUnal; in.omitSecSeq = h->samOut.omitSecSeq; in.rgTag = h->dRgTag;
     in.rnaStrandness = h->samOut.rnaStrandness; in.noQnameTrunc = h->samOut.noQnameTrunc;
-    in.unitOut = h->recordOut ? S.dOut : NULL;
+    in.unitOut = h->recordOut ? S.dOut.p : NULL;
     return in;
 }
 
@@ -1367,23 +1377,18 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
 {
     const uint32_t units = S.units;
     const uint32_t nBlk = (units + HT2_SAM_TPB - 1) / HT2_SAM_TPB;
-    CK(growBuf(S.dSamLen, S.capSamLen, units));
-    CK(growBuf(S.dBlk, S.capBlk, (size_t)nBlk + 2));
-    if (h->collectSs) CK(growBuf(S.dColRecs, S.capCol, (size_t)S.batch.n_reads * 4 + 1024, 1, 1));
+    CK(S.dSamLen.reserve(units));
+    CK(S.dBlk.reserve((size_t)nBlk + 2));
+    if (h->collectSs) CK(S.dColRecs.reserve((size_t)S.batch.n_reads * 4 + 1024, 1, 1));
     if (h->recordOut) {
-        CK(growBuf(S.dOut, S.capOut, units));
-        if (units > S.capHOut) {
-            if (S.hOut) CK(cudaFreeHost(S.hOut));
-            S.hOut = NULL; S.capHOut = 0;
-            CK(cudaHostAlloc(&S.hOut, (size_t)units + units / 8 + 4096, cudaHostAllocPortable));
-            S.capHOut = (size_t)units + units / 8 + 4096;
-        }
+        CK(S.dOut.reserve(units));
+        CK(S.hOut.reserve(units));
     }
     std::lock_guard<std::mutex> lk(h->pool->mu);
     CK(cudaStreamWaitEvent(S.stream, h->pool->evDone, 0));
-    if (withAlign) { int rc = launchAlign(h, S, &S.batch, units, S.ev[2]); if (rc) return rc; S.nLaunch++; }
-    else CK(cudaEventRecord(S.ev[2], S.stream));
-    CK(cudaEventRecord(S.ev[3], S.stream));
+    if (withAlign) { int rc = launchAlign(h, S, &S.batch, units, S.ev[EV_ALIGN_START]); if (rc) return rc; S.nLaunch++; }
+    else CK(cudaEventRecord(S.ev[EV_ALIGN_START], S.stream));
+    CK(cudaEventRecord(S.ev[EV_ALIGN_END], S.stream));
     if (h->collectSs) CK(cudaMemsetAsync(S.dCounters + 6, 0, sizeof(unsigned int), S.stream));
     // the counting pass tallies the batch's ReportingMetrics; a re-run (ht2gpu_wait_sam) must not count it twice
     CK(cudaMemsetAsync(S.dTally, 0, HT2_T_N * sizeof(unsigned long long), S.stream));
@@ -1393,16 +1398,16 @@ static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
     if (S.evSplit[1]) CK(cudaEventRecord(S.evSplit[1], S.stream));
     ht2_sam_scan_kernel<<<1, 1024, 0, S.stream>>>(S.dBlk, nBlk);
     if (S.evSplit[2]) CK(cudaEventRecord(S.evSplit[2], S.stream));
-    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, h->samStage, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.capSam, S.dCounters,
+    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, h->samStage, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.dSam.cap, S.dCounters,
                                                                         S.dTally, h->samStage);
     CK(cudaGetLastError());
     S.nLaunch += 3;
-    CK(cudaEventRecord(S.ev[4], S.stream));
+    CK(cudaEventRecord(S.ev[EV_SAM_END], S.stream));
     CK(cudaEventRecord(h->pool->evDone, S.stream));
     // meta: total SAM bytes, result counters, reads with errors
-    CK(cudaMemcpyAsync(&S.hMeta[0], S.dBlk + nBlk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
-    CK(cudaMemcpyAsync(&S.hMeta[1], S.dCounters, 8 * sizeof(unsigned int), cudaMemcpyDeviceToHost, S.stream));
-    CK(cudaMemcpyAsync(&S.hMeta[HT2_META_TALLY], S.dTally, HT2_T_N * sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
+    CK(cudaMemcpyAsync(S.hMeta.p, S.dBlk.p + nBlk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
+    CK(cudaMemcpyAsync(S.hMeta.p + 1, S.dCounters, 8 * sizeof(unsigned int), cudaMemcpyDeviceToHost, S.stream));
+    CK(cudaMemcpyAsync(S.hMeta.p + HT2_META_TALLY, S.dTally, HT2_T_N * sizeof(unsigned long long), cudaMemcpyDeviceToHost, S.stream));
     if (h->recordOut) CK(cudaMemcpyAsync(S.hOut, S.dOut, units, cudaMemcpyDeviceToHost, S.stream));
     return HT2GPU_OK;
 }
@@ -1413,6 +1418,26 @@ extern "C" void ht2gpu_host_free(void* p) { if (p) cudaFreeHost(p); }
 extern "C" void ht2gpu_set_error(ht2gpu_handle_t* h, const char* msg) { if (h) h->err = msg ? msg : ""; }
 extern "C" void* ht2gpu_ctx_get(ht2gpu_handle_t* h) { return h ? h->pipeCtx : NULL; }
 extern "C" void ht2gpu_ctx_set(ht2gpu_handle_t* h, void* ctx, void (*release)(void*)) { if (h) { h->pipeCtx = ctx; h->pipeCtxFree = release; } }
+
+// Upload the claimed slot's batch, size its buffers and enqueue its kernels
+static int enqueueBatch(ht2gpu_handle* h, SamSlot& S, const ht2gpu_read_batch_t* b, const char* names, const uint32_t* name_offs,
+                        size_t names_bytes)
+{
+    CK(cudaEventRecord(S.ev[EV_START], S.stream));
+    int rc = uploadBatch(h, S, b, names, name_offs, names_bytes, S.h2dBytes);
+    if (rc) return rc;
+    CK(cudaEventRecord(S.ev[EV_UPLOADED], S.stream));
+    rc = ensureOut(h, S, S.units, (size_t)b->n_reads * 2 + 1024, (size_t)b->n_reads * 4 + 4096, (size_t)S.units * 2 + 1024);
+    if (rc) return rc;
+    // SAM text: ~2.2 bytes per base + ~170 per record at one record per read; grown from the measured size if short
+    // (+ "\tRG:Z:<id>" per record with a read group, + "\tXS:A:<c>" under a known strandness; every name is counted
+    // whole)
+    const size_t rgBytes = h->samOut.rgId.empty() ? 0 : h->samOut.rgTag().size() + 1;
+    const size_t xsBytes = h->samOut.rnaStrandness ? 7 : 0;
+    const size_t est = (size_t)((double)b->offs[b->n_reads] * 2.6) + (size_t)b->n_reads * (260 + rgBytes + xsBytes) + names_bytes + 4096;
+    CK(S.dSam.reserve(est, 1, 1));
+    return enqueueKernels(h, S, true);
+}
 
 extern "C" int ht2gpu_submit_sam(ht2gpu_handle_t* h, int slot, const ht2gpu_read_batch_t* b, const char* names,
                                  const uint32_t* name_offs, size_t names_bytes)
@@ -1428,20 +1453,12 @@ extern "C" int ht2gpu_submit_sam(ht2gpu_handle_t* h, int slot, const ht2gpu_read
     S.batch = *b; S.units = b->paired ? b->n_reads / 2 : b->n_reads; S.namesBytes = names_bytes; S.nLaunch = 0; S.h2dBytes = 0;
     S.pending = true; S.outValid = false;
     if (b->n_reads == 0) return HT2GPU_OK;
-    CK(cudaEventRecord(S.ev[0], S.stream));
-    rc = uploadBatch(h, S, b, names, name_offs, names_bytes, S.h2dBytes);
-    if (rc) return rc;
-    CK(cudaEventRecord(S.ev[1], S.stream));
-    rc = ensureOut(h, S, S.units, (size_t)b->n_reads * 2 + 1024, (size_t)b->n_reads * 4 + 4096, (size_t)S.units * 2 + 1024);
-    if (rc) return rc;
-    // SAM text: ~2.2 bytes per base + ~170 per record at one record per read; grown from the measured size if short
-    // (+ "\tRG:Z:<id>" per record with a read group, + "\tXS:A:<c>" under a known strandness; every name is counted
-    // whole)
-    const size_t rgBytes = h->samOut.rgId.empty() ? 0 : h->samOut.rgTag().size() + 1;
-    const size_t xsBytes = h->samOut.rnaStrandness ? 7 : 0;
-    const size_t est = (size_t)((double)b->offs[b->n_reads] * 2.6) + (size_t)b->n_reads * (260 + rgBytes + xsBytes) + names_bytes + 4096;
-    if (est > S.capSam) CK(growBuf(S.dSam, S.capSam, est, 1, 1));
-    return enqueueKernels(h, S, true);
+    rc = enqueueBatch(h, S, b, names, name_offs, names_bytes);
+    if (rc) {   // the slot is free again once nothing of the batch runs on its stream
+        cudaStreamSynchronize(S.stream);
+        S.pending = false;
+    }
+    return rc;
 }
 
 extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t* out)
@@ -1452,36 +1469,30 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
     if (!S.init || !S.pending) { h->err = "ht2gpu_wait_sam: nothing was submitted on this slot"; return HT2GPU_ERR_ARG; }
     S.pending = false;
     out->n_units = S.units;
-    if (S.batch.n_reads == 0) { out->sam = S.hSam ? S.hSam : (char*)""; S.outValid = h->recordOut; return HT2GPU_OK; }
+    if (S.batch.n_reads == 0) { out->sam = S.hSam.p ? S.hSam.p : (char*)""; S.outValid = h->recordOut; return HT2GPU_OK; }
     CK(cudaSetDevice(h->device));
     for (int attempt = 0; ; attempt++) {
         CK(cudaStreamSynchronize(S.stream));
         const unsigned int* c = (const unsigned int*)&S.hMeta[1];
-        const bool poolsOk = c[0] <= S.capAlns && c[1] <= S.capEdits && c[2] <= S.capPairs;
-        const bool textOk = S.hMeta[0] <= S.capSam;
+        const bool poolsOk = c[0] <= S.dAlns.cap && c[1] <= S.dEdits.cap && c[2] <= S.dPairs.cap;
+        const bool textOk = S.hMeta[0] <= S.dSam.cap;
         if (poolsOk && textOk) break;
         if (attempt >= 3) { h->err = "ht2gpu_wait_sam: result pools still too small after three re-runs"; return HT2GPU_ERR_CUDA; }
         // a pool was too small: grow it and re-run (results are deterministic); rare, sizes are kept afterwards
         if (!poolsOk) { int rc = ensureOut(h, S, S.units, (size_t)c[0] + 1024, (size_t)c[1] + 4096, (size_t)c[2] + 1024); if (rc) return rc; }
-        if (!textOk) CK(growBuf(S.dSam, S.capSam, (size_t)S.hMeta[0] + 4096, 9, 8));
+        if (!textOk) CK(S.dSam.reserve((size_t)S.hMeta[0] + 4096, 9, 8));
         int rc = enqueueKernels(h, S, !poolsOk);
         if (rc) return rc;
     }
     const size_t total = (size_t)S.hMeta[0];
-    if (total + 1 > S.capHSam) {
-        if (S.hSam) cudaFreeHost(S.hSam);
-        S.hSam = NULL; S.capHSam = 0;
-        const size_t cap = total + total / 8 + 4096;
-        CK(cudaHostAlloc(&S.hSam, cap, cudaHostAllocPortable));
-        S.capHSam = cap;
-    }
+    CK(S.hSam.reserve(total + 1));   // and the NUL
     CK(cudaMemcpyAsync(S.hSam, S.dSam, total, cudaMemcpyDeviceToHost, S.stream));
-    CK(cudaEventRecord(S.ev[5], S.stream));
+    CK(cudaEventRecord(S.ev[EV_COPIED], S.stream));
     CK(cudaStreamSynchronize(S.stream));
     S.hSam[total] = 0;
     if (h->collectSs) {
         const unsigned int nrec = ((const unsigned int*)&S.hMeta[1])[6];
-        if (nrec > S.capCol) { h->err = "ht2gpu_wait_sam: more junction records than the batch's buffer holds"; return HT2GPU_ERR_CAPACITY; }
+        if (nrec > S.dColRecs.cap) { h->err = "ht2gpu_wait_sam: more junction records than the batch's buffer holds"; return HT2GPU_ERR_CAPACITY; }
         std::vector<Ht2SsRec> recs(nrec);
         if (nrec) CK(cudaMemcpy(recs.data(), S.dColRecs, (size_t)nrec * sizeof(Ht2SsRec), cudaMemcpyDeviceToHost));
         std::lock_guard<std::mutex> lk(h->novelMu);
@@ -1497,7 +1508,7 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
         float ms[3];
         CK(cudaEventElapsedTime(&ms[0], S.evSplit[0], S.evSplit[1]));
         CK(cudaEventElapsedTime(&ms[1], S.evSplit[1], S.evSplit[2]));
-        CK(cudaEventElapsedTime(&ms[2], S.evSplit[2], S.ev[4]));
+        CK(cudaEventElapsedTime(&ms[2], S.evSplit[2], S.ev[EV_SAM_END]));
         fprintf(stderr, "sam kernels: count %.3f ms  scan %.3f ms  write %.3f ms  total %.3f ms  |  %zu bytes of SAM, %u units  |  "
                 "%.1f GB/s over the three, %.1f GB/s over the writing pass\n", ms[0], ms[1], ms[2], ms[0] + ms[1] + ms[2], total, S.units,
                 total / ((ms[0] + ms[1] + ms[2]) * 1e6), total / (ms[2] * 1e6));
@@ -1506,10 +1517,10 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
     S.outValid = h->recordOut;
     out->sam = S.hSam; out->sam_len = total;
     out->n_alns = c[0]; out->n_err_reads = c[4];
-    CK(cudaEventElapsedTime(&out->ms_h2d, S.ev[0], S.ev[1]));
-    CK(cudaEventElapsedTime(&out->ms_align, S.ev[2], S.ev[3]));
-    CK(cudaEventElapsedTime(&out->ms_sam, S.ev[3], S.ev[4]));
-    CK(cudaEventElapsedTime(&out->ms_d2h, S.ev[4], S.ev[5]));
+    CK(cudaEventElapsedTime(&out->ms_h2d, S.ev[EV_START], S.ev[EV_UPLOADED]));
+    CK(cudaEventElapsedTime(&out->ms_align, S.ev[EV_ALIGN_START], S.ev[EV_ALIGN_END]));
+    CK(cudaEventElapsedTime(&out->ms_sam, S.ev[EV_ALIGN_END], S.ev[EV_SAM_END]));
+    CK(cudaEventElapsedTime(&out->ms_d2h, S.ev[EV_SAM_END], S.ev[EV_COPIED]));
     out->h2d_bytes = S.h2dBytes; out->d2h_bytes = total + 9 * sizeof(unsigned long long) + (h->recordOut ? S.units : 0);
     out->n_launches = S.nLaunch;
     if (c[4]) {
@@ -1522,9 +1533,8 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
 extern "C" int ht2gpu_align_sam(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* b, const char* names, const uint32_t* name_offs,
                                 size_t names_bytes, ht2gpu_sam_result_t* out)
 {
-    int rc = ht2gpu_submit_sam(h, 0, b, names, name_offs, names_bytes);
-    if (rc) { if (h && h->slots[0].init) h->slots[0].pending = false; return rc; }
-    return ht2gpu_wait_sam(h, 0, out);
+    const int rc = ht2gpu_submit_sam(h, 0, b, names, name_offs, names_bytes);
+    return rc ? rc : ht2gpu_wait_sam(h, 0, out);
 }
 
 // ---------------------------------------------------------------------------
@@ -1618,31 +1628,18 @@ extern "C" int ht2gpu_sw_selftest(int device, uint32_t n, uint32_t seed, uint64_
         q.minsc = -(int64_t)(10 + rnd(3 * q.nrow));
     }
     const int grid = 64;
-    SwTestProblem* dP = NULL; Ht2SwScratch* dS = NULL; uint32_t* dPool = NULL; unsigned long long* dOut = NULL;
-    int rc = HT2GPU_OK;
-    if (cudaMalloc(&dP, sizeof(SwTestProblem) * (size_t)(n ? n : 1)) != cudaSuccess || cudaMalloc(&dS, sizeof(Ht2SwScratch) * 2 * grid) != cudaSuccess ||
-        cudaMalloc(&dPool, sizeof(uint32_t) * (size_t)HT2_SW_POOL_WORDS * 2 * grid) != cudaSuccess || cudaMalloc(&dOut, 4 * sizeof(unsigned long long)) != cudaSuccess) rc = HT2GPU_ERR_CUDA;
-    if (rc == HT2GPU_OK) {
-        cudaMemcpy(dP, probs.data(), sizeof(SwTestProblem) * (size_t)n, cudaMemcpyHostToDevice);
-        cudaMemset(dOut, 0, 4 * sizeof(unsigned long long));
-        cudaMemset(dS, 0, sizeof(Ht2SwScratch) * 2 * grid);
-        size_t lim = 0; cudaDeviceGetLimit(&lim, cudaLimitStackSize);
-        if (lim < 8192) cudaDeviceSetLimit(cudaLimitStackSize, 8192);
-        ht2_sw_selftest_kernel<<<grid, 32>>>(dP, n, dS, dPool, dOut);
-        unsigned long long o4[4] = {0, 0, 0, 0};
-        if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(o4, dOut, sizeof(o4), cudaMemcpyDeviceToHost) != cudaSuccess) rc = HT2GPU_ERR_CUDA;
-        for (int i = 0; i < 4; i++) out[i] = o4[i];
-    }
-    cudaFree(dP); cudaFree(dS); cudaFree(dPool); cudaFree(dOut);
+    DevBuf<SwTestProblem> dP; DevBuf<Ht2SwScratch> dS; DevBuf<uint32_t> dPool; DevBuf<unsigned long long> dOut;
+    if (dP.alloc(n ? n : 1) || dS.alloc(2 * grid) || dPool.alloc((size_t)HT2_SW_POOL_WORDS * 2 * grid) || dOut.alloc(4)) return HT2GPU_ERR_CUDA;
+    cudaMemcpy(dP, probs.data(), sizeof(SwTestProblem) * (size_t)n, cudaMemcpyHostToDevice);
+    cudaMemset(dOut, 0, 4 * sizeof(unsigned long long));
+    cudaMemset(dS, 0, sizeof(Ht2SwScratch) * 2 * grid);
+    size_t lim = 0; cudaDeviceGetLimit(&lim, cudaLimitStackSize);
+    if (lim < 8192) cudaDeviceSetLimit(cudaLimitStackSize, 8192);
+    ht2_sw_selftest_kernel<<<grid, 32>>>(dP, n, dS, dPool, dOut);
+    unsigned long long o4[4] = {0, 0, 0, 0};
+    const int rc = cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(o4, dOut, sizeof(o4), cudaMemcpyDeviceToHost) != cudaSuccess ? HT2GPU_ERR_CUDA : HT2GPU_OK;
+    for (int i = 0; i < 4; i++) out[i] = o4[i];
     return rc;
-}
-
-namespace {
-struct DevTmp {   // temporaries of one ht2gpu_seed_search / ht2gpu_sw_extend call: freed on every return path
-    std::vector<void*> ptrs;
-    template <typename T> cudaError_t alloc(T*& p, size_t bytes) { void* q = NULL; cudaError_t e = cudaMalloc(&q, bytes); if (e == cudaSuccess) ptrs.push_back(q); p = (T*)q; return e; }
-    ~DevTmp() { for (void* q : ptrs) cudaFree(q); }
-};
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1712,17 +1709,16 @@ extern "C" int ht2gpu_sw_extend(ht2gpu_handle_t* h, uint32_t n, const ht2gpu_sw_
     for (uint32_t i = 0; i < n; i++) { const size_t e = (size_t)jobs[i].read_off + jobs[i].read_len; if (e > bases) bases = e; }
     CK(cudaSetDevice(h->device));
     const uint32_t nt = (n + 31) / 32 * 32;                  // every lane of a launched warp indexes its own scratch
-    DevTmp tmp;
-    ht2gpu_sw_job_t* dJobs = NULL; uint8_t *dSeq = NULL, *dQual = NULL; Ht2Work* dWork = NULL; Ht2SwScratch* dScr = NULL;
-    uint32_t* dPool = NULL; ht2gpu_sw_result_t* dRes = NULL; ht2gpu_edit_t* dEd = NULL;
-    CK(tmp.alloc(dJobs, sizeof(ht2gpu_sw_job_t) * n));
-    CK(tmp.alloc(dSeq, bases + 1));
-    CK(tmp.alloc(dQual, bases + 1));
-    CK(tmp.alloc(dWork, sizeof(Ht2Work) * n));
-    CK(tmp.alloc(dScr, sizeof(Ht2SwScratch) * nt));
-    CK(tmp.alloc(dPool, sizeof(uint32_t) * (size_t)HT2_SW_POOL_WORDS * nt));
-    CK(tmp.alloc(dRes, sizeof(ht2gpu_sw_result_t) * n));
-    CK(tmp.alloc(dEd, sizeof(ht2gpu_edit_t) * (size_t)HT2GPU_SW_MAX_EDITS * n));
+    DevBuf<ht2gpu_sw_job_t> dJobs; DevBuf<uint8_t> dSeq, dQual; DevBuf<Ht2Work> dWork; DevBuf<Ht2SwScratch> dScr;
+    DevBuf<uint32_t> dPool; DevBuf<ht2gpu_sw_result_t> dRes; DevBuf<ht2gpu_edit_t> dEd;
+    CK(dJobs.alloc(n));
+    CK(dSeq.alloc(bases + 1));
+    CK(dQual.alloc(bases + 1));
+    CK(dWork.alloc(n));
+    CK(dScr.alloc(nt));
+    CK(dPool.alloc((size_t)HT2_SW_POOL_WORDS * nt));
+    CK(dRes.alloc(n));
+    CK(dEd.alloc((size_t)HT2GPU_SW_MAX_EDITS * n));
     CK(cudaMemcpy(dJobs, jobs, sizeof(ht2gpu_sw_job_t) * n, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(dSeq, seq, bases, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(dQual, qual, bases, cudaMemcpyHostToDevice));
@@ -1763,29 +1759,28 @@ extern "C" int ht2gpu_seed_search(ht2gpu_handle_t* h, const ht2gpu_read_batch_t*
 #ifdef HT2_ENABLE_SPLICED
     db.splT = NULL; db.ssT = NULL;
 #endif
-    DevTmp tmp;
-    uint32_t *dCounts = NULL, *dOffs3 = NULL;
-    unsigned long long* dTot = NULL;
+    DevBuf<uint32_t> dCounts, dOffs3;
+    DevBuf<unsigned long long> dTot;
     SeedOut so; memset(&so, 0, sizeof(so));
-    CK(tmp.alloc(dCounts, (size_t)n * 12));
-    CK(tmp.alloc(dOffs3, (size_t)n * 12));
-    CK(tmp.alloc(dTot, 3 * sizeof(unsigned long long)));
+    CK(dCounts.alloc((size_t)n * 3));
+    CK(dOffs3.alloc((size_t)n * 3));
+    CK(dTot.alloc(3));
     CK(cudaMemsetAsync(dTot, 0, 3 * sizeof(unsigned long long), S.stream));
     so.counts = dCounts; so.offs = dOffs3; so.totals = dTot;
     const int tpb = 128;
     int grid = (int)((n + tpb - 1) / tpb);
     const int maxGrid = h->nSM * 16;
     if (grid > maxGrid) grid = maxGrid;
-    CK(cudaEventRecord(S.ev[1], S.stream));
+    CK(cudaEventRecord(S.ev[EV_ALIGN_START], S.stream));
     if (h->graph) ht2_seed_kernel<true, false><<<grid, tpb, 0, S.stream>>>(h->dBlob, h->P, db, n, maxRange, so);
     else ht2_seed_kernel<false, false><<<grid, tpb, 0, S.stream>>>(h->dBlob, h->P, db, n, maxRange, so);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(S.ev[2], S.stream));
+    CK(cudaEventRecord(S.ev[EV_ALIGN_END], S.stream));
     std::vector<uint32_t> counts((size_t)n * 3), offs((size_t)n * 3);
     CK(cudaMemcpyAsync(counts.data(), dCounts, (size_t)n * 12, cudaMemcpyDeviceToHost, S.stream));
     CK(cudaStreamSynchronize(S.stream));
     float ms0 = 0, ms1 = 0;
-    CK(cudaEventElapsedTime(&ms0, S.ev[1], S.ev[2]));
+    CK(cudaEventElapsedTime(&ms0, S.ev[EV_ALIGN_START], S.ev[EV_ALIGN_END]));
     uint64_t th = 0, te = 0, tc = 0;
     for (uint32_t i = 0; i < n; i++) {
         offs[3 * (size_t)i] = (uint32_t)th; offs[3 * (size_t)i + 1] = (uint32_t)te; offs[3 * (size_t)i + 2] = (uint32_t)tc;
@@ -1794,17 +1789,17 @@ extern "C" int ht2gpu_seed_search(ht2gpu_handle_t* h, const ht2gpu_read_batch_t*
     }
     pv->firstHit[n] = (uint32_t)th;
     if (th > 0xfffffff0ull || tc > 0xfffffff0ull) { h->err = "seed search result too large for one batch"; return HT2GPU_ERR_CAPACITY; }
-    ht2gpu_seed_hit_t* dHits = NULL; uint16_t* dIe = NULL; ht2gpu_seed_coord_t* dCo = NULL;
-    CK(tmp.alloc(dHits, (th + 1) * sizeof(ht2gpu_seed_hit_t)));
-    CK(tmp.alloc(dIe, (te + 1) * 4));
-    CK(tmp.alloc(dCo, (tc + 1) * sizeof(ht2gpu_seed_coord_t)));
+    DevBuf<ht2gpu_seed_hit_t> dHits; DevBuf<uint16_t> dIe; DevBuf<ht2gpu_seed_coord_t> dCo;
+    CK(dHits.alloc(th + 1));
+    CK(dIe.alloc((te + 1) * 2));   // two per iedge
+    CK(dCo.alloc(tc + 1));
     CK(cudaMemcpyAsync(dOffs3, offs.data(), (size_t)n * 12, cudaMemcpyHostToDevice, S.stream));
     so.hits = dHits; so.iedges = dIe; so.coords = dCo;
-    CK(cudaEventRecord(S.ev[1], S.stream));
+    CK(cudaEventRecord(S.ev[EV_ALIGN_START], S.stream));
     if (h->graph) ht2_seed_kernel<true, true><<<grid, tpb, 0, S.stream>>>(h->dBlob, h->P, db, n, maxRange, so);
     else ht2_seed_kernel<false, true><<<grid, tpb, 0, S.stream>>>(h->dBlob, h->P, db, n, maxRange, so);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(S.ev[2], S.stream));
+    CK(cudaEventRecord(S.ev[EV_ALIGN_END], S.stream));
     pv->hits.resize(th); pv->iedges.resize(te * 2); pv->coords.resize(tc);
     unsigned long long tot[3] = {0, 0, 0};
     if (th) CK(cudaMemcpyAsync(pv->hits.data(), dHits, th * sizeof(ht2gpu_seed_hit_t), cudaMemcpyDeviceToHost, S.stream));
@@ -1812,7 +1807,7 @@ extern "C" int ht2gpu_seed_search(ht2gpu_handle_t* h, const ht2gpu_read_batch_t*
     if (tc) CK(cudaMemcpyAsync(pv->coords.data(), dCo, tc * sizeof(ht2gpu_seed_coord_t), cudaMemcpyDeviceToHost, S.stream));
     CK(cudaMemcpyAsync(tot, dTot, sizeof(tot), cudaMemcpyDeviceToHost, S.stream));
     CK(cudaStreamSynchronize(S.stream));
-    CK(cudaEventElapsedTime(&ms1, S.ev[1], S.ev[2]));
+    CK(cudaEventElapsedTime(&ms1, S.ev[EV_ALIGN_START], S.ev[EV_ALIGN_END]));
     res->n_hits = (uint32_t)th; res->hits = pv->hits.data();
     res->n_iedges = (uint32_t)te; res->iedges = pv->iedges.data();
     res->n_coords = (uint32_t)tc; res->coords = pv->coords.data();
@@ -1842,17 +1837,27 @@ extern "C" int ht2gpu_sam_header(ht2gpu_handle_t* h, char** out, size_t* out_len
 }
 extern "C" void ht2gpu_free_text(char* p) { free(p); }
 
+// What a batch in flight reads (the splice-site DB, the SAM output settings, whether outcomes are recorded) changes
+// only while no slot of the handle holds a batch: ht2gpu_wait_sam may re-run the batch's kernels.
+static int refuseInFlight(ht2gpu_handle* h, const char* call)
+{
+    for (const SamSlot& S : h->slots)
+        if (S.pending) { h->err = std::string(call) + ": a batch is in flight (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
+    return HT2GPU_OK;
+}
+
 // The run's read-only splice-site DB: --known-splicesite-infile / --novel-splicesite-infile (hisat2.cpp:4101-4116,
-// SpliceSiteDB::read splice_site.cpp:727).  Replaces a DB loaded earlier.  Call between batches, not during one.
+// SpliceSiteDB::read splice_site.cpp:727).  Replaces a DB loaded earlier.  Refused while a batch is in flight.
 extern "C" int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_path, const char* novel_path, uint32_t* n_sites)
 {
     if (!h) return HT2GPU_ERR_ARG;
+    if (int rc = refuseInFlight(h, "ht2gpu_load_splicesites")) return rc;
 #ifdef HT2_ENABLE_SPLICED
     std::vector<Ht2SsFile> files;
     if (known_path && *known_path) files.push_back({known_path, true});
     if (novel_path && *novel_path) files.push_back({novel_path, false});
     if (h->collectSs && files.size()) { h->err = "ht2gpu: a splice-site DB cannot be loaded while novel splice sites are collected"; return HT2GPU_ERR_UNSUPPORTED; }
-    if (h->dSsT) { cudaFree(h->dSsT); h->dSsT = NULL; }
+    h->dSsT.release();
     h->ssBlob.clear();
     if (n_sites) *n_sites = 0;
     if (files.empty()) return HT2GPU_OK;
@@ -1860,8 +1865,7 @@ extern "C" int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_pat
     std::string err; uint32_t ns = 0;
     if (!ht2_ssdb_build(*h->img, files, h->ssBlob, ns, err, &h->refNames)) { h->err = err; h->ssBlob.clear(); return HT2GPU_ERR_INDEX; }
     CK(cudaSetDevice(h->device));
-    CK(cudaMalloc(&h->dSsT, h->ssBlob.size()));
-    CK(cudaMemcpy(h->dSsT, h->ssBlob.data(), h->ssBlob.size(), cudaMemcpyHostToDevice));
+    CK(h->dSsT.upload(h->ssBlob.data(), h->ssBlob.size()));
     if (n_sites) *n_sites = ns;
     return HT2GPU_OK;
 #else
@@ -1909,8 +1913,7 @@ extern "C" int ht2gpu_format_sam(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* 
 extern "C" int ht2gpu_record_outcomes(ht2gpu_handle_t* h, int enable)
 {
     if (!h) return HT2GPU_ERR_ARG;
-    for (int k = 0; k < HT2GPU_N_SLOTS; k++)
-        if (h->slots[k].pending) { h->err = "ht2gpu_record_outcomes: a batch is in flight (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
+    if (int rc = refuseInFlight(h, "ht2gpu_record_outcomes")) return rc;
     h->recordOut = enable != 0;
     return HT2GPU_OK;
 }
@@ -1935,8 +1938,7 @@ extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output
 {
     if (!h || !cfg || cfg->n_rg < 0 || (cfg->n_rg > 0 && !cfg->rg)) return HT2GPU_ERR_ARG;
     if (cfg->rna_strandness < 0 || cfg->rna_strandness > 4) { h->err = "ht2gpu_set_sam_output: rna_strandness must be 0 (unknown) .. 4 (RF)"; return HT2GPU_ERR_ARG; }
-    for (int k = 0; k < HT2GPU_N_SLOTS; k++)
-        if (h->slots[k].pending) { h->err = "ht2gpu_set_sam_output: a batch is in flight (call ht2gpu_wait_sam first)"; return HT2GPU_ERR_ARG; }
+    if (int rc = refuseInFlight(h, "ht2gpu_set_sam_output")) return rc;
     Ht2SamOutput so;
     so.noUnal = cfg->no_unal != 0; so.omitSecSeq = cfg->omit_sec_seq != 0; so.noSq = cfg->no_sq != 0;
     so.rnaStrandness = (uint32_t)cfg->rna_strandness; so.noQnameTrunc = cfg->no_qname_trunc != 0; so.noTlenAdj = cfg->no_templatelen_adjustment != 0;
@@ -1944,12 +1946,9 @@ extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output
     for (int i = 0; i < cfg->n_rg; i++) { if (!cfg->rg[i]) return HT2GPU_ERR_ARG; so.rg.push_back(cfg->rg[i]); }
     CK(cudaSetDevice(h->device));
     for (int k = 0; k < HT2GPU_N_SLOTS; k++) if (h->slots[k].init) CK(cudaStreamSynchronize(h->slots[k].stream));
-    if (h->dRgTag) { CK(cudaFree(h->dRgTag)); h->dRgTag = NULL; }
+    h->dRgTag.release();
     const std::string tag = so.rgTag();
-    if (!tag.empty()) {
-        CK(cudaMalloc(&h->dRgTag, tag.size() + 1));
-        CK(cudaMemcpy(h->dRgTag, tag.c_str(), tag.size() + 1, cudaMemcpyHostToDevice));
-    }
+    if (!tag.empty()) CK(h->dRgTag.upload(tag.c_str(), tag.size() + 1));
     h->samOut = so;
     return HT2GPU_OK;
 }

@@ -555,6 +555,8 @@ struct Run {
             if (rc == HT2GPU_OK && !F->released && (F->exhausted || F->lastBatch >= 0)) { const int v = F->verify(e); if (v) fail(v, e); }
         if (rc != HT2GPU_OK)   // a failed inflate explains a failed run better than what the parser made of its bytes
             for (InFile* F : files) { const int z = F->verify(e, false); if (z) { std::lock_guard<std::mutex> lk(mu); rc = z; err = e; } }
+        if (rc != HT2GPU_OK)   // drain the batches still in flight (a handle refuses to stop recording outcomes before)
+            for (int s = 0; s < nSlots; s++) if (state[s] == 1) { ht2gpu_sam_result_t r; ht2gpu_wait_sam(hs[s % nDev], s / nDev, &r); }
         if (route) {
             const double tr = nowS();
             router.finish();
@@ -563,8 +565,6 @@ struct Run {
             routes->s_route = routeS;
             for (int i = 0; i < nDev; i++) ht2gpu_record_outcomes(hs[i], 0);
         }
-        if (rc != HT2GPU_OK)   // drain the batches still in flight
-            for (int s = 0; s < nSlots; s++) if (state[s] == 1) { ht2gpu_sam_result_t r; ht2gpu_wait_sam(hs[s % nDev], s / nDev, &r); }
         for (InFile* F : files) F->release(C->gz);
         S.s_index = indexS; S.s_parse = parseS; S.s_submit = submitS; S.s_wait = waitS; S.s_sink = sinkS; S.s_total = nowS() - t0;
         if (st) *st = S;

@@ -198,8 +198,8 @@ void ht2gpu_free_results(ht2gpu_result_batch_t* res);
  * ht2gpu_submit_sam enqueues a batch on one of ht2gpu_sam_slots() slots and returns; ht2gpu_wait_sam blocks
  * until that batch is done and hands back its text (valid until the next submit on the same slot).  Slots have
  * their own streams and buffers, so the copies of one batch overlap the kernels of another; the host buffers
- * of a submitted batch must stay valid (ideally pinned) until its wait returns.  One thread at a time per
- * slot; ht2gpu_align_batch / ht2gpu_align_sam / ht2gpu_seed_search use slot 0. */
+ * of a submitted batch must stay valid (ideally pinned) until its wait returns; a failed submit leaves the slot
+ * free and nothing of it running.  One thread at a time per slot; ht2gpu_align_batch / _align_sam / _seed_search use slot 0. */
 typedef struct {
     char*    sam;          /* pinned host memory owned by the library, '\0'-terminated */
     size_t   sam_len;
@@ -490,7 +490,7 @@ uint32_t ht2gpu_read_seed(const uint8_t* seq, const uint8_t* qual, uint32_t len,
  * three `if(!ssdb.empty())` branches of hybridSearch_recur (spliced_aligner.h:409-668, 685-811, 1365-1494):
  * short exon ends next to a listed site are aligned across it, and the template length of a concordant pair
  * excludes the longest listed intron between the mates (aligner_result.h:1631-1690).  Replaces a DB loaded
- * earlier; not to be called while a batch is in flight.  Temporary sites (learned while aligning) are not
+ * earlier; refused (HT2GPU_ERR_ARG) while a batch is in flight.  Temporary sites (learned while aligning) are not
  * modelled: the reference's own output depends on thread timing there (DESIGN.md). */
 int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_path, const char* novel_path, uint32_t* n_sites);
 

@@ -6,15 +6,18 @@
 //   - ht2gpu_wait_sam formats the batch from the caller's staging when it is waited for, not when it is submitted: the
 //     staging must stay valid until the wait, so a pipeline that reuses it too early writes wrong reads.  One line per
 //     read: name, sequence (ACGTN), qualities or '*', seed, tab-separated;
-//   - ht2gpu_unit_outcomes gives unit u the outcome FNV-1a(name of its first read) & 7.
+//   - ht2gpu_unit_outcomes gives unit u the outcome FNV-1a(name of its first read) & 7;
+//   - ht2gpu_record_outcomes is refused while a slot of the handle holds a batch, as the library refuses it.
 //
 //   ht2_pipesim [-1 a,b -2 c,d] [-U e,f] [-f|-q] [-s N] [-u N] [--batch N] [-p N] [--gpus N] [--slots N]
 //               [--un P] [--al P] [--un-conc P] [--al-conc P] [--al-conc-disc P]       ('%' in a -conc path: 1 / 2)
 //               [--fail-wait K] [--sleep SEED] [--routed] -S out.txt [--log batches.txt]
 //       runs ht2gpu_run_reads_files (ht2gpu_run_reads_routed on a single -U file or -1/-2 pair with --routed), writes
 //       the reads, the read files and one line per waited batch ("device slot paired n_reads"), and prints the run's
-//       stats and the summed gunzip stats as "key=value" pairs.  --fail-wait K: the wait of batch K fails.  --sleep:
-//       each wait sleeps a pseudo-random 0..500 us.  Exit 1 with the run's message on stderr when the run fails.
+//       stats, the summed gunzip stats and, per handle i, outcomes_i (recording on) and busy_i (slots holding a batch)
+//       as "key=value" pairs.  --fail-wait K: the wait of batch K fails; where the handles have another slot, it first
+//       waits (up to 5 s) until a later batch is in flight, and in_flight_at_fail is 1 if one was.  --sleep: each
+//       wait sleeps a pseudo-random 0..500 us.  Exit 1 with the run's message on stderr when the run fails.
 //   ht2_pipesim --parse [-1 a -2 b | -U a] [-f|-q] [-s N] [-u N] -S out.txt
 //       the same lines from ht2gpu_parse_reads (the whole input as one batch).
 //   ht2_pipesim --route [-1 a -2 b | -U a] [-f|-q] [-s N] [-u N] --outcomes F [--un P ...]
@@ -34,8 +37,10 @@
 #include "../../hisat2_b200/csrc/ht2_inflate.h"
 
 namespace {
-int gSlots = 2;
+int gSlots = 2, gGpus = 1;
 int64_t gFailWait = -1;
+std::atomic<int> gBusy{0};   // slots of every handle that hold a batch
+bool gInFlightAtFail = false;
 uint64_t gSleepSeed = 0;
 bool gSleep = false;
 std::atomic<int64_t> gWaits{0};
@@ -91,14 +96,20 @@ int ht2gpu_submit_sam(ht2gpu_handle_t* h, int slot, const ht2gpu_read_batch_t* b
     if (name_offs[batch->n_reads] != names_bytes) { ht2gpu_set_error(h, "fake device: names_bytes"); return HT2GPU_ERR_ARG; }
     ht2gpu_handle::Slot& s = h->slots[slot];
     s.busy = true; s.rb = *batch; s.names = names; s.nameOffs = name_offs;
+    gBusy++;
     return HT2GPU_OK;
 }
 int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t* out)
 {
     if (slot < 0 || slot >= (int)h->slots.size() || !h->slots[slot].busy) { ht2gpu_set_error(h, "fake device: nothing submitted"); return HT2GPU_ERR_ARG; }
     ht2gpu_handle::Slot& s = h->slots[slot];
-    s.busy = false;
     const int64_t k = gWaits++;
+    if (k == gFailWait && gSlots * gGpus > 1) {   // fail with a later batch in flight, where the producer has one
+        for (int t = 0; t < 5000 && gBusy < 2; t++) std::this_thread::sleep_for(std::chrono::milliseconds(1));
+        gInFlightAtFail = gBusy >= 2;
+    }
+    s.busy = false;
+    gBusy--;
     if (gSleep) {
         uint64_t x = (gSleepSeed + (uint64_t)k) * 0x9E3779B97F4A7C15ull;
         x ^= x >> 29;
@@ -119,7 +130,13 @@ int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t* out)
     out->sam = &s.sam[0]; out->sam_len = s.sam.size(); out->n_units = (uint32_t)s.out.size();
     return HT2GPU_OK;
 }
-int ht2gpu_record_outcomes(ht2gpu_handle_t* h, int enable) { h->outcomes = enable != 0; return HT2GPU_OK; }
+int ht2gpu_record_outcomes(ht2gpu_handle_t* h, int enable)
+{
+    for (const ht2gpu_handle::Slot& s : h->slots)
+        if (s.busy) { ht2gpu_set_error(h, "fake device: ht2gpu_record_outcomes: a batch is in flight"); return HT2GPU_ERR_ARG; }
+    h->outcomes = enable != 0;
+    return HT2GPU_OK;
+}
 int ht2gpu_unit_outcomes(ht2gpu_handle_t* h, int slot, const uint8_t** bytes, uint32_t* n_units)
 {
     if (!h->outcomes || slot < 0 || slot >= (int)h->slots.size()) { ht2gpu_set_error(h, "fake device: outcomes are off"); return HT2GPU_ERR_ARG; }
@@ -216,7 +233,7 @@ int main(int argc, char** argv)
         else if (a == "-u") in.upto = strtoull(val(), NULL, 10);
         else if (a == "--batch") in.batch_reads = (uint32_t)strtoul(val(), NULL, 10);
         else if (a == "-p") in.threads = atoi(val());
-        else if (a == "--gpus") gpus = atoi(val());
+        else if (a == "--gpus") gGpus = gpus = atoi(val());
         else if (a == "--slots") gSlots = atoi(val());
         else if (a == "--fail-wait") gFailWait = atoll(val());
         else if (a == "--sleep") { gSleep = true; gSleepSeed = strtoull(val(), NULL, 10); }
@@ -296,6 +313,12 @@ int main(int argc, char** argv)
            (unsigned long long)st.n_reads, (unsigned long long)st.n_units, (unsigned long long)st.n_batches,
            (unsigned long long)st.sam_bytes, (unsigned long long)routes.n_spans, (unsigned long long)routes.bytes,
            (unsigned long long)gz.in_bytes, (unsigned long long)gz.out_bytes, (unsigned long long)gz.members);
+    for (int g = 0; g < gpus; g++) {
+        int busy = 0;
+        for (const ht2gpu_handle::Slot& s : hs[g]->slots) busy += s.busy;
+        printf("outcomes_%d=%d busy_%d=%d\n", g, (int)hs[g]->outcomes, g, busy);
+    }
+    printf("in_flight_at_fail=%d\n", (int)gInFlightAtFail);
     if (rc != HT2GPU_OK) fprintf(stderr, "error: %s\n", ht2gpu_last_error(hs[0]));
     for (ht2gpu_handle* h : hs) { if (h->release) h->release(h->ctx); delete h; }
     return rc == HT2GPU_OK ? 0 : 1;

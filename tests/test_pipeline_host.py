@@ -218,6 +218,14 @@ def test_single_input_entry_point(pipesim, corpus, tmp_path_factory, tmp_path, v
             assert all(int(l.split()[2]) == paired for l in log.splitlines())
 
 
+def assert_handles_idle(r, gpus):
+    """After a run, failed or not: every handle has outcome recording off and no slot holding a batch."""
+    st = dict(kv.split(b"=") for kv in r.stdout.split())
+    for g in range(gpus):
+        assert (st[b"outcomes_%d" % g], st[b"busy_%d" % g]) == (b"0", b"0"), (g, r.stdout)
+    return st
+
+
 def corrupt(src, dst):
     """A gzip file whose last member's CRC-32 is wrong: every byte inflates, the check fails."""
     b = bytearray(open(src, "rb").read())
@@ -228,7 +236,8 @@ def corrupt(src, dst):
 @pytest.mark.parametrize("variant", list(VARIANTS))
 def test_errors(pipesim, corpus, tmp_path, variant):
     """Mate totals that differ, a missing file, a corrupt gzip file in a list and a failed wait end the run with their
-    message, write nothing they must not, and never hang."""
+    message, write nothing they must not, never hang, and leave every handle with outcome recording off and no batch in
+    flight.  Every run routes reads (read files), so recording is on while it runs."""
     exe = pipesim[variant]
     cfgs = [(7, 4, 2, 8), (64, 1, 1, 1)]
     # -1 and -2 totals that differ: the reference's message (pat.cpp:270, 279); not an error when -u ends the run first
@@ -240,6 +249,7 @@ def test_errors(pipesim, corpus, tmp_path, variant):
             assert r.returncode == 1
             other = 3 - short
             assert b"fewer reads in file specified with -%d than in file specified with -%d" % (short, other) in r.stderr
+            assert_handles_idle(r, cfg[2])
         r, sam, _, _ = run_case(exe, corpus, str(tmp_path / ("mates%d_u" % short)), "pe_two_lanes", cfgs[0],
                                 inputs=inputs, extra=["-u", "300"])
         assert r.returncode == 0 and sam.count(b"\n") == 600
@@ -248,6 +258,7 @@ def test_errors(pipesim, corpus, tmp_path, variant):
         inputs = ["-U", d + "s1.fq," + d + "no_such_file.fq"]
         r, sam, log, got = run_case(exe, corpus, str(tmp_path / ("missing%d" % j)), "se_fq_plain_gz_bgzf", cfg, inputs=inputs)
         assert r.returncode == 1 and b"no_such_file.fq" in r.stderr
+        assert_handles_idle(r, cfg[2])
         assert sam == b"" and log == "" and all(v == b"" for v in got.values())
     # a corrupt gzip file: the inflate's message; no record of it (or after it) is written, nothing at all when it is first
     bad = str(tmp_path / "bad.fq.gz")
@@ -261,6 +272,7 @@ def test_errors(pipesim, corpus, tmp_path, variant):
         r, sam, _, got = run_case(exe, corpus, str(tmp_path / ("bad_mid%d" % j)), "se_fq_plain_gz_bgzf", cfg,
                                   inputs=["-U", ",".join([d + "s1.fq", bad, d + "s3.fq.bgz"])])
         assert r.returncode == 1 and b"gzip input: " in r.stderr
+        assert_handles_idle(r, cfg[2])
         msgs.add(r.stderr.split(b"error: ")[-1])
         lines = sam.splitlines(True)
         assert lines == s1[:len(lines)]
@@ -269,16 +281,20 @@ def test_errors(pipesim, corpus, tmp_path, variant):
         for first in (["-U", bad + "," + d + "s1.fq"], ["-1", d + "p1a.fq," + d + "p1b.fq.gz", "-2", bad + "," + d + "p2b.fq"]):
             r, sam, _, got = run_case(exe, corpus, str(tmp_path / ("bad_first%d" % j)), "se_fq_plain_gz_bgzf", cfg, inputs=first)
             assert r.returncode == 1 and b"gzip input: " in r.stderr
+            assert_handles_idle(r, cfg[2])
             msgs.add(r.stderr.split(b"error: ")[-1])
             assert sam == b"" and all(v == b"" for v in got.values())
     assert len(msgs) == 1, msgs
-    # a failed wait: the device's message; the batches before it reached the sink, in order
+    # a failed wait: the device's message; the batches before it reached the sink, in order.  With 4 slots on each of 2
+    # devices, the wait fails while later batches are in flight: they are drained before recording is turned off.
     reads = None
     for k in (0, 3):
         for j, cfg in enumerate(cfgs):
             r, sam, log, _ = run_case(exe, corpus, str(tmp_path / ("wait%d_%d" % (k, j))), "mixed_read_files_no_unal_new_summary",
                                       cfg, extra=["--fail-wait", str(k)])
             assert r.returncode == 1 and b"fake device: the wait of batch %d failed" % k in r.stderr
+            st = assert_handles_idle(r, cfg[2])
+            assert st[b"in_flight_at_fail"] == (b"1" if cfg[1] * cfg[2] > 1 else b"0"), (k, cfg)
             n = sum(int(l.split()[3]) for l in log.splitlines()[:k])
             if reads is None:
                 full = run_case(pipesim["plain"], corpus, str(tmp_path / "wait_full"), "mixed_read_files_no_unal_new_summary", cfg)
