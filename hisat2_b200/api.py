@@ -26,10 +26,13 @@ class Options(C.Structure):
         "ignore_quals", "nofw", "norc", "min_frag", "max_frag", "no_mixed", "no_discordant")] + [
         ("seed", C.c_uint32), ("threads_per_block", C.c_int32), ("blocks_per_sm", C.c_int32), ("slots_per_lane", C.c_int32), ("warp_per_read", C.c_int32),
         ("bowtie2_dp", C.c_int32), ("gbar", C.c_int32), ("score_min_type", C.c_int32),
-        ("score_min_const", C.c_double), ("score_min_coeff", C.c_double), ("chr_names", C.c_int32)]
+        ("score_min_const", C.c_double), ("score_min_coeff", C.c_double), ("chr_names", C.c_int32),
+        ("pe_orient", C.c_int32), ("n_ceil_type", C.c_int32), ("n_ceil_const", C.c_double), ("n_ceil_coeff", C.c_double)]
 
 # Index(chr_names=...): the reference names of --remove-chrname / --add-chrname (ht2gpu_options_t.chr_names)
 CHR_NAMES = {None: 0, "remove": 1, "add": 2}
+# Index(pe_orient=...): --fr / --rf / --ff (ht2gpu_options_t.pe_orient)
+PE_ORIENT = {None: 0, "fr": 0, "rf": 1, "ff": 2}
 # set_sam_output(rna_strandness=...): --rna-strandness, numbered as ht2gpu_sam_output_t.rna_strandness
 RNA_STRANDNESS = {None: 0, "F": 1, "R": 2, "FR": 3, "RF": 4}
 
@@ -70,7 +73,7 @@ class CReadsInput(C.Structure):
     _fields_ = [("path1", C.c_char_p), ("path2", C.c_char_p), ("data1", C.c_void_p), ("len1", C.c_size_t),
                 ("data2", C.c_void_p), ("len2", C.c_size_t), ("format", C.c_int32), ("trim5", C.c_int32), ("trim3", C.c_int32),
                 ("phred64", C.c_int32), ("seed", C.c_uint32), ("skip", C.c_uint64), ("upto", C.c_uint64),
-                ("batch_reads", C.c_uint32), ("threads", C.c_int32)]
+                ("batch_reads", C.c_uint32), ("threads", C.c_int32), ("solexa_quals", C.c_int32), ("int_quals", C.c_int32)]
 
 
 class CReadsFiles(C.Structure):
@@ -604,7 +607,8 @@ class SeedResult(object):
 
 
 def _options(lib, opts):
-    """ht2gpu_options_t: the defaults, then opts (chr_names by name, see CHR_NAMES)."""
+    """ht2gpu_options_t: the defaults, then opts (chr_names and pe_orient by name, see CHR_NAMES and PE_ORIENT;
+    n_ceil_type as a character, e.g. "L")."""
     o = Options()
     lib.ht2gpu_default_options(C.byref(o))
     for k, v in opts.items():
@@ -612,6 +616,12 @@ def _options(lib, opts):
             if v not in CHR_NAMES:
                 raise ValueError("chr_names must be 'remove', 'add' or None, not %r" % (v,))
             v = CHR_NAMES[v]
+        elif k == "pe_orient":
+            if v not in PE_ORIENT:
+                raise ValueError("pe_orient must be 'fr', 'rf', 'ff' or None, not %r" % (v,))
+            v = PE_ORIENT[v]
+        elif k == "n_ceil_type" and isinstance(v, str):
+            v = ord(v)
         setattr(o, k, v)
     return o
 
@@ -621,7 +631,8 @@ class Index(object):
 
     def __init__(self, base=None, image=None, device_image=None, device=0, **opts):
         """opts: the fields of ht2gpu_options_t; chr_names is "remove" (--remove-chrname), "add" (--add-chrname) or
-        None (the index's names)."""
+        None (the index's names); pe_orient is "fr" (default), "rf" or "ff"; n_ceil_type / n_ceil_const /
+        n_ceil_coeff are --n-ceil (type "C", "L", "S" or "G"; 0 = the default L,0,0.15)."""
         self._lib = load_library()
         self._opts = dict(opts)
         o = _options(self._lib, opts)

@@ -75,12 +75,12 @@ static void usage() {
     fprintf(stderr, "hisat2-b200 -x <index> {-U <r> | -1 <m1> -2 <m2> [-U <r>]} [-S out.sam] [-f|-q] --no-spliced-alignment [-k N]\n"
                     "            [--mp MX,MN] [--sp MX,MN] [--np N] [--rdg C,L] [--rfg C,L] [--ignore-quals] [--nofw] [--norc]\n"
                     "            [-I N] [-X N] [--no-mixed] [--no-discordant] [--seed N] [--batch N] [--device N] [--gpus N] [-p N]\n"
-                    "            [-5 N] [-3 N] [-s N] [-u N] [--phred33|--phred64] [--no-temp-splicesite]\n"
+                    "            [-5 N] [-3 N] [-s N] [-u N] [--phred33|--phred64|--solexa-quals] [--int-quals] [--no-temp-splicesite]\n"
                     "            [--known-splicesite-infile F] [--novel-splicesite-infile F] [--novel-splicesite-outfile F]\n"
                     "            [--bowtie2-dp 0|1|2] [--score-min F,C,L] [--gbar N] [--sensitive] [--very-sensitive] [--fast]\n"
                     "            [--no-unal] [--omit-sec-seq] [--no-hd] [--no-sq] [--rg-id ID] [--rg TEXT]...\n"
                     "            [--rna-strandness F|R|FR|RF] [--remove-chrname|--add-chrname] [--no-templatelen-adjustment]\n"
-                    "            [--sam-no-qname-trunc]\n"
+                    "            [--sam-no-qname-trunc] [--fr|--rf|--ff] [--n-ceil F,C,L] [--no-softclip] [--ma N (ignored)]\n"
                     "            [--summary-file F] [--new-summary] [--quiet]\n"
                     "            [--un P] [--al P] [--un-conc P] [--al-conc P] [--al-conc-disc P], each also as --<opt>-gz\n"
                     "            and --<opt>-bz2: write unpaired reads that did not / did align, pairs that did not / did align\n"
@@ -91,6 +91,38 @@ static void usage() {
                     "  are one stream of pairs, the -U files one stream of unpaired reads, aligned after the pairs\n");
 }
 static void two(const char* a, int32_t& x, int32_t& y) { sscanf(a, "%d,%d", &x, &y); }
+// tokenize() (tokenize.h:33-51): a leading empty token is kept, later runs of the delimiter are one
+static std::vector<std::string> refTokens(const std::string& v, char delim)
+{
+    std::vector<std::string> t;
+    for (size_t p = 0, c = v.find(delim); c != std::string::npos || p != std::string::npos;) {
+        t.push_back(v.substr(p, c == std::string::npos ? std::string::npos : c - p));
+        p = v.find_first_not_of(delim, c);
+        c = p == std::string::npos ? p : v.find(delim, p);
+    }
+    return t;
+}
+// --n-ceil: one token is C,<x>, two are <type>,<const>, three <type>,<const>,<coeff> (hisat2.cpp:1525-1550, PARSE_FUNC
+// aligner_seed_policy.cpp:47-62).  Tokens left out keep the default L,0,0.15.  Returns false after printing the
+// reference's error.  A later --n-ceil overrides only the tokens it gives, as the reference appends each to its policy.
+static bool nCeil(const std::string& v, ht2gpu_options_t& o)
+{
+    if (o.n_ceil_type == 0) { o.n_ceil_const = (double)0.0f; o.n_ceil_coeff = (double)0.15f; }
+    std::vector<std::string> t = refTokens(v, ',');
+    if (t.size() > 3) { fprintf(stderr, "Error: expected 3 or fewer comma-separated arguments to --n-ceil option, got %zu\n", t.size()); return false; }
+    if (t.empty()) { fprintf(stderr, "Error: expected at least one argument to --n-ceil option\n"); return false; }
+    if (t.size() == 1) { t.insert(t.begin(), "C"); if (t[1].empty()) t.pop_back(); }   // "C,<x>", tokenized once more
+    const std::string& ty = t[0];
+    if (ty == "C" || ty == "Constant") o.n_ceil_type = 'C'; else if (ty == "L" || ty == "Linear") o.n_ceil_type = 'L';
+    else if (ty == "S" || ty == "Sqrt") o.n_ceil_type = 'S'; else if (ty == "G" || ty == "Log") o.n_ceil_type = 'G';
+    else {
+        fprintf(stderr, "Error: Bad function type '%s'.  Should be C (constant), L (linear), S (square root) or G (natural log).\n", ty.c_str());
+        return false;
+    }
+    if (t.size() > 1) o.n_ceil_const = atof(t[1].c_str());
+    if (t.size() > 2) o.n_ceil_coeff = atof(t[2].c_str());
+    return true;
+}
 // -U / -1 / -2 a,b,c: appended to the list, empty names dropped (tokenize, hisat2.cpp:1120-1121, 1621-1626)
 static void addFiles(std::vector<std::string>& v, const char* arg)
 {
@@ -110,7 +142,7 @@ int main(int argc, char** argv)
     const char *idx = NULL, *out = NULL;
     std::vector<std::string> us, m1s, m2s;   // -U, -1, -2
     bool fastq = true; size_t batchSz = 0 /* library default */; uint32_t gseed = 0;
-    int trim5 = 0, trim3 = 0, threads = 0, gpus = 1; bool phred64 = false; uint64_t skip = 0, upto = 0;
+    int trim5 = 0, trim3 = 0, threads = 0, gpus = 1; bool phred64 = false, solexa = false, intQuals = false; uint64_t skip = 0, upto = 0;
     bool sensitive = false, verySensitive = false, fast = false, noTempSpliceSite = false;
     const char *knownSs = NULL, *novelSs = NULL, *novelOut = NULL;   // --known-splicesite-infile / --novel-splicesite-infile (hisat2.cpp:1689-1691)
     // SAM output (hisat2.cpp:601-623, 1342-1343, 1389-1407): --no-hd prints no header at all (no @PG either,
@@ -120,6 +152,7 @@ int main(int argc, char** argv)
     std::string rgId; std::vector<std::string> rgFields;
     const char* summaryFile = NULL;
     ReadFiles rfs;
+    int maBonus = 0;   // --ma: the last one counts (MA=, aligner_seed_policy.cpp:363-373)
     bool mpGiven = false;   // "--mp a,b" becomes MMP=Q,a,b, which switches the cost model back to quality-aware even
                             // under --ignore-quals (aligner_seed_policy.cpp:396-418)
     for (int i = 1; i < argc; i++) {
@@ -155,7 +188,7 @@ int main(int argc, char** argv)
         else if (a == "-p" || a == "--threads") threads = atoi(next());   // host parser threads; the alignment itself runs on the GPU
         else if (a == "-5" || a == "--trim5") trim5 = atoi(next()); else if (a == "-3" || a == "--trim3") trim3 = atoi(next());
         else if (a == "-s" || a == "--skip") skip = (uint64_t)atoll(next()); else if (a == "-u" || a == "--upto" || a == "--qupto") upto = (uint64_t)atoll(next());
-        else if (a == "--phred64" || a == "--phred64-quals" || a == "--solexa1.3-quals") phred64 = true; else if (a == "--phred33" || a == "--phred33-quals") phred64 = false;
+        else if (a == "--phred64" || a == "--phred64-quals" || a == "--solexa1.3-quals") phred64 = true; else if (a == "--phred33" || a == "--phred33-quals") phred64 = solexa = false;
         else if (a == "--no-unal") noUnal = 1;
         else if (a == "--omit-sec-seq" || a == "--sam-omit-sec-seq") omitSecSeq = 1;
         else if (a == "--no-hd" || a == "--no-head" || a == "--no-HD" || a == "--sam-no-hd" || a == "--sam-no-head" || a == "--sam-nohead" || a == "--sam-noHD") noHd = true;
@@ -179,7 +212,17 @@ int main(int argc, char** argv)
                          for (int c = 0; c < 3; c++)
                              if (a == std::string("--") + kReadOpt[w] + (c == 1 ? "-gz" : c == 2 ? "-bz2" : "")) { rfs.spec[w] = next(); rfs.compress[w] = c; return true; }
                      return false; }()) {}
-        else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--fr" || a == "--no-unal-ignored") {}
+        else if (a == "--fr") o.pe_orient = HT2GPU_PE_FR; else if (a == "--rf") o.pe_orient = HT2GPU_PE_RF; else if (a == "--ff") o.pe_orient = HT2GPU_PE_FF;
+        else if (a == "--n-ceil") { if (!nCeil(next(), o)) return 1; }
+        else if (a == "--ma") {   // the match bonus is always 0 in end-to-end mode: warned about below, then ignored
+            const std::string v = next();
+            if (refTokens(v, ',').size() != 1) { fprintf(stderr, "Error parsing alignment policy setting MA=%s; RHS must have 1 token\n", v.c_str()); return 1; }
+            maBonus = atoi(v.c_str());
+        }
+        else if (a == "--no-softclip") { o.sp_max = o.sp_min = 2147483647; }   // SCP=Q,INT_MAX,INT_MAX, in order with --sp (hisat2.cpp:1588-1596)
+        else if (a == "--solexa-quals") solexa = true;
+        else if (a == "--int-quals" || a == "--integer-quals") intQuals = true;
+        else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--no-unal-ignored") {}
         else if (a == "-h" || a == "--help") { usage(); return 0; }
         else { fprintf(stderr, "Error: option %s is not supported by hisat2-b200\n", a.c_str()); return 1; }
     }
@@ -199,6 +242,7 @@ int main(int argc, char** argv)
         fprintf(stderr, "Warning: temporary splice sites (the reference's default) make results depend on the order reads are processed in;\n"
                         "         hisat2-b200 aligns every read independently, i.e. as with --no-temp-splicesite\n");
     if (mpGiven) o.ignore_quals = 0;
+    if (maBonus > 0) fprintf(stderr, "Warning: Match bonus always = 0 in --end-to-end mode; ignoring user setting\n");   // hisat2.cpp:3916-3919
     // presets, spelled out the way hisat2.cpp:1889-1909 applies them after option parsing
     if (fast) {}
     else if (sensitive) {
@@ -247,6 +291,7 @@ int main(int argc, char** argv)
     lists.paths1 = p1.data(); lists.n1 = (uint32_t)p1.size(); lists.paths2 = p2.data(); lists.n2 = (uint32_t)p2.size();
     lists.paths_u = pu.data(); lists.n_u = (uint32_t)pu.size();
     in.format = fastq ? 1 : 0; in.trim5 = trim5; in.trim3 = trim3; in.phred64 = phred64 ? 1 : 0; in.seed = gseed;
+    in.solexa_quals = solexa ? 1 : 0; in.int_quals = intQuals ? 1 : 0;
     in.skip = skip; in.upto = upto; in.batch_reads = (uint32_t)batchSz; in.threads = threads;
     ht2gpu_read_routes_t routes; memset(&routes, 0, sizeof(routes));
     routes.mask = rfs.mask(); routes.ctx = &rfs;

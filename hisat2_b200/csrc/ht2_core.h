@@ -86,6 +86,12 @@ struct Ht2Edit {          // edit.h:41-330
     uint8_t  pad;
     uint32_t snpID;
 };
+// The N ceiling of a read length from Ht2Params::nCeilTab.  NULL is the default L,0,0.15 (for host callers that give
+// no table).  The read filter compares it as unsigned: SimpleFunc::f<size_t> is huge wherever f<int> is INT_MIN.
+HT2_HD int32_t ht2_nceil(const int32_t* tab, uint32_t len) {
+    if (!tab) return (int32_t)((double)0.0f + (double)0.15f * (double)len);
+    return tab[len <= HT2_PARAMS_MAX_RDLEN ? len : HT2_PARAMS_MAX_RDLEN];
+}
 // HT2_SPL_* direction codes: ht2_ssdb.h (splice_site.h:37-43)
 // A splice edit (type HT2_EDIT_SPL; spliced alignment, host test build only for now, DESIGN.md 8.2) keeps the
 // same 12 bytes: intron length (20 bits) in chr | qchr << 8 | (pad & 15) << 16, direction in pad bits 4-6,
@@ -338,12 +344,16 @@ HT2_HD int ht2_score(const Ht2ParamsCore& P, int rdc, int refm, int q) {
     if ((refm & (1 << rdc)) != 0) return 0;
     return -ht2_mmpen(P, q);
 }
-// Scoring::sc(q) soft-clip penalty (scoring.h:312-318)
+// float to int as x86-64's cvttss2si converts it: values outside int's range (and NaN) give INT_MIN.  The device's
+// cvt.rzi.s32.f32 would saturate them instead, so both builds take this step.
+HT2_HD int ht2_f2i_x86(float f) { return f >= -2147483648.0f && f < 2147483648.0f ? (int)f : (int)0x80000000u; }
+// Scoring::sc(q) soft-clip penalty (scoring.h:312-318).  --no-softclip (--sp INT_MAX,INT_MAX) makes the float
+// 2^31, which converts to INT_MIN in the reference; sc(0) returns scpMin itself.
 HT2_HD int ht2_scpen(const Ht2ParamsCore& P, int q) {
     if (q <= 33) return P.scpMin;
     q -= 33;
     if (q > 40) q = 40;
-    return (int)(((float)q / 40.0f) * (float)(P.scpMax - P.scpMin) + (float)P.scpMin);
+    return ht2_f2i_x86(((float)q / 40.0f) * (float)(P.scpMax - P.scpMin) + (float)P.scpMin);
 }
 HT2_HD int ht2_asc2code(uint8_t ch) { // dna2col[ch]-'0'
     switch (ch) { case 'A': return 0; case 'C': return 1; case 'G': return 2; case 'T': return 3; default: return 4; }
@@ -505,6 +515,7 @@ struct Ht2AlignerT {
     uint32_t              swStride;
     uint32_t              swStage; // 0, or set by the pool kernel's DP round: 1 = problem framed and filled by the warp, 2 = nothing to fill (answer in swRetv)
     bool                  swRetv;
+    const int32_t*        nCeilTab; // --n-ceil per read length for the DP (Ht2Params::nCeilTab); NULL = the default
 #ifdef HT2_ENABLE_SPLICED
     const Ht2SplTables*   splT;    // donor / acceptor probability tables (spliced mode)
     const uint8_t*        ssT;     // read-only splice-site DB of the run (ht2_ssdb.h), NULL = empty (SpliceSiteDB::empty())
@@ -532,10 +543,15 @@ struct Ht2AlignerT {
         gfm.init(blob_, &H->global);
         P = P_;
         W = W_;
-        sw = NULL; swPl = NULL; swStride = 1; swStage = 0; swRetv = false;
+        sw = NULL; swPl = NULL; swStride = 1; swStage = 0; swRetv = false; nCeilTab = NULL;
 #ifdef HT2_ENABLE_SPLICED
         splT = NULL; ssT = NULL;
 #endif
+    }
+    // host builds hold the whole parameter set, tables included
+    HT2_HD void bind(const uint8_t* blob_, const Ht2Params* P_, Ht2Work* W_) {
+        bind(blob_, static_cast<const Ht2ParamsCore*>(P_), W_);
+        nCeilTab = P_->nCeilTab;
     }
 
     // ---- edits / hits ---------------------------------------------------

@@ -38,7 +38,7 @@ struct DevBatch {
     int32_t         paired;
     Ht2SwScratch*   sw;     // --bowtie2-dp scratch, one per launched thread (NULL when dp is off)
     uint32_t*       swPool; // ... and the H / E / F plane pool: HT2_SW_POOL_WORDS words per thread, interleaved per warp
-    const int32_t*  minscTab; // --score-min per read length (Ht2Params::minscTab)
+    const int32_t*  minscTab; // --score-min per read length, then --n-ceil from HT2_PARAMS_NCEIL on (Ht2Params)
     uint32_t        elect;    // a warp stays on the block's current target state while it has at least this many claimable slots
 #ifdef HT2_ENABLE_SPLICED
     const Ht2SplTables* splT; // donor / acceptor probability tables (spliced mode)
@@ -114,10 +114,9 @@ __device__ __noinline__ void ht2_load_read(Ht2Read& dst, const DevBatch& b, uint
 }
 
 // Per-read filters and minimum score (hisat2.cpp:3387-3440): length filter,
-// N filter (Scoring::nFilter, nCeil = L,0,0.15 -- the parseString default, aligner_seed_policy.cpp:293-296), score filter
-// (minsc = --score-min(len), default L,0,-0.2, clamped to <= 0 -- hisat2.cpp:441, 3380-3402; the
-// function is tabulated per read length on the host, Ht2Params::minscTab).  The N-ceiling product is
-// exact in double (24-bit constant x length < 2^9), so host (ht2_host.cpp:ht2_filters) and device agree.
+// N filter (Scoring::nFilter, --n-ceil, default L,0,0.15), score filter (minsc = --score-min(len), default L,0,-0.2,
+// clamped to <= 0 -- hisat2.cpp:441, 3380-3402).  Both functions are tabulated per read length on the host
+// (Ht2Params::minscTab, nCeilTab: one buffer), so host (ht2_host.cpp:ht2_filters) and device agree for every function type.
 __device__ __forceinline__ bool ht2_dev_filter(const DevBatch& b, uint32_t ri, int64_t& minsc)
 {
     const uint64_t o0 = b.offs[ri];
@@ -125,7 +124,7 @@ __device__ __forceinline__ bool ht2_dev_filter(const DevBatch& b, uint32_t ri, i
     int64_t m = b.minscTab[len <= HT2_PARAMS_MAX_RDLEN ? len : HT2_PARAMS_MAX_RDLEN];   // --score-min, tabulated on the host (ht2_set_score_min)
     if (m > 0) m = 0;
     minsc = m;
-    const uint32_t maxns = (uint32_t)((double)0.0f + (double)0.15f * (double)len);   // nCeil = L,0,0.15 (aligner_seed_policy.cpp:293-296)
+    const uint32_t maxns = (uint32_t)ht2_nceil(b.minscTab + HT2_PARAMS_NCEIL, len);
     const uint8_t* s = b.seq + o0;
     uint32_t ns = 0;
     for (uint32_t k = 0; k < len; k += 4) {
@@ -337,6 +336,7 @@ ht2_align_pool_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatc
     A.sw = b.sw ? b.sw + ((size_t)blockIdx.x * blockDim.x + threadIdx.x) : NULL;
     A.swPl = b.swPool ? b.swPool + ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * (size_t)HT2_SW_POOL_WORDS : NULL;
     A.swStride = 1;
+    A.nCeilTab = b.minscTab + HT2_PARAMS_NCEIL;
 #ifdef HT2_ENABLE_SPLICED
     A.splT = b.splT; A.ssT = b.ssT;
 #endif
@@ -757,7 +757,7 @@ struct ht2gpu_handle {
     bool           graph = false;
     int            poolWarps = 0;
     int            rgK = 0;
-    DevBuf<int32_t> dMinsc;  // --score-min table on the device (Ht2Params::minscTab)
+    DevBuf<int32_t> dMinsc;  // --score-min and --n-ceil tables on the device (Ht2Params::minscTab, nCeilTab)
     DevBuf<uint8_t> dSplT;   // spliced mode: Ht2SplTables on the device
     DevBuf<uint8_t> dSsT;    // the run's splice-site DB on the device (ht2gpu_load_splicesites) or NULL
     bool           collectSs = false; // --novel-splicesite-outfile: collect the junctions of printed alignments
@@ -842,6 +842,10 @@ static void applyOptions(Ht2Params& P, const Ht2Image& img, const ht2gpu_options
     P.mixed = o.no_mixed ? 0 : 1; P.discord = o.no_discordant ? 0 : 1;
     P.bowtie2Dp = (uint32_t)o.bowtie2_dp; P.gapbar = o.gbar < 1 ? 1 : o.gbar;   // hisat2.cpp:1969-1973
     if (o.score_min_type != 0) ht2_set_score_min(P, (char)o.score_min_type, o.score_min_const, o.score_min_coeff);
+    if (o.n_ceil_type != 0) ht2_set_n_ceil(P, (char)o.n_ceil_type, o.n_ceil_const, o.n_ceil_coeff);
+    // hisat2.cpp:1166-1168 and 3227-3236: the mates' strands, and the pair policy they give (0 FF, 2 FR, 3 RF)
+    P.gMate1fw = o.pe_orient != HT2GPU_PE_RF; P.gMate2fw = o.pe_orient != HT2GPU_PE_FR;
+    P.pePolicy = o.pe_orient == HT2GPU_PE_FF ? 0 : o.pe_orient == HT2GPU_PE_RF ? 3 : 2;
 }
 
 // ---- ht2gpu_open*: the steps after the host image and the device blob have arrived -------------------------------
@@ -867,7 +871,7 @@ static int loadNamesAndParams(ht2gpu_handle* h)
     h->refNames.build(*h->img, h->opt.chr_names);
     CK(h->dRefNames.upload(h->refNames.blob.data(), h->refNames.blob.size()));
     applyOptions(h->P, *h->img, h->opt);
-    CK(h->dMinsc.upload(h->P.minscTab, sizeof(h->P.minscTab) / sizeof(h->P.minscTab[0])));
+    CK(h->dMinsc.upload(h->P.minscTab, 2 * HT2_PARAMS_NCEIL));   // nCeilTab follows minscTab (ht2_params.h)
     return HT2GPU_OK;
 }
 
@@ -975,6 +979,9 @@ static int startOpen(ht2gpu_handle* h)
     const int32_t cn = h->opt.chr_names;
     if (cn == (HT2GPU_CHR_NAMES_REMOVE | HT2GPU_CHR_NAMES_ADD)) { h->err = "--remove-chrname and --add-chrname cannot be used at the same time"; return HT2GPU_ERR_ARG; }
     if (cn != HT2GPU_CHR_NAMES_INDEX && cn != HT2GPU_CHR_NAMES_REMOVE && cn != HT2GPU_CHR_NAMES_ADD) { h->err = "chr_names must be 0, 1 (remove) or 2 (add)"; return HT2GPU_ERR_ARG; }
+    const int32_t pe = h->opt.pe_orient, nt = h->opt.n_ceil_type;
+    if (pe != HT2GPU_PE_FR && pe != HT2GPU_PE_RF && pe != HT2GPU_PE_FF) { h->err = "pe_orient must be 0 (--fr), 1 (--rf) or 2 (--ff)"; return HT2GPU_ERR_ARG; }
+    if (nt != 0 && nt != 'C' && nt != 'L' && nt != 'S' && nt != 'G') { h->err = "n_ceil_type must be 0 (default), 'C', 'L', 'S' or 'G'"; return HT2GPU_ERR_ARG; }
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n <= 0) {
@@ -1050,7 +1057,9 @@ extern "C" int ht2gpu_open_peer(const ht2gpu_handle_t* src, const ht2gpu_options
 {
     if (!src || !out || !src->dBlob || !src->img) return HT2GPU_ERR_ARG;
     ht2gpu_options_t o = opt ? *opt : src->opt;
-    o.chr_names = src->opt.chr_names;   // one run prints one set of names
+    o.chr_names = src->opt.chr_names;   // one run prints one set of names ...
+    o.pe_orient = src->opt.pe_orient;   // ... and filters and pairs the reads one way
+    o.n_ceil_type = src->opt.n_ceil_type; o.n_ceil_const = src->opt.n_ceil_const; o.n_ceil_coeff = src->opt.n_ceil_coeff;
     return openHandle(&o, out, [&](ht2gpu_handle* h) -> int {
         h->img.reset(new Ht2Image());
         h->img->blob = src->img->blob;            // host copy: reference names / lengths for SAM
@@ -1651,12 +1660,12 @@ extern "C" int ht2gpu_sw_selftest(int device, uint32_t n, uint32_t seed, uint64_
 __global__ void __launch_bounds__(32)
 ht2_sw_extend_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, const ht2gpu_sw_job_t* jobs, const uint8_t* seq,
                      const uint8_t* qual, uint32_t n, Ht2Work* work, Ht2SwScratch* scr, uint32_t* pools, int warpFill,
-                     ht2gpu_sw_result_t* res, ht2gpu_edit_t* edits)
+                     ht2gpu_sw_result_t* res, ht2gpu_edit_t* edits, const int32_t* nCeilTab)
 {
     const uint32_t lane = threadIdx.x, j = blockIdx.x * 32 + lane;
     Ht2AlignerT<false, true> A;
     A.bind(blob, &P, NULL);
-    A.sw = scr + j; A.swPl = pools + (size_t)j * HT2_SW_POOL_WORDS; A.swStride = 1;
+    A.sw = scr + j; A.swPl = pools + (size_t)j * HT2_SW_POOL_WORDS; A.swStride = 1; A.nCeilTab = nCeilTab;
     Ht2Work* W = NULL;
     if (j < n) {
         const ht2gpu_sw_job_t& q = jobs[j];
@@ -1728,7 +1737,7 @@ extern "C" int ht2gpu_sw_extend(ht2gpu_handle_t* h, uint32_t n, const ht2gpu_sw_
     size_t lim = 0;
     CK(cudaDeviceGetLimit(&lim, cudaLimitStackSize));
     if (lim < 8192) CK(cudaDeviceSetLimit(cudaLimitStackSize, 8192));
-    ht2_sw_extend_kernel<<<nt / 32, 32>>>(h->dBlob, h->P, dJobs, dSeq, dQual, n, dWork, dScr, dPool, warp_fill, dRes, dEd);
+    ht2_sw_extend_kernel<<<nt / 32, 32>>>(h->dBlob, h->P, dJobs, dSeq, dQual, n, dWork, dScr, dPool, warp_fill, dRes, dEd, h->dMinsc + HT2_PARAMS_NCEIL);
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(res, dRes, sizeof(ht2gpu_sw_result_t) * n, cudaMemcpyDeviceToHost));
@@ -1953,9 +1962,13 @@ extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output
     return HT2GPU_OK;
 }
 
-// The output settings and reference names of two handles are the same (ht2gpu_run_reads_multi: one run prints one
-// kind of record)
-bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b) { return a->samOut == b->samOut && a->opt.chr_names == b->opt.chr_names; }
+// The output settings, reference names, mate orientation and N ceiling of two handles are the same
+// (ht2gpu_run_reads_multi: one run filters, pairs and prints every read one way)
+bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b)
+{
+    return a->samOut == b->samOut && a->opt.chr_names == b->opt.chr_names && a->P.pePolicy == b->P.pePolicy &&
+           memcmp(a->P.nCeilTab, b->P.nCeilTab, sizeof(a->P.nCeilTab)) == 0;
+}
 int ht2_handle_device(const ht2gpu_handle_t* h) { return h->device; }
 
 extern "C" int ht2gpu_align_counts(ht2gpu_handle_t** hs, int n, int reset, ht2gpu_align_counts_t* out)

@@ -51,6 +51,9 @@ void ht2_default_params(Ht2Params& P, const Ht2Image& img, bool noSplicedAlignme
     P.noncanSplPen = 12;                                // hisat2.cpp:494
 #endif
     ht2_set_score_min(P, 'L', (double)0.0f, (double)-0.2f);   // hisat2.cpp:441
+    // hisat2.cpp:443 initialises 2 + 0.1 len, but SeedAlignmentPolicy::parseString -- always called, hisat2.cpp:1849 --
+    // resets it to DEFAULT_N_CEIL_CONST / LINEAR = 0.0 / 0.15 (aligner_seed_policy.cpp:293-296, scoring.h:65-67)
+    ht2_set_n_ceil(P, 'L', (double)0.0f, (double)0.15f);
 }
 
 // SimpleFunc::f<TAlScore> (simple_func.h:86-108) with min = -DBL_MAX, max = DBL_MAX
@@ -70,9 +73,19 @@ bool ht2_set_score_min(Ht2Params& P, char type, double C, double L)
     return true;
 }
 
-// SimpleFunc::f<T> for the linear functions the defaults use (simple_func.h:86-108)
-static double simpleLinear(double I, double X, double C, double L, double x) {
-    return std::max(I, std::min(X, C + L * x));
+// SimpleFunc::f<int> (simple_func.h:86-108) with min = 0 and max = DBL_MAX, as the reference's nCeil.  The value is
+// converted as x86-64 does: DBL_MAX gives INT_MAX, anything else at or above 2^31 gives INT_MIN.
+bool ht2_set_n_ceil(Ht2Params& P, char type, double C, double L)
+{
+    if (type != 'C' && type != 'L' && type != 'S' && type != 'G') return false;
+    const double dmax = 1.7976931348623157e308;
+    for (uint32_t len = 0; len <= HT2_PARAMS_MAX_RDLEN; len++) {
+        double x = (double)len, X;
+        if (type == 'C') X = 0.0; else if (type == 'L') X = x; else if (type == 'S') X = sqrt(x); else X = log(x);
+        const double v = std::max(0.0, std::min(dmax, C + L * X));
+        P.nCeilTab[len] = v == dmax ? 2147483647 : v >= 2147483648.0 ? (int32_t)0x80000000u : (int32_t)v;
+    }
+    return true;
 }
 
 int64_t ht2_minsc(const Ht2Params& P, uint32_t rdlen)
@@ -83,14 +96,12 @@ int64_t ht2_minsc(const Ht2Params& P, uint32_t rdlen)
     return m;
 }
 
-Ht2ReadFilters ht2_filters(const Ht2HostRead& rd, int64_t minsc)
+Ht2ReadFilters ht2_filters(const Ht2HostRead& rd, int64_t minsc, const int32_t* nCeilTab)
 {
     Ht2ReadFilters f;
     size_t rdlen = rd.seq.size();
-    // Scoring::nFilter (scoring.cpp:104-117).  The effective default is nCeil = L,0,0.15: hisat2.cpp:443
-    // initialises 2 + 0.1 len, but SeedAlignmentPolicy::parseString -- always called, hisat2.cpp:1849 --
-    // resets it to DEFAULT_N_CEIL_CONST/LINEAR = 0.0 / 0.15 (aligner_seed_policy.cpp:293-296, scoring.h:65-67).
-    size_t maxns = (size_t)simpleLinear(0.0, 1.7976931348623157e308, (double)0.0f, (double)0.15f, (double)rdlen);
+    // Scoring::nFilter (scoring.cpp:104-117)
+    const size_t maxns = (uint32_t)ht2_nceil(nCeilTab, (uint32_t)rdlen);
     size_t ns = 0;
     f.nfilt = true;
     for (size_t i = 0; i < rdlen; i++) {

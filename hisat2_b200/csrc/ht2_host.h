@@ -35,7 +35,10 @@ void ht2_default_params(Ht2Params& P, const Ht2Image& img, bool noSplicedAlignme
 int64_t ht2_minsc(const Ht2Params& P, uint32_t rdlen);
 // --score-min <type>,<const>,<coeff>: type one of C, L, S, G (simple_func.h)
 bool ht2_set_score_min(Ht2Params& P, char type, double C, double L);
-Ht2ReadFilters ht2_filters(const Ht2HostRead& rd, int64_t minsc);
+// --n-ceil <type>,<const>,<coeff> into P.nCeilTab; type one of C, L, S, G
+bool ht2_set_n_ceil(Ht2Params& P, char type, double C, double L);
+// nCeilTab: Ht2Params::nCeilTab; NULL = the default N ceiling
+Ht2ReadFilters ht2_filters(const Ht2HostRead& rd, int64_t minsc, const int32_t* nCeilTab = NULL);
 uint32_t ht2_gen_rand_seed(const Ht2HostRead& rd, uint32_t seed);
 void ht2_fill_read(Ht2Read& dst, const Ht2HostRead& src);
 

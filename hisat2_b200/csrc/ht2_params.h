@@ -68,6 +68,14 @@ struct Ht2Params : Ht2ParamsCore {
     // simple_func.h:86-108), computed once on the host so that host and device agree for every
     // function type (C, L, S = sqrt, G = log).  NOT yet clamped to <= 0.
     int32_t  minscTab[HT2_PARAMS_MAX_RDLEN + 1];
+    // --n-ceil as a table, SimpleFunc::f<int>(len) with min 0 and max DBL_MAX (aligner_seed_policy.cpp:293-296, 547-549;
+    // default L,0,0.15): the most Ns a read of that length may hold (Scoring::nFilter) and the DP's N ceiling
+    // (SwAligner::initRead).  Read lengths above the table take its last entry.  It directly follows minscTab, and the
+    // two travel as one buffer: the device's (DevBatch::minscTab) and the formatter's (Ht2SamIn::minscTab) hold the
+    // N ceilings from HT2_PARAMS_NCEIL on, so no kernel parameter grows.
+    int32_t  nCeilTab[HT2_PARAMS_MAX_RDLEN + 1];
 };
+#define HT2_PARAMS_NCEIL (HT2_PARAMS_MAX_RDLEN + 1)
+static_assert(sizeof(Ht2Params) == sizeof(Ht2ParamsCore) + 2 * sizeof(int32_t) * HT2_PARAMS_NCEIL, "minscTab and nCeilTab must be adjacent");
 
 #endif

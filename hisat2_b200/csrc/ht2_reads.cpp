@@ -2,6 +2,7 @@
 #include "ht2_reads.h"
 
 #include <fcntl.h>
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -223,6 +224,14 @@ void Ht2HostBatch::freeAll()
 
 namespace {
 
+// solexaToPhred (qual.h:46-50): Solexa -10 .. 255 to Phred, round(10 log10(10^(sol/10) + 1)); below -10 is 0
+struct SolexaTable {
+    uint8_t phred[266];
+    SolexaTable() { for (int s = -10; s <= 255; s++) phred[s + 10] = (uint8_t)(10.0 * log10(pow(10.0, s / 10.0) + 1.0) + 0.5); }
+    int operator()(int sol) const { return sol < -10 ? 0 : phred[(sol > 255 ? 255 : sol) + 10]; }
+};
+static const SolexaTable kSolexa;
+
 struct Tables {
     uint8_t isBase[256];   // FASTA: asc2dnacat > 0 (alphabet.cpp)
     uint8_t isAlpha[256];  // FASTQ: letters, and '.' which reads as N (pat.cpp:1030-1290)
@@ -317,14 +326,44 @@ bool parseRecord(const Ht2ReadSource& src, uint64_t r, uint64_t rdid, int mate, 
         // qualities: the line's characters (minus '\r'), trimmed like the bases, converted to Phred+33
         uint8_t* ql = L.qual.p + L.qual.n;
         size_t qn = 0;
-        for (; p < e && d[p] != '\n'; p++) { const uint8_t c = (uint8_t)d[p]; ql[qn] = c; qn += (c != '\r'); }
-        const size_t qkeep = qn > (size_t)o.trim5 + t3 ? qn - (size_t)o.trim5 - t3 : 0;
-        if (qkeep != n) {
-            L.err = std::string(qkeep < n ? "fewer" : "more") + " quality values than bases for read " + std::string(nm, nl);
-            return false;
+        if (o.intQuals) {   // pat.cpp:997-1030: tokenize(line, " ") keeps a leading empty token (atoi gives 0)
+            const size_t l0 = p; while (p < e && d[p] != '\n') p++;
+            size_t l1 = p; while (l1 > l0 && d[l1 - 1] == '\r') l1--;
+            size_t nTok = 0;
+            for (size_t k = l0; l1 > l0;) {   // an empty line has no tokens
+                size_t k1 = k; while (k1 < l1 && d[k1] != ' ') k1++;
+                if (k1 > k || k == l0) {
+                    char tok[32]; size_t tl = 0;
+                    for (size_t j = k; j < k1 && tl < sizeof(tok) - 1; j++) tok[tl++] = d[j];
+                    tok[tl] = '\0';
+                    const int v = atoi(tok);   // intToPhred33 (qual.h:143-165); Solexa values above 255 read as 255
+                    const int pq = o.solexa ? kSolexa(v) + 33 : (v <= 93 ? v : 93) + 33;
+                    if (pq < 33) { L.err = "negative Phred quality " + std::to_string(pq - 33) + " in read " + std::string(nm, nl); return false; }
+                    if (nTok++ >= (size_t)o.trim5) ql[qn++] = (uint8_t)(pq <= 126 ? pq : 126);
+                }
+                if (k1 >= l1) break;
+                k = k1 + 1;
+            }
+            qn -= (size_t)o.trim3 < qn ? (size_t)o.trim3 : qn;   // trimEnd(gTrim3); one value more than bases is cut
+            if (qn < n || qn > n + 1) {
+                L.err = std::string(qn < n ? "fewer" : "more") + " quality values than bases for read " + std::string(nm, nl);
+                return false;
+            }
+        } else {
+            for (; p < e && d[p] != '\n'; p++) { const uint8_t c = (uint8_t)d[p]; ql[qn] = c; qn += (c != '\r'); }
+            const size_t qkeep = qn > (size_t)o.trim5 + t3 ? qn - (size_t)o.trim5 - t3 : 0;
+            if (qkeep != n) {
+                L.err = std::string(qkeep < n ? "fewer" : "more") + " quality values than bases for read " + std::string(nm, nl);
+                return false;
+            }
+            if (o.trim5 > 0) memmove(ql, ql + o.trim5, n);
         }
-        if (o.trim5 > 0) memmove(ql, ql + o.trim5, n);
-        if (o.phred64) {
+        if (o.solexa && !o.intQuals) {   // charToPhred33 (qual.h:106-141): the character is a signed char
+            for (size_t i = 0; i < n; i++) {
+                if (ql[i] == ' ') { L.err = "space in the quality values of read " + std::string(nm, nl) + "; integer qualities need --int-quals"; return false; }
+                ql[i] = (uint8_t)(kSolexa((int)(int8_t)ql[i] - 64) + 33);
+            }
+        } else if (o.phred64 && !o.intQuals) {
             for (size_t i = 0; i < n; i++) { if (ql[i] < 64) { L.err = "quality value below Phred+64 range in read " + std::string(nm, nl); return false; } ql[i] = (uint8_t)(ql[i] - 31); }
         }
         uint8_t lo = 255;

@@ -82,8 +82,10 @@ struct Ht2ReadsOpts {
     bool     fastq;
     int      trim5, trim3;      // -5 / -3
     bool     phred64;           // --phred64
+    bool     solexa;            // --solexa-quals (wins over phred64, as charToPhred33 tests it first)
+    bool     intQuals;          // --int-quals: space-separated integer qualities
     uint32_t seed;              // --seed
-    Ht2ReadsOpts() : fastq(false), trim5(0), trim3(0), phred64(false), seed(0) {}
+    Ht2ReadsOpts() : fastq(false), trim5(0), trim3(0), phred64(false), solexa(false), intQuals(false), seed(0) {}
 };
 
 // Host staging of one batch.  Buffers come from alloc / release (pinned memory when the CUDA side provides them).

@@ -27,7 +27,7 @@
 struct Ht2SamIn {
     const uint8_t*  blob;        // index image (ALT table + names)
     const uint8_t*  refNames;    // the handle's reference names (Ht2RefNames::blob, ht2_index.h): RNAME, RNEXT
-    const int32_t*  minscTab;    // --score-min per read length (Ht2Params::minscTab)
+    const int32_t*  minscTab;    // --score-min per read length, then --n-ceil from HT2_PARAMS_NCEIL on (Ht2Params)
     const uint8_t*  seq;         // read batch (ht2gpu_read_batch_t)
     const uint8_t*  qual;        // NULL = all 'I'
     const uint64_t* offs;
@@ -257,9 +257,9 @@ struct Ht2SamFmt {
         rd.len = (uint32_t)(in->offs[i + 1] - o0);
         rd.name = in->names + in->nameOffs[i];
         rd.mate = mate;
-        // ht2_filters (hisat2.cpp:3417-3440; Scoring::nFilter with nCeil = L,0,0.15)
+        // ht2_filters (hisat2.cpp:3417-3440; Scoring::nFilter)
         int64_t m = minscOf(rd.len); if (m > 0) m = 0;
-        const uint32_t maxns = (uint32_t)((double)0.0f + (double)0.15f * (double)rd.len);
+        const uint32_t maxns = (uint32_t)ht2_nceil(in->minscTab + HT2_PARAMS_NCEIL, rd.len);
         uint32_t ns = 0;
 #ifdef __CUDA_ARCH__
         {   // base codes are 0..4, so bit 2 marks an N; aligned words, bytes outside the read masked off

@@ -486,8 +486,8 @@ HT2_NI bool swFinish(uint32_t rdi, Ht2Hit& gh) {
     const int64_t msc = S.jmsc;
     const SwRect rect = S.jrect;
     const bool use16 = !(msc >= -254);                    // the reference's 16-bit path (aligner_sw.cpp:496): only the RNG reseeding differs
-    // nCeil = L,0,0.15 (SwAligner::initRead, aligner_sw.cpp:45)
-    const int nceil = (int)((double)0.0f + (double)0.15f * (double)rdlen);
+    // nCeil.f<int>(rdlen) (SwAligner::initRead, aligner_sw.cpp:44)
+    const int nceil = ht2_nceil(nCeilTab, rdlen);
     if (S.jbest == HT2_MIN_I64) return false;
     // SwAligner::nextAlignment: candidates in (score desc, col desc) order
     int64_t prevScore = 0; uint32_t prevCol = 0; bool havePrev = false;

@@ -81,8 +81,19 @@ typedef struct {
      * ht2gpu_open_peer takes the source handle's setting.  ht2gpu_ref_name and the ht2_* compatibility calls keep the
      * index's own names, as the reference's hisat2lib does: it has no such option. */
     int32_t  chr_names;
+    /* --fr / --rf / --ff (hisat2.cpp:1166-1168, 3227-3236): the orientations of mate 1 and mate 2 on the forward strand
+     * of a concordant pair.  HT2GPU_PE_FR (0) mate 1 forward, mate 2 reverse-complement; _RF the opposite; _FF both
+     * forward.  Any other value is HT2GPU_ERR_ARG. */
+    int32_t  pe_orient;
+    /* --n-ceil <type>,<const>,<coeff> (NCEIL, aligner_seed_policy.cpp:547-549): the most Ns a read of length x may hold
+     * (reads with more are filtered, YF:Z:NS) and the N ceiling of the --bowtie2-dp extension, as
+     * max(0, const + coeff * F(x)) with F as for score_min_type.  0 = the default L,0,0.15. */
+    int32_t  n_ceil_type;
+    double   n_ceil_const;
+    double   n_ceil_coeff;
 } ht2gpu_options_t;
 enum { HT2GPU_CHR_NAMES_INDEX = 0, HT2GPU_CHR_NAMES_REMOVE = 1, HT2GPU_CHR_NAMES_ADD = 2 };
+enum { HT2GPU_PE_FR = 0, HT2GPU_PE_RF = 1, HT2GPU_PE_FF = 2 };
 
 /* A batch of reads, structure-of-arrays, host memory.  Read i occupies
  * seq[offs[i] .. offs[i+1]).  Bases are codes 0..4 (A,C,G,T,N) exactly as
@@ -241,6 +252,11 @@ typedef struct {
     uint64_t    upto;       /* -u; 0 = no limit */
     uint32_t    batch_reads;/* reads per device batch; 0 = 4,000,000 */
     int32_t     threads;    /* host parser threads (-p); 0 = all cores, at most 64 */
+    /* --solexa-quals: FASTQ qualities are Solexa-scaled, 64-based (qual.h:46-50, 106-136); wins over phred64.
+     * --int-quals: the quality line is space-separated integers (pat.cpp:997-1030), Phred unless solexa_quals; one
+     * value more than bases is cut, fewer or more is an error.  Qualities are converted before the per-read seed. */
+    int32_t     solexa_quals;
+    int32_t     int_quals;
 } ht2gpu_reads_input_t;
 typedef struct {
     uint64_t n_reads, n_units, sam_bytes, n_err_reads, n_batches;
