@@ -27,12 +27,19 @@ class Options(C.Structure):
         ("seed", C.c_uint32), ("threads_per_block", C.c_int32), ("blocks_per_sm", C.c_int32), ("slots_per_lane", C.c_int32), ("warp_per_read", C.c_int32),
         ("bowtie2_dp", C.c_int32), ("gbar", C.c_int32), ("score_min_type", C.c_int32),
         ("score_min_const", C.c_double), ("score_min_coeff", C.c_double), ("chr_names", C.c_int32),
-        ("pe_orient", C.c_int32), ("n_ceil_type", C.c_int32), ("n_ceil_const", C.c_double), ("n_ceil_coeff", C.c_double)]
+        ("pe_orient", C.c_int32), ("n_ceil_type", C.c_int32), ("n_ceil_const", C.c_double), ("n_ceil_coeff", C.c_double),
+        ("pen_cansplice", C.c_int32), ("pen_noncansplice", C.c_int32), ("pen_conflictsplice", C.c_int32),
+        ("can_intronlen_type", C.c_int32), ("can_intronlen_const", C.c_double), ("can_intronlen_coeff", C.c_double),
+        ("noncan_intronlen_type", C.c_int32), ("noncan_intronlen_const", C.c_double), ("noncan_intronlen_coeff", C.c_double),
+        ("min_intronlen", C.c_int32), ("max_intronlen", C.c_int32), ("dta", C.c_int32), ("no_anchorstop", C.c_int32),
+        ("tmo", C.c_int32), ("avoid_pseudogene", C.c_int32)]
 
 # Index(chr_names=...): the reference names of --remove-chrname / --add-chrname (ht2gpu_options_t.chr_names)
 CHR_NAMES = {None: 0, "remove": 1, "add": 2}
 # Index(pe_orient=...): --fr / --rf / --ff (ht2gpu_options_t.pe_orient)
 PE_ORIENT = {None: 0, "fr": 0, "rf": 1, "ff": 2}
+# Index(dta=...): --dta / --dta-cufflinks (ht2gpu_options_t.dta)
+DTA = {None: 0, False: 0, True: 1, "stringtie": 1, "cufflinks": 2}
 # set_sam_output(rna_strandness=...): --rna-strandness, numbered as ht2gpu_sam_output_t.rna_strandness
 RNA_STRANDNESS = {None: 0, "F": 1, "R": 2, "FR": 3, "RF": 4}
 
@@ -620,7 +627,11 @@ def _options(lib, opts):
             if v not in PE_ORIENT:
                 raise ValueError("pe_orient must be 'fr', 'rf', 'ff' or None, not %r" % (v,))
             v = PE_ORIENT[v]
-        elif k == "n_ceil_type" and isinstance(v, str):
+        elif k == "dta":
+            if v not in DTA and v not in (0, 1, 2):
+                raise ValueError("dta must be None, True ('stringtie', --dta) or 'cufflinks' (--dta-cufflinks), not %r" % (v,))
+            v = DTA.get(v, v)
+        elif k in ("n_ceil_type", "can_intronlen_type", "noncan_intronlen_type") and isinstance(v, str):
             v = ord(v)
         setattr(o, k, v)
     return o
@@ -632,7 +643,11 @@ class Index(object):
     def __init__(self, base=None, image=None, device_image=None, device=0, **opts):
         """opts: the fields of ht2gpu_options_t; chr_names is "remove" (--remove-chrname), "add" (--add-chrname) or
         None (the index's names); pe_orient is "fr" (default), "rf" or "ff"; n_ceil_type / n_ceil_const /
-        n_ceil_coeff are --n-ceil (type "C", "L", "S" or "G"; 0 = the default L,0,0.15)."""
+        n_ceil_coeff are --n-ceil (type "C", "L", "S" or "G"; 0 = the default L,0,0.15).  Spliced alignment:
+        pen_cansplice, pen_noncansplice, pen_conflictsplice, can_intronlen_type / _const / _coeff and
+        noncan_intronlen_* (--pen-canintronlen / --pen-noncanintronlen; type as n_ceil_type, 0 = G,-8,1),
+        min_intronlen, max_intronlen, dta (True or "stringtie" = --dta, "cufflinks" = --dta-cufflinks), no_anchorstop
+        tmo (--tmo) and avoid_pseudogene (--avoid-pseudogene)."""
         self._lib = load_library()
         self._opts = dict(opts)
         o = _options(self._lib, opts)

@@ -7,6 +7,7 @@
 #include <string.h>
 #include <sys/stat.h>
 #include <sys/wait.h>
+#include <sstream>
 #include <string>
 #include <vector>
 #include "ht2gpu.h"
@@ -81,6 +82,9 @@ static void usage() {
                     "            [--no-unal] [--omit-sec-seq] [--no-hd] [--no-sq] [--rg-id ID] [--rg TEXT]...\n"
                     "            [--rna-strandness F|R|FR|RF] [--remove-chrname|--add-chrname] [--no-templatelen-adjustment]\n"
                     "            [--sam-no-qname-trunc] [--fr|--rf|--ff] [--n-ceil F,C,L] [--no-softclip] [--ma N (ignored)]\n"
+                    "            [--pen-cansplice N] [--pen-noncansplice N] [--pen-conflictsplice N] [--pen-canintronlen F,C,L]\n"
+                    "            [--pen-noncanintronlen F,C,L] [--min-intronlen N] [--max-intronlen N] [--dta|--dta-cufflinks]\n"
+                    "            [--no-anchorstop] [--tmo] [--avoid-pseudogene] [--splicesite-db-only (ignored)]\n"
                     "            [--summary-file F] [--new-summary] [--quiet]\n"
                     "            [--un P] [--al P] [--un-conc P] [--al-conc P] [--al-conc-disc P], each also as --<opt>-gz\n"
                     "            and --<opt>-bz2: write unpaired reads that did not / did align, pairs that did not / did align\n"
@@ -121,6 +125,36 @@ static bool nCeil(const std::string& v, ht2gpu_options_t& o)
     }
     if (t.size() > 1) o.n_ceil_const = atof(t[1].c_str());
     if (t.size() > 2) o.n_ceil_coeff = atof(t[2].c_str());
+    return true;
+}
+// parseInt (hisat2.cpp:1016-1039): strtol, then the bounds; a value that is no number reads as 0.  Returns false after
+// printing the reference's message.
+static bool refInt(const char* arg, int lower, const char* msg, int32_t& out)
+{
+    const long l = strtol(arg, NULL, 10);
+    if (l < lower || l > 2147483647L) { fprintf(stderr, "%s\n", msg); return false; }
+    out = (int32_t)l;
+    return true;
+}
+// --pen-canintronlen / --pen-noncanintronlen <type>[,<const>[,<coeff>]] (hisat2.cpp:1643-1680): the first three
+// tokens become CANINTRONLEN= / NONCANINTRONLEN= of the policy string, read by PARSE_FUNC (aligner_seed_policy.cpp:47-62,
+// 652-659).  Tokens left out keep the previous value, G,-8,1 at first.  An empty first token, which the reference does
+// not handle, is refused.
+static bool intronFunc(const char* opt, const std::string& v, int32_t& type, double& C, double& L)
+{
+    std::vector<std::string> t = refTokens(v, ',');
+    if (t.empty() || t[0].empty()) { fprintf(stderr, "Error: %s needs a function type as its first comma-separated token\n", opt); return false; }
+    if (type == 0) { C = -8.0; L = 1.0; }
+    const std::string& ty = t[0];
+    if (ty == "C" || ty == "Constant") type = 'C'; else if (ty == "L" || ty == "Linear") type = 'L';
+    else if (ty == "S" || ty == "Sqrt") type = 'S'; else if (ty == "G" || ty == "Log") type = 'G';
+    else {
+        fprintf(stderr, "Error: Bad function type '%s'.  Should be C (constant), L (linear), S (square root) or G (natural log).\n", ty.c_str());
+        return false;
+    }
+    auto num = [](const std::string& x) { double d = 0; std::istringstream ss(x); ss >> d; return d; };   // as PARSE_FUNC reads it
+    if (t.size() > 1) C = num(t[1]);
+    if (t.size() > 2) L = num(t[2]);
     return true;
 }
 // -U / -1 / -2 a,b,c: appended to the list, empty names dropped (tokenize, hisat2.cpp:1120-1121, 1621-1626)
@@ -222,7 +256,19 @@ int main(int argc, char** argv)
         else if (a == "--no-softclip") { o.sp_max = o.sp_min = 2147483647; }   // SCP=Q,INT_MAX,INT_MAX, in order with --sp (hisat2.cpp:1588-1596)
         else if (a == "--solexa-quals") solexa = true;
         else if (a == "--int-quals" || a == "--integer-quals") intQuals = true;
-        else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--no-unal-ignored") {}
+        else if (a == "--pen-cansplice") { if (!refInt(next(), 0, "--pen-cansplice arg must be at least 0", o.pen_cansplice)) return 1; }
+        else if (a == "--pen-noncansplice") { if (!refInt(next(), 0, "--pen-noncansplice arg must be at least 0", o.pen_noncansplice)) return 1; }
+        else if (a == "--pen-conflictsplice") { if (!refInt(next(), 0, "--pen-conflictsplice arg must be at least 0", o.pen_conflictsplice)) return 1; }
+        else if (a == "--pen-canintronlen" || a == "--pen-intronlen") { if (!intronFunc(a.c_str(), next(), o.can_intronlen_type, o.can_intronlen_const, o.can_intronlen_coeff)) return 1; }
+        else if (a == "--pen-noncanintronlen") { if (!intronFunc(a.c_str(), next(), o.noncan_intronlen_type, o.noncan_intronlen_const, o.noncan_intronlen_coeff)) return 1; }
+        else if (a == "--min-intronlen") { if (!refInt(next(), 20, "--min-intronlen arg must be at least 20", o.min_intronlen)) return 1; }
+        else if (a == "--max-intronlen") { if (!refInt(next(), 20, "--max-intronlen arg must be at least 20", o.max_intronlen)) return 1; }
+        else if (a == "--dta" || a == "--downstream-transcriptome-assembly") { if (o.dta == HT2GPU_DTA_NONE) o.dta = HT2GPU_DTA_STRINGTIE; }
+        else if (a == "--dta-cufflinks") o.dta = HT2GPU_DTA_CUFFLINKS;
+        else if (a == "--no-anchorstop") o.no_anchorstop = 1;
+        else if (a == "--tmo" || a == "--transcriptome-mapping-only") o.tmo = 1;
+        else if (a == "--avoid-pseudogene") o.avoid_pseudogene = 1;
+        else if (a == "--reorder" || a == "-t" || a == "--time" || a == "--no-unal-ignored" || a == "--splicesite-db-only") {}
         else if (a == "-h" || a == "--help") { usage(); return 0; }
         else { fprintf(stderr, "Error: option %s is not supported by hisat2-b200\n", a.c_str()); return 1; }
     }
@@ -241,6 +287,10 @@ int main(int argc, char** argv)
     if (!o.no_spliced_alignment && !noTempSpliceSite)
         fprintf(stderr, "Warning: temporary splice sites (the reference's default) make results depend on the order reads are processed in;\n"
                         "         hisat2-b200 aligns every read independently, i.e. as with --no-temp-splicesite\n");
+    if (o.min_intronlen > o.max_intronlen) {   // hisat2.cpp:4278-4283
+        fprintf(stderr, "--min-intronlen(%d) should not be greater than --max-intronlen(%d)\n", o.min_intronlen, o.max_intronlen);
+        return 1;
+    }
     if (mpGiven) o.ignore_quals = 0;
     if (maBonus > 0) fprintf(stderr, "Warning: Match bonus always = 0 in --end-to-end mode; ignoring user setting\n");   // hisat2.cpp:3916-3919
     // presets, spelled out the way hisat2.cpp:1889-1909 applies them after option parsing

@@ -479,18 +479,13 @@ HT2_HD float ht2_intron_len_prob_noncan(uint32_t anchor, uint32_t intronLen, uin
     if (result > 1.0f) result = 1.0f;
     return result;
 }
-// Scoring::canSpl / noncanSpl (scoring.h:473-487) with the default penalty functions
-// (--pen-cansplice 0, --pen-noncansplice 12, --pen-canintronlen / --pen-noncanintronlen G,-8,1; hisat2.cpp:493-497)
-#define HT2_PEN_CONFLICTSPLICE 1000000
-// max(0, (int)(-8 + ln(x))) as integer breakpoints (the first x at which the value becomes k, found by
-// scanning the double-precision expression; exhaustively equal to it for x <= 2e6): no libm call, so the
-// device build will agree with the host bit for bit
-HT2_HD int64_t ht2_intron_pen(int intronlen) {
-    const uint32_t bp[13] = {8104u, 22027u, 59875u, 162755u, 442414u, 1202605u, 3269018u, 8886111u, 24154953u,
-                                    65659970u, 178482301u, 485165196u, 1318815735u};
-    int pen = 0;
-    if (intronlen > 0) for (int k = 0; k < 13 && (uint32_t)intronlen >= bp[k]; k++) pen = k + 1;
-    return pen;
+// The intron-length part of Scoring::canSpl / noncanSpl (scoring.h:473-487), max(0, f<int>(intronlen)), from the
+// function's runs (Ht2IntronPen, built on the host by ht2_set_intron_pen).  The runs cover every length the scorer
+// is given: a novel intron is at most maxIntronLen (canCombine) and HT2_MAX_SPL_LEN; longer ones take the last run.
+HT2_HD int64_t ht2_intron_pen(const Ht2IntronPen& t, uint32_t intronlen) {
+    uint32_t lo = 0, hi = t.n;
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (t.start[mid] <= intronlen) lo = mid; else hi = mid; }
+    return t.pen[lo];
 }
 #endif // HT2_ENABLE_SPLICED
 
@@ -515,7 +510,8 @@ struct Ht2AlignerT {
     uint32_t              swStride;
     uint32_t              swStage; // 0, or set by the pool kernel's DP round: 1 = problem framed and filled by the warp, 2 = nothing to fill (answer in swRetv)
     bool                  swRetv;
-    const int32_t*        nCeilTab; // --n-ceil per read length for the DP (Ht2Params::nCeilTab); NULL = the default
+    const int32_t*        nCeilTab; // --n-ceil per read length for the DP (Ht2Params::nCeilTab); NULL = the default.  The
+                                    // spliced scorer reads the intron-length penalties that follow it (Ht2Params::intronPen)
 #ifdef HT2_ENABLE_SPLICED
     const Ht2SplTables*   splT;    // donor / acceptor probability tables (spliced mode)
     const uint8_t*        ssT;     // read-only splice-site DB of the run (ht2_ssdb.h), NULL = empty (SpliceSiteDB::empty())
@@ -797,8 +793,9 @@ struct Ht2AlignerT {
                         }
                     }
                     {   // (edit.snpID is always "none" here: splice-site ALTs are not built)
-                        if (canon) score -= ht2_intron_pen((int)eLen) + P->canSplPen;
-                        else score -= ht2_intron_pen((int)eLen) + P->noncanSplPen;
+                        const Ht2IntronPen* ip = (const Ht2IntronPen*)(nCeilTab + HT2_PARAMS_NCEIL);   // Ht2Params::intronPen
+                        if (canon) score -= ht2_intron_pen(ip[0], eLen) + P->canSplPen;
+                        else score -= ht2_intron_pen(ip[1], eLen) + P->noncanSplPen;
                     }
                     if (shorter_anchor_len <= 15) { numsplices += 1; splicescore += (double)eLen; }
                 }
@@ -816,7 +813,7 @@ struct Ht2AlignerT {
         for (uint32_t i = 0; i < h.trim5; i++) score -= ht2_scpen(*P, qual[i]);
         for (uint32_t i = 0; i < h.trim3; i++) score -= ht2_scpen(*P, qual[i]);
 #ifdef HT2_ENABLE_SPLICED
-        if (conflict_splicesites) score -= HT2_PEN_CONFLICTSPLICE;
+        if (conflict_splicesites) score -= P->conflictSplPen;
         if (numsplices > 1) splicescore /= (double)numsplices;
         h.splicescore = splicescore;
 #endif
@@ -1872,6 +1869,31 @@ struct Ht2AlignerT {
         (void)numSpliced;
     }
 
+#ifdef HT2_ENABLE_SPLICED
+    // The transcriptome policy's filters of reportHit (hi_aligner.h:6098-6127): --dta-cufflinks drops a spliced hit
+    // whose GenomeHit::splicing_dir() is SPL_UNKNOWN (hi_aligner.h:1128-1150); --tmo drops every hit that is not
+    // spliced through known sites only (GenomeHit::spliced().second), so with no DB, or without spliced alignment,
+    // every hit (that case is decided in reportHit).  Edits of a reverse-strand hit are not yet inverted here, which
+    // changes neither answer.
+    HT2_NI bool tranFilterPass(const Ht2Hit& hit) const {
+        bool spl = false, known = true, conflict = false;
+        uint32_t dir = HT2_SPL_UNKNOWN;
+        for (uint32_t i = 0; i < hit.nedits; i++) {
+            const Ht2Edit& e = hit.edits[i];
+            if (e.type != HT2_EDIT_SPL) continue;
+            spl = true; known = known && ht2_spl_known(e);
+            const uint32_t d = ht2_spl_dir(e);
+            if (dir == HT2_SPL_UNKNOWN) dir = d;
+            else if (d != HT2_SPL_UNKNOWN) {
+                if ((dir == HT2_SPL_FW || dir == HT2_SPL_SEMI_FW) && d != HT2_SPL_FW && d != HT2_SPL_SEMI_FW) conflict = true;
+                if ((dir == HT2_SPL_RC || dir == HT2_SPL_SEMI_RC) && d != HT2_SPL_RC && d != HT2_SPL_SEMI_RC) conflict = true;
+            }
+        }
+        if ((P->tranFilter & HT2_TRAN_XS_ONLY) && spl && (conflict || dir == HT2_SPL_UNKNOWN)) return false;
+        if ((P->tranFilter & HT2_TRAN_TMO) && !(spl && known)) return false;
+        return true;
+    }
+#endif
     // HI_Aligner::reportHit (hi_aligner.h:6064-6198), unpaired form.
     HT2_NI bool reportHit(uint32_t rdi, const Ht2Hit& hit) {
 #if !defined(__CUDA_ARCH__) && defined(HT2_TRACE)
@@ -1880,6 +1902,15 @@ struct Ht2AlignerT {
         const uint32_t rdlen = W->rd[rdi].len;
         if (hit.rdoff - hit.trim5 > 0 || hit.len + hit.trim5 + hit.trim3 < rdlen) return false;
         if (hit.score < minsc[rdi]) return false;
+        if ((P->tranFilter & HT2_TRAN_FILTERS) != 0) {
+            // without spliced alignment no hit is spliced: --dta-cufflinks keeps all, --tmo none
+#ifdef HT2_ENABLE_SPLICED
+            if (NOSPL || noSpl()) { if (P->tranFilter & HT2_TRAN_TMO) return false; }
+            else if (!tranFilterPass(hit)) return false;
+#else
+            if (P->tranFilter & HT2_TRAN_TMO) return false;
+#endif
+        }
         uint32_t slot = (rdi == 0 && !rightendonly) ? 0 : 1;
         if (W->nRes[slot] >= HT2_MAX_RES) { W->err |= HT2_ERR_RES; return false; }
         if (W->nResEdits + hit.nedits > HT2_RES_EDITS) { W->err |= HT2_ERR_RES; return false; }

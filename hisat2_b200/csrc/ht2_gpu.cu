@@ -486,7 +486,7 @@ ht2_seed_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatch b, u
             st.len = len; st.cur = 0; st.done = 0; st.numPartialSearch = 0; st.numUniqueSearch = 0;
             while (!st.done) {
                 Ht2SeedHit ph;
-                bool pseudogeneStop = !GRAPH && !P.noSplicedAlignment, anchorStop = true;   // hi_aligner.h:4669-4670
+                bool pseudogeneStop = !GRAPH && !P.noSplicedAlignment, anchorStop = P.anchorStop != 0;   // hi_aligner.h:4669-4670
                 ht2_seed_partial<GRAPH>(fm, P, seq, st, ph, pseudogeneStop, anchorStop);
                 const bool blank = ph.top == HT2_IDX_MAX32;
                 const uint32_t nelt = blank ? 0u : ph.node_bot - ph.node_top;
@@ -826,9 +826,12 @@ extern "C" void ht2gpu_default_options(ht2gpu_options_t* o)
     o->min_frag = 0; o->max_frag = 1000;
     o->bowtie2_dp = 0; o->gbar = 4;
     o->score_min_type = 'L'; o->score_min_const = (double)0.0f; o->score_min_coeff = (double)-0.2f;   // hisat2.cpp:441
+    o->pen_noncansplice = 12; o->pen_conflictsplice = 1000000;                                         // hisat2.cpp:493-495
+    o->min_intronlen = 20; o->max_intronlen = 500000;                                                  // hisat2.cpp:498-499
 }
 
-static void applyOptions(Ht2Params& P, const Ht2Image& img, const ht2gpu_options_t& o)
+// Returns an error message for a configuration the device cannot reproduce, or NULL
+static const char* applyOptions(Ht2Params& P, const Ht2Image& img, const ht2gpu_options_t& o)
 {
     ht2_default_params(P, img, o.no_spliced_alignment != 0);
     if (o.khits > 0) P.khits = (uint32_t)o.khits;
@@ -846,6 +849,7 @@ static void applyOptions(Ht2Params& P, const Ht2Image& img, const ht2gpu_options
     // hisat2.cpp:1166-1168 and 3227-3236: the mates' strands, and the pair policy they give (0 FF, 2 FR, 3 RF)
     P.gMate1fw = o.pe_orient != HT2GPU_PE_RF; P.gMate2fw = o.pe_orient != HT2GPU_PE_FR;
     P.pePolicy = o.pe_orient == HT2GPU_PE_FF ? 0 : o.pe_orient == HT2GPU_PE_RF ? 3 : 2;
+    return ht2_apply_spliced_options(P, o);
 }
 
 // ---- ht2gpu_open*: the steps after the host image and the device blob have arrived -------------------------------
@@ -870,8 +874,8 @@ static int loadNamesAndParams(ht2gpu_handle* h)
     h->graph = !h->img->header()->global.linearFM;   // graph (SNP) indexes: ALT-aware aligner instantiation, graph seed kernel
     h->refNames.build(*h->img, h->opt.chr_names);
     CK(h->dRefNames.upload(h->refNames.blob.data(), h->refNames.blob.size()));
-    applyOptions(h->P, *h->img, h->opt);
-    CK(h->dMinsc.upload(h->P.minscTab, 2 * HT2_PARAMS_NCEIL));   // nCeilTab follows minscTab (ht2_params.h)
+    if (const char* why = applyOptions(h->P, *h->img, h->opt)) { h->err = why; return HT2GPU_ERR_UNSUPPORTED; }
+    CK(h->dMinsc.upload(h->P.minscTab, HT2_PARAMS_TABLE_WORDS));   // nCeilTab and intronPen follow minscTab (ht2_params.h)
     return HT2GPU_OK;
 }
 
@@ -982,6 +986,17 @@ static int startOpen(ht2gpu_handle* h)
     const int32_t pe = h->opt.pe_orient, nt = h->opt.n_ceil_type;
     if (pe != HT2GPU_PE_FR && pe != HT2GPU_PE_RF && pe != HT2GPU_PE_FF) { h->err = "pe_orient must be 0 (--fr), 1 (--rf) or 2 (--ff)"; return HT2GPU_ERR_ARG; }
     if (nt != 0 && nt != 'C' && nt != 'L' && nt != 'S' && nt != 'G') { h->err = "n_ceil_type must be 0 (default), 'C', 'L', 'S' or 'G'"; return HT2GPU_ERR_ARG; }
+    // the spliced-alignment options, with the reference's messages where it has one (hisat2.cpp:1631-1688, 4278-4283)
+    const ht2gpu_options_t& o = h->opt;
+    if (o.pen_cansplice < 0) { h->err = "--pen-cansplice arg must be at least 0"; return HT2GPU_ERR_ARG; }
+    if (o.pen_noncansplice < 0) { h->err = "--pen-noncansplice arg must be at least 0"; return HT2GPU_ERR_ARG; }
+    if (o.pen_conflictsplice < 0) { h->err = "--pen-conflictsplice arg must be at least 0"; return HT2GPU_ERR_ARG; }
+    if (o.min_intronlen < 20) { h->err = "--min-intronlen arg must be at least 20"; return HT2GPU_ERR_ARG; }
+    if (o.max_intronlen < 20) { h->err = "--max-intronlen arg must be at least 20"; return HT2GPU_ERR_ARG; }
+    if (o.min_intronlen > o.max_intronlen) { h->err = "--min-intronlen should not be greater than --max-intronlen"; return HT2GPU_ERR_ARG; }
+    for (const int32_t t : {o.can_intronlen_type, o.noncan_intronlen_type})
+        if (t != 0 && t != 'C' && t != 'L' && t != 'S' && t != 'G') { h->err = "can_intronlen_type / noncan_intronlen_type must be 0 (default), 'C', 'L', 'S' or 'G'"; return HT2GPU_ERR_ARG; }
+    if (o.dta != HT2GPU_DTA_NONE && o.dta != HT2GPU_DTA_STRINGTIE && o.dta != HT2GPU_DTA_CUFFLINKS) { h->err = "dta must be 0, 1 (--dta) or 2 (--dta-cufflinks)"; return HT2GPU_ERR_ARG; }
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n <= 0) {
@@ -1060,6 +1075,13 @@ extern "C" int ht2gpu_open_peer(const ht2gpu_handle_t* src, const ht2gpu_options
     o.chr_names = src->opt.chr_names;   // one run prints one set of names ...
     o.pe_orient = src->opt.pe_orient;   // ... and filters and pairs the reads one way
     o.n_ceil_type = src->opt.n_ceil_type; o.n_ceil_const = src->opt.n_ceil_const; o.n_ceil_coeff = src->opt.n_ceil_coeff;
+    // ... and scores and filters spliced alignments one way
+    o.pen_cansplice = src->opt.pen_cansplice; o.pen_noncansplice = src->opt.pen_noncansplice; o.pen_conflictsplice = src->opt.pen_conflictsplice;
+    o.can_intronlen_type = src->opt.can_intronlen_type; o.can_intronlen_const = src->opt.can_intronlen_const; o.can_intronlen_coeff = src->opt.can_intronlen_coeff;
+    o.noncan_intronlen_type = src->opt.noncan_intronlen_type; o.noncan_intronlen_const = src->opt.noncan_intronlen_const;
+    o.noncan_intronlen_coeff = src->opt.noncan_intronlen_coeff;
+    o.min_intronlen = src->opt.min_intronlen; o.max_intronlen = src->opt.max_intronlen;
+    o.dta = src->opt.dta; o.no_anchorstop = src->opt.no_anchorstop; o.tmo = src->opt.tmo; o.avoid_pseudogene = src->opt.avoid_pseudogene;
     return openHandle(&o, out, [&](ht2gpu_handle* h) -> int {
         h->img.reset(new Ht2Image());
         h->img->blob = src->img->blob;            // host copy: reference names / lengths for SAM
@@ -1373,6 +1395,7 @@ static Ht2SamIn samIn(const ht2gpu_handle* h, const SamSlot& S)
     in.reads = S.dReads; in.alns = S.dAlns; in.edits = S.dEdits; in.pairs = (const uint16_t*)S.dPairs.p;
     in.khits = h->P.khits; in.secondary = h->P.secondary; in.mixed = h->P.mixed; in.discord = h->P.discord;
     in.ssT = h->samOut.noTlenAdj ? NULL : h->dSsT.p;
+    in.nearSsT = (h->P.tranFilter & HT2_TRAN_AVOID_PSEUDOGENE) && !h->P.noSplicedAlignment ? h->dSsT.p : NULL;
     in.colCount = h->collectSs ? S.dCounters + 6 : NULL; in.colRecs = S.dColRecs; in.colCap = (uint32_t)S.dColRecs.cap;
     in.noUnal = h->samOut.noUnal; in.omitSecSeq = h->samOut.omitSecSeq; in.rgTag = h->dRgTag;
     in.rnaStrandness = h->samOut.rnaStrandness; in.noQnameTrunc = h->samOut.noQnameTrunc;
@@ -1962,12 +1985,20 @@ extern "C" int ht2gpu_set_sam_output(ht2gpu_handle_t* h, const ht2gpu_sam_output
     return HT2GPU_OK;
 }
 
-// The output settings, reference names, mate orientation and N ceiling of two handles are the same
-// (ht2gpu_run_reads_multi: one run filters, pairs and prints every read one way)
+// The output settings, reference names, mate orientation, N ceiling and spliced-alignment options of two handles are
+// the same (ht2gpu_run_reads_multi: one run filters, pairs, scores and prints every read one way)
 bool ht2_same_sam_output(const ht2gpu_handle_t* a, const ht2gpu_handle_t* b)
 {
-    return a->samOut == b->samOut && a->opt.chr_names == b->opt.chr_names && a->P.pePolicy == b->P.pePolicy &&
-           memcmp(a->P.nCeilTab, b->P.nCeilTab, sizeof(a->P.nCeilTab)) == 0;
+    const Ht2Params &p = a->P, &q = b->P;
+    bool spl = p.minIntronLen == q.minIntronLen && p.maxIntronLen == q.maxIntronLen && p.minAnchorLen == q.minAnchorLen &&
+               p.minAnchorLenNoncan == q.minAnchorLenNoncan && p.anchorStop == q.anchorStop && p.canSplPen == q.canSplPen &&
+               memcmp(p.intronPen, q.intronPen, sizeof(p.intronPen)) == 0;
+#ifdef HT2_ENABLE_SPLICED
+    spl = spl && p.noncanSplPen == q.noncanSplPen && p.conflictSplPen == q.conflictSplPen;
+#endif
+    spl = spl && p.tranFilter == q.tranFilter;
+    return a->samOut == b->samOut && a->opt.chr_names == b->opt.chr_names && p.pePolicy == q.pePolicy &&
+           memcmp(p.nCeilTab, q.nCeilTab, sizeof(p.nCeilTab)) == 0 && spl;
 }
 int ht2_handle_device(const ht2gpu_handle_t* h) { return h->device; }
 

@@ -6,6 +6,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <limits>
 #include <functional>
 #include <thread>
 
@@ -54,6 +55,13 @@ void ht2_default_params(Ht2Params& P, const Ht2Image& img, bool noSplicedAlignme
     // hisat2.cpp:443 initialises 2 + 0.1 len, but SeedAlignmentPolicy::parseString -- always called, hisat2.cpp:1849 --
     // resets it to DEFAULT_N_CEIL_CONST / LINEAR = 0.0 / 0.15 (aligner_seed_policy.cpp:293-296, scoring.h:65-67)
     ht2_set_n_ceil(P, 'L', (double)0.0f, (double)0.15f);
+    // --pen-canintronlen / --pen-noncanintronlen G,-8,1 (hisat2.cpp:496-497) over the lengths the scorer can be given
+    const uint32_t cover = ht2_intron_cover(P);
+    ht2_set_intron_pen(P, 0, 'G', -8.0, 1.0, cover);
+    ht2_set_intron_pen(P, 1, 'G', -8.0, 1.0, cover);
+#ifdef HT2_ENABLE_SPLICED
+    P.conflictSplPen = 1000000;                         // hisat2.cpp:495
+#endif
 }
 
 // SimpleFunc::f<TAlScore> (simple_func.h:86-108) with min = -DBL_MAX, max = DBL_MAX
@@ -86,6 +94,56 @@ bool ht2_set_n_ceil(Ht2Params& P, char type, double C, double L)
         P.nCeilTab[len] = v == dmax ? 2147483647 : v >= 2147483648.0 ? (int32_t)0x80000000u : (int32_t)v;
     }
     return true;
+}
+
+// The runs of max(0, SimpleFunc::f<int>(x)) (simple_func.h:86-108, min -DBL_MAX, max DBL_MAX; scoring.h:473-487) for
+// the intron lengths x = 1 .. maxLen, into P.intronPen[which]; length 0 scores 0.  The value is converted as x86-64
+// converts it: DBL_MAX gives INT_MAX, DBL_MIN and anything outside int's range INT_MIN, which the max makes 0.
+// False for a bad type, or when the function takes more than HT2_INTRON_RUNS values over the range.
+bool ht2_set_intron_pen(Ht2Params& P, int which, char type, double C, double L, uint32_t maxLen)
+{
+    if (type != 'C' && type != 'L' && type != 'S' && type != 'G') return false;
+    Ht2IntronPen& t = P.intronPen[which];
+    const double dmax = std::numeric_limits<double>::max(), dmin = std::numeric_limits<double>::min();
+    t.n = 1; t.start[0] = 0; t.pen[0] = 0;
+    for (uint32_t len = 1; len <= maxLen; len++) {
+        const double x = (double)len;
+        double X;
+        if (type == 'C') X = 0.0; else if (type == 'L') X = x; else if (type == 'S') X = sqrt(x); else X = log(x);
+        const double v = std::max(-dmax, std::min(dmax, C + L * X));
+        int32_t pen = v == dmax ? 2147483647 : v == dmin ? (int32_t)0x80000000u
+                    : (v >= -2147483648.0 && v < 2147483648.0) ? (int32_t)v : (int32_t)0x80000000u;
+        if (pen < 0) pen = 0;
+        if (pen == t.pen[t.n - 1]) continue;
+        if (t.n == HT2_INTRON_RUNS) return false;
+        t.start[t.n] = len; t.pen[t.n] = pen; t.n++;
+    }
+    return true;
+}
+
+const char* ht2_apply_spliced_options(Ht2Params& P, const ht2gpu_options_t& o)
+{
+    // hisat2.cpp:1631-1728, 3920-3922, 4075-4084.  maxIntronLen also bounds concordant pairs without spliced
+    // alignment (ht2_pair.h).
+    P.minIntronLen = (uint32_t)o.min_intronlen; P.maxIntronLen = (uint32_t)o.max_intronlen;
+    P.anchorStop = o.no_anchorstop ? 0 : 1;
+    P.canSplPen = o.pen_cansplice;
+#ifdef HT2_ENABLE_SPLICED
+    P.noncanSplPen = o.pen_noncansplice; P.conflictSplPen = o.pen_conflictsplice;
+#endif
+    P.tranFilter = (o.dta == HT2GPU_DTA_CUFFLINKS ? HT2_TRAN_XS_ONLY : 0u) | (o.tmo ? HT2_TRAN_TMO : 0u) |
+                   (o.avoid_pseudogene ? HT2_TRAN_AVOID_PSEUDOGENE : 0u);
+    if (o.dta != HT2GPU_DTA_NONE) { P.minAnchorLen = 15; P.minAnchorLenNoncan = 20; }
+    // the intron-length functions: tokens left out keep G,-8,1; --dta sets the non-canonical one to G,-8,2 after
+    // everything else was parsed.  No splice is scored without spliced alignment.
+    const uint32_t cover = P.noSplicedAlignment ? 0u : ht2_intron_cover(P);
+    const bool can = o.can_intronlen_type != 0, noncan = o.noncan_intronlen_type != 0 && o.dta == HT2GPU_DTA_NONE;
+    if (!ht2_set_intron_pen(P, 0, can ? (char)o.can_intronlen_type : 'G', can ? o.can_intronlen_const : -8.0, can ? o.can_intronlen_coeff : 1.0, cover))
+        return "--pen-canintronlen takes more distinct values over the intron lengths up to --max-intronlen than the device holds (1024)";
+    if (!ht2_set_intron_pen(P, 1, noncan ? (char)o.noncan_intronlen_type : 'G', noncan ? o.noncan_intronlen_const : -8.0,
+                            noncan ? o.noncan_intronlen_coeff : o.dta != HT2GPU_DTA_NONE ? 2.0 : 1.0, cover))
+        return "--pen-noncanintronlen takes more distinct values over the intron lengths up to --max-intronlen than the device holds (1024)";
+    return NULL;
 }
 
 int64_t ht2_minsc(const Ht2Params& P, uint32_t rdlen)
@@ -401,7 +459,9 @@ bool ht2_format_batch(const Ht2Image& img, const Ht2Params& P, const ht2gpu_read
     in.n_reads = b->n_reads; in.paired = b->paired;
     in.reads = res->reads; in.alns = res->alns; in.edits = res->edits; in.pairs = res->pairs;
     in.khits = P.khits; in.secondary = P.secondary; in.mixed = P.mixed; in.discord = P.discord;
-    in.ssT = so && so->noTlenAdj ? NULL : ssT; in.colCount = colCount; in.colRecs = colRecs; in.colCap = colCap;
+    in.ssT = so && so->noTlenAdj ? NULL : ssT;
+    in.nearSsT = (P.tranFilter & HT2_TRAN_AVOID_PSEUDOGENE) && !P.noSplicedAlignment ? ssT : NULL;
+    in.colCount = colCount; in.colRecs = colRecs; in.colCap = colCap;
     in.noUnal = so && so->noUnal; in.omitSecSeq = so && so->omitSecSeq; in.rgTag = rgTag.empty() ? NULL : rgTag.c_str();
     in.rnaStrandness = so ? so->rnaStrandness : 0; in.noQnameTrunc = so && so->noQnameTrunc;
     in.unitOut = unitOut;

@@ -37,6 +37,16 @@ int64_t ht2_minsc(const Ht2Params& P, uint32_t rdlen);
 bool ht2_set_score_min(Ht2Params& P, char type, double C, double L);
 // --n-ceil <type>,<const>,<coeff> into P.nCeilTab; type one of C, L, S, G
 bool ht2_set_n_ceil(Ht2Params& P, char type, double C, double L);
+// --pen-canintronlen (which 0) / --pen-noncanintronlen (1) <type>,<const>,<coeff> into P.intronPen over the intron
+// lengths 1 .. maxLen; false for a bad type or a function with more than HT2_INTRON_RUNS values there
+bool ht2_set_intron_pen(Ht2Params& P, int which, char type, double C, double L, uint32_t maxLen);
+// The longest intron the spliced scorer can be given: a novel intron is at most --max-intronlen (canCombine) and
+// what a splice edit holds
+inline uint32_t ht2_intron_cover(const Ht2ParamsCore& P) { return P.maxIntronLen < HT2_MAX_SPL_LEN ? P.maxIntronLen : HT2_MAX_SPL_LEN; }
+// The spliced-alignment settings of o (penalties, intron bounds, --dta, --no-anchorstop, --tmo, --avoid-pseudogene)
+// into P, as ht2gpu_open applies them; P.noSplicedAlignment must already be set.  Returns the refusal message of a
+// configuration the device cannot reproduce, or NULL.
+const char* ht2_apply_spliced_options(Ht2Params& P, const ht2gpu_options_t& o);
 // nCeilTab: Ht2Params::nCeilTab; NULL = the default N ceiling
 Ht2ReadFilters ht2_filters(const Ht2HostRead& rd, int64_t minsc, const int32_t* nCeilTab = NULL);
 uint32_t ht2_gen_rand_seed(const Ht2HostRead& rd, uint32_t seed);

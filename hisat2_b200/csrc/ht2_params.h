@@ -54,9 +54,27 @@ struct Ht2ParamsCore {
     // --bowtie2-dp (hisat2.cpp:293, 1770): 0 off, 1 when the anchor search found nothing >= minsc, 2 always
     uint32_t bowtie2Dp;
     int32_t  gapbar;       // --gbar (4): no gaps within this many rows of either read end (DP only)
+    uint32_t tranFilter;   // the transcriptome policy (HT2_TRAN_*), 0 = none
 #ifdef HT2_ENABLE_SPLICED
     int32_t  noncanSplPen; // --pen-noncansplice (12); --pen-cansplice is canSplPen above
+    int32_t  conflictSplPen; // --pen-conflictsplice (1000000)
 #endif
+};
+#define HT2_TRAN_XS_ONLY 1u   // --dta-cufflinks: reportHit drops spliced hits of unknown sense (hi_aligner.h:6101-6104)
+#define HT2_TRAN_TMO     2u   // --tmo: reportHit drops hits not spliced through known sites only (hi_aligner.h:6126-6127)
+#define HT2_TRAN_FILTERS (HT2_TRAN_XS_ONLY | HT2_TRAN_TMO)
+#define HT2_TRAN_AVOID_PSEUDOGENE 4u   // --avoid-pseudogene: unspliced alignments near listed sites rank as spliced ones
+                                       // (hi_aligner.h:6105-6125); read by the SAM formatter's selection key only
+
+// An intron-length penalty function (--pen-canintronlen / --pen-noncanintronlen) as the runs of its integer value:
+// the penalty of an intron of x bases is pen[k] for the last k with start[k] <= x.  The host evaluates
+// max(0, SimpleFunc::f<int>(x)) for every length a kernel can score (ht2_set_intron_pen), so no device libm call
+// is involved.  A function with more runs than HT2_INTRON_RUNS over that range is refused.
+#define HT2_INTRON_RUNS 1024
+struct Ht2IntronPen {
+    uint32_t n;
+    uint32_t start[HT2_INTRON_RUNS];
+    int32_t  pen[HT2_INTRON_RUNS];
 };
 
 // Host-side parameters = the core + the --score-min table.  The table reaches the device as a
@@ -74,8 +92,14 @@ struct Ht2Params : Ht2ParamsCore {
     // two travel as one buffer: the device's (DevBatch::minscTab) and the formatter's (Ht2SamIn::minscTab) hold the
     // N ceilings from HT2_PARAMS_NCEIL on, so no kernel parameter grows.
     int32_t  nCeilTab[HT2_PARAMS_MAX_RDLEN + 1];
+    // The intron-length penalties, canonical ([0]) and non-canonical ([1]), as runs.  They follow nCeilTab in the same
+    // buffer (the device reads them at nCeilTab + HT2_PARAMS_NCEIL); the spliced scorer is their only reader.
+    Ht2IntronPen intronPen[2];
 };
 #define HT2_PARAMS_NCEIL (HT2_PARAMS_MAX_RDLEN + 1)
-static_assert(sizeof(Ht2Params) == sizeof(Ht2ParamsCore) + 2 * sizeof(int32_t) * HT2_PARAMS_NCEIL, "minscTab and nCeilTab must be adjacent");
+// the tables after the core, in int32 words: the size of the device buffer (DevBatch::minscTab)
+#define HT2_PARAMS_TABLE_WORDS (2 * HT2_PARAMS_NCEIL + 2 * (sizeof(Ht2IntronPen) / sizeof(int32_t)))
+static_assert(sizeof(Ht2Params) == sizeof(Ht2ParamsCore) + sizeof(int32_t) * HT2_PARAMS_TABLE_WORDS,
+              "minscTab, nCeilTab and intronPen must be adjacent");
 
 #endif

@@ -369,7 +369,7 @@ struct Run {
         if (route && !routes->write) return HT2GPU_ERR_ARG;
         if (routes) { routes->n_spans = 0; routes->bytes = 0; routes->s_route = 0; }
         for (int i = 1; i < nDev; i++)
-            if (!ht2_same_sam_output(hs[0], hs[i])) { ht2gpu_set_error(hs[0], "ht2gpu_run_reads_multi: the handles' SAM output, mate orientation or N-ceiling settings differ"); return HT2GPU_ERR_ARG; }
+            if (!ht2_same_sam_output(hs[0], hs[i])) { ht2gpu_set_error(hs[0], "ht2gpu_run_reads_multi: the handles' SAM output, mate orientation, N-ceiling or spliced-alignment settings differ"); return HT2GPU_ERR_ARG; }
         const double t0 = nowS();
         nSlots = ht2gpu_sam_slots(hs[0]) * nDev;   // stage k: device k % nDev, device slot k / nDev
         C = ctxOf(hs[0], threadCount(in), nSlots);

@@ -42,6 +42,7 @@ struct Ht2SamIn {
     uint32_t khits, secondary, mixed, discord;
     const uint8_t*  ssT;         // the run's splice-site DB (ht2_ssdb.h) or NULL: template-length adjustment of concordant
                                  // pairs (NULL under --no-templatelen-adjustment)
+    const uint8_t*  nearSsT;     // --avoid-pseudogene in spliced mode: the run's splice-site DB, or NULL
     uint32_t*       colCount;    // --novel-splicesite-outfile: junctions of the printed alignments (write pass only), or NULL
     Ht2SsRec*       colRecs;
     uint32_t        colCap;
@@ -279,6 +280,24 @@ struct Ht2SamFmt {
         rd.nfilt = ns <= maxns; rd.scfilt = (0 >= m); rd.lenfilt = rd.len >= 2;
     }
 
+#ifdef HT2_ENABLE_SPLICED
+    // --avoid-pseudogene (hi_aligner.h:6105-6125): an unspliced alignment is near splice sites when the DB has a site
+    // whose left or right end lies in [refoff - 10000, refoff + len + 10000] (SpliceSiteDB::hasSpliceSites with both
+    // windows equal, novel sites included; the _bwIndex tree is keyed on the right end, _fwIndex on the left,
+    // splice_site.cpp:436-506), len being the read bases the alignment covers.
+    HT2_HD bool nearSpliceSites(const ht2gpu_aln_t& al, uint32_t rdlen) const {
+        Ht2SsView v; v.init(in->nearSsT);
+        if (al.tidx >= v.h->nRefs) return false;
+        const uint32_t left = al.toff > 10000u ? al.toff - 10000u : 0u, right = al.toff + (rdlen - al.trim5 - al.trim3) + 10000u;
+        const uint32_t a = v.refOff[al.tidx], b = v.refOff[al.tidx + 1];
+        uint32_t l = a, r = b;
+        while (l < r) { const uint32_t m = l + ((r - l) >> 1); if (v.bw[m].right < left) l = m + 1; else r = m; }
+        if (l < b && v.bw[l].right <= right) return true;
+        l = a; r = b;
+        while (l < r) { const uint32_t m = l + ((r - l) >> 1); if (v.fw[m].left < left) l = m + 1; else r = m; }
+        return l < b && v.fw[l].left <= right;
+    }
+#endif
     // AlnScore::calculate_hisat2_score (aligner_result.h:322-348), repeat = 0.  The splice part of the key
     // follows from the edits alone: GenomeHit::spliced() and the splicescore rule of calculateScore
     // (hi_aligner.h:3745-3817) in the hit's (reference-forward) orientation.
@@ -313,7 +332,7 @@ struct Ht2SamFmt {
             if (nss > 1) ss /= (double)nss;
             splicescore = (int64_t)(ss / 100);     // TAlScore splicescore = splicescore_ / 100 (aligner_result.h:339)
             if (splicescore > 255) splicescore = 0; else splicescore = 255 - splicescore;
-            transcript_score = (spl && known) ? 2 : (spl ? 1 : 0);
+            transcript_score = (spl && known) ? 2 : (spl || (in->nearSsT != NULL && nearSpliceSites(al, rdlen))) ? 1 : 0;
         }
 #else
         (void)rdlen;

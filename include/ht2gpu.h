@@ -91,9 +91,39 @@ typedef struct {
     int32_t  n_ceil_type;
     double   n_ceil_const;
     double   n_ceil_coeff;
+    /* Spliced alignment (hisat2.cpp:1631-1728, 4075-4084).  A negative penalty, an intron bound below 20 or
+     * min_intronlen > max_intronlen is HT2GPU_ERR_ARG before a device is used.
+     *   pen_cansplice / pen_noncansplice / pen_conflictsplice: --pen-cansplice 0, --pen-noncansplice 12,
+     *     --pen-conflictsplice 1000000 (a read spliced in both senses).
+     *   can_intronlen_* / noncan_intronlen_*: --pen-canintronlen / --pen-noncanintronlen <type>,<const>,<coeff>, the
+     *     intron-length penalty max(0, (int)(const + coeff * F(len))) of novel canonical and non-canonical junctions,
+     *     F as for score_min_type.  Type 0 = the default G,-8,1.  A function that takes more than 1024 distinct
+     *     values over the intron lengths up to max_intronlen is HT2GPU_ERR_UNSUPPORTED.
+     *   min_intronlen / max_intronlen: --min-intronlen 20 / --max-intronlen 500000.  max_intronlen also bounds the
+     *     distance of concordant mates under --no-spliced-alignment, as in the reference.
+     *   dta: HT2GPU_DTA_STRINGTIE (--dta) needs anchors of 15 (canonical) / 20 (non-canonical) bases for long
+     *     introns and makes the non-canonical function G,-8,2 whatever noncan_intronlen_* say; HT2GPU_DTA_CUFFLINKS
+     *     (--dta-cufflinks) does the same and drops spliced alignments of unknown or conflicting sense.
+     *   no_anchorstop: --no-anchorstop, partial searches do not stop at a unique anchor.
+     *   tmo: --tmo, only alignments spliced through known sites (ht2gpu_load_splicesites) are reported.
+     *   avoid_pseudogene: --avoid-pseudogene, in spliced mode an unspliced alignment within 10 000 bases of a loaded
+     *     splice site ranks like a spliced one when the primary alignment is chosen (the SAM formatter's key).  No
+     *     effect without a loaded DB.
+     * ht2gpu_open_peer takes the source handle's settings. */
+    int32_t  pen_cansplice, pen_noncansplice, pen_conflictsplice;
+    int32_t  can_intronlen_type;
+    double   can_intronlen_const, can_intronlen_coeff;
+    int32_t  noncan_intronlen_type;
+    double   noncan_intronlen_const, noncan_intronlen_coeff;
+    int32_t  min_intronlen, max_intronlen;
+    int32_t  dta;
+    int32_t  no_anchorstop;
+    int32_t  tmo;
+    int32_t  avoid_pseudogene;
 } ht2gpu_options_t;
 enum { HT2GPU_CHR_NAMES_INDEX = 0, HT2GPU_CHR_NAMES_REMOVE = 1, HT2GPU_CHR_NAMES_ADD = 2 };
 enum { HT2GPU_PE_FR = 0, HT2GPU_PE_RF = 1, HT2GPU_PE_FF = 2 };
+enum { HT2GPU_DTA_NONE = 0, HT2GPU_DTA_STRINGTIE = 1, HT2GPU_DTA_CUFFLINKS = 2 };
 
 /* A batch of reads, structure-of-arrays, host memory.  Read i occupies
  * seq[offs[i] .. offs[i+1]).  Bases are codes 0..4 (A,C,G,T,N) exactly as
