@@ -559,7 +559,22 @@ struct Ht2AlignerT {
         d.splicescore = s.splicescore;
 #endif
         d.nedits = s.nedits;
-        for (uint32_t i = 0; i < s.nedits; i++) d.edits[i] = s.edits[i];
+        moveEdits(d.edits, s.edits, s.nedits);
+    }
+    // Moves and reversals of Ht2Edit ranges, one out-of-line copy each: inlined, every caller carried its own unrolled
+    // loop of 12-byte copies, for lists that hold one edit or none on most hits.  moveEdits allows overlap (memmove).
+    HT2_NI static void moveEdits(Ht2Edit* d, const Ht2Edit* s, uint32_t n) {
+        if (d <= s) {
+#pragma unroll 1
+            for (uint32_t i = 0; i < n; i++) d[i] = s[i];
+        } else {
+#pragma unroll 1
+            for (uint32_t i = n; i > 0; i--) d[i - 1] = s[i - 1];
+        }
+    }
+    HT2_NI static void reverseEdits(Ht2Edit* ed, uint32_t n) {
+#pragma unroll 1
+        for (uint32_t i = 0; i < n / 2; i++) { Ht2Edit t = ed[i]; ed[i] = ed[n - i - 1]; ed[n - i - 1] = t; }
     }
     HT2_HD static void initHit(Ht2Hit& h, bool fw, uint32_t rdoff, uint32_t len, uint32_t trim5, uint32_t trim3,
                                uint32_t tidx, uint32_t toff, uint32_t joinedOff) {
@@ -578,19 +593,22 @@ struct Ht2AlignerT {
     }
     HT2_NI bool insertEditFront(Ht2Hit& h, const Ht2Edit& e) {
         if (h.nedits >= HT2_MAX_EDITS) { W->err |= HT2_ERR_EDITS; return false; }
-        for (uint32_t i = h.nedits; i > 0; i--) h.edits[i] = h.edits[i - 1];
+        moveEdits(h.edits + 1, h.edits, h.nedits);
         h.edits[0] = e; h.nedits++; HT2_HIWATER(maxEdits, h.nedits); return true;
     }
+    // A splice edit.  Only combineWith's spliced join makes one, so an instantiation for --no-spliced-alignment never
+    // holds one, and every test for one compiles away there.
+    HT2_HD static bool isSpl(const Ht2Edit& e) { return !NOSPL && e.type == HT2_EDIT_SPL; }
     HT2_HD static bool editEq(const Ht2Edit& a, const Ht2Edit& b) { // Edit::operator== (edit.h)
         if (a.type != b.type) return false;
         if (a.pos != b.pos) return false;
 #ifdef HT2_ENABLE_SPLICED
-        if (a.type == HT2_EDIT_SPL) return ht2_spl_len(a) == ht2_spl_len(b) && ht2_spl_dir(a) == ht2_spl_dir(b);
+        if (isSpl(a)) return ht2_spl_len(a) == ht2_spl_len(b) && ht2_spl_dir(a) == ht2_spl_dir(b);
 #endif
         return a.chr == b.chr && a.qchr == b.qchr;
     }
     HT2_HD static bool isGapOrSnp(const Ht2Edit& e) {
-        return e.type == HT2_EDIT_SPL || e.type == HT2_EDIT_READ_GAP || e.type == HT2_EDIT_REF_GAP ||
+        return isSpl(e) || e.type == HT2_EDIT_READ_GAP || e.type == HT2_EDIT_REF_GAP ||
                (e.type == HT2_EDIT_MM && e.snpID != HT2_IDX_MAX32);
     }
     // GenomeHit::operator== (hi_aligner.h:1156-1183)
@@ -608,9 +626,10 @@ struct Ht2AlignerT {
     }
     // Edit::invertPoss (edit.cpp:70-111), sort=false
     HT2_HD static void invertPoss(Ht2Edit* ed, uint32_t n, uint32_t sz) {
-        for (uint32_t i = 0; i < n / 2; i++) { Ht2Edit t = ed[i]; ed[i] = ed[n - i - 1]; ed[n - i - 1] = t; }
+        reverseEdits(ed, n);
+#pragma unroll 1
         for (uint32_t i = 0; i < n; i++) {
-            if (ed[i].type == HT2_EDIT_READ_GAP || ed[i].type == HT2_EDIT_SPL) ed[i].pos = (uint32_t)(sz - ed[i].pos);
+            if (ed[i].type == HT2_EDIT_READ_GAP || isSpl(ed[i])) ed[i].pos = (uint32_t)(sz - ed[i].pos);
             else ed[i].pos = (uint32_t)(sz - ed[i].pos - 1);
         }
     }
@@ -695,7 +714,7 @@ struct Ht2AlignerT {
             if (h.edits[i].type == HT2_EDIT_READ_GAP) toff++;
             else if (h.edits[i].type == HT2_EDIT_REF_GAP) toff--;
 #ifdef HT2_ENABLE_SPLICED
-            else if (h.edits[i].type == HT2_EDIT_SPL) toff += ht2_spl_len(h.edits[i]);
+            else if (isSpl(h.edits[i])) toff += ht2_spl_len(h.edits[i]);
 #endif
         }
         return toff;
@@ -749,7 +768,7 @@ struct Ht2AlignerT {
                 if (e.snpID == HT2_IDX_MAX32) score -= open ? (P->rfGapConst + P->rfGapLinear) : P->rfGapLinear;
             }
 #ifdef HT2_ENABLE_SPLICED
-            else if (e.type == HT2_EDIT_SPL) {   // hi_aligner.h:3745-3838
+            else if (isSpl(e)) {   // hi_aligner.h:3745-3838
                 const uint32_t eDir = ht2_spl_dir(e), eLen = ht2_spl_len(e);
                 const bool canon = (eDir == HT2_SPL_FW || eDir == HT2_SPL_RC);
                 if (!ht2_spl_known(e)) {
@@ -810,7 +829,9 @@ struct Ht2AlignerT {
 #endif
         }
         // soft-clip penalty indexes qual[i], not the clipped position (hi_aligner.h:3872-3878)
+#pragma unroll 1
         for (uint32_t i = 0; i < h.trim5; i++) score -= ht2_scpen(*P, qual[i]);
+#pragma unroll 1
         for (uint32_t i = 0; i < h.trim3; i++) score -= ht2_scpen(*P, qual[i]);
 #ifdef HT2_ENABLE_SPLICED
         if (conflict_splicesites) score -= P->conflictSplPen;
@@ -1308,8 +1329,7 @@ struct Ht2AlignerT {
         } else {
             // edits are only committed when the scan improved on best_rdoff
             if (h.nedits > nedits0) {
-                uint32_t added = h.nedits - nedits0;
-                for (uint32_t i = 0; i + added < h.nedits; i++) h.edits[i] = h.edits[i + added];
+                moveEdits(h.edits, h.edits + (h.nedits - nedits0), nedits0);
                 h.nedits = nedits0;
             }
         }
@@ -1383,7 +1403,7 @@ struct Ht2AlignerT {
         if (extlen > 0 && h.nedits > 0) {
             const Ht2Edit& f = h.edits[0];
             if (f.pos + extlen == base_rdoff + 1) {
-                if (f.type == HT2_EDIT_READ_GAP || f.type == HT2_EDIT_REF_GAP || f.type == HT2_EDIT_SPL) extlen = 0;
+                if (f.type == HT2_EDIT_READ_GAP || f.type == HT2_EDIT_REF_GAP || isSpl(f)) extlen = 0;
                 if (f.type == HT2_EDIT_MM && f.chr == 'N') extlen = 0;
             }
             const Ht2Edit& b = h.edits[h.nedits - 1];
@@ -1391,11 +1411,8 @@ struct Ht2AlignerT {
                 if (b.type == HT2_EDIT_READ_GAP || b.type == HT2_EDIT_REF_GAP) extlen = 0;
             }
             if (extlen == 0 && h.nedits > nedits0) {
-                if (left) {
-                    uint32_t added = h.nedits - nedits0;
-                    for (uint32_t i = 0; i + added < h.nedits; i++) h.edits[i] = h.edits[i + added];
-                    h.nedits = nedits0;
-                } else h.nedits = nedits0;
+                if (left) moveEdits(h.edits, h.edits + (h.nedits - nedits0), nedits0);
+                h.nedits = nedits0;
             }
         }
         return extlen;
@@ -1424,6 +1441,7 @@ struct Ht2AlignerT {
                 leftext = best_ext;
                 uint32_t added_edits = h.nedits - num_prev_edits;
                 int ref_ext = (int)best_ext;
+#pragma unroll 1
                 for (uint32_t i = 0; i < added_edits; i++) {
                     if (h.edits[i].type == HT2_EDIT_REF_GAP) ref_ext--;
                     else if (h.edits[i].type == HT2_EDIT_READ_GAP) ref_ext++;
@@ -1432,6 +1450,7 @@ struct Ht2AlignerT {
                 h.toff -= (uint32_t)ref_ext;
                 h.len += best_ext;
                 h.joinedOff -= (uint32_t)(ref_ext - (int)numNs);
+#pragma unroll 1
                 for (uint32_t i = 0; i < h.nedits; i++) {
                     if (i < added_edits) h.edits[i].pos -= h.rdoff;
                     else h.edits[i].pos += best_ext;
@@ -1527,6 +1546,47 @@ struct Ht2AlignerT {
             }
             ei = ei2;
         }
+    }
+
+    // The split point of a join with an insertion (inslen > 0) or a deletion (dellen > 0), hi_aligner.h:1759-1795: the
+    // best sum of this hit's prefix scores and the other hit's suffix scores over the window, on this hit's decoded
+    // reference (refbuf) and the other's (refbuf2, decoded here).  rd / qu start at this hit's read offset; otherEnd is
+    // other_toff + other_len.  Out of line: most bench joins have no gap and never come here.
+    HT2_NI bool gapJoinSplit(uint32_t tidx, const uint8_t* rd, const uint8_t* qu, const uint8_t* refbuf, uint32_t len, uint32_t otherEnd,
+                             int read_gaps, int inslen, int dellen, int64_t remainsc, const uint8_t*& refbuf2, uint32_t& maxscorei) {
+        int other_ref_ext = read_gaps;
+        int lim = (int)(otherEnd - len);
+        if (lim < other_ref_ext) other_ref_ext = lim;
+        if ((int)len + other_ref_ext > (int)HT2_REFBUF || other_ref_ext < 0) { W->err |= HT2_ERR_RDLEN; return false; }
+        refbuf2 = getStretch(W->refbuf2, tidx, otherEnd - len - (uint32_t)other_ref_ext, len + (uint32_t)other_ref_ext) + other_ref_ext;
+        int64_t* ts = W->tscores; int64_t* ts2 = W->tscores2;
+        int64_t gap_penalty;
+        if (inslen > 0) gap_penalty = -((int64_t)(P->rfGapConst + P->rfGapLinear) + (int64_t)P->rfGapLinear * (inslen - 1));
+        else gap_penalty = -((int64_t)(P->rdGapConst + P->rdGapLinear) + (int64_t)P->rdGapLinear * (dellen - 1));
+        if (gap_penalty < remainsc) return false;
+        int i;
+        for (i = 0; i < (int)len; i++) {
+            int rdc = rd[i], rfc = refbuf[i];
+            ts[i] = i > 0 ? ts[i - 1] : 0;
+            if (rdc != rfc) ts[i] += ht2_score(*P, rdc, 1 << rfc, (int)qu[i] - 33);
+            if (ts[i] + gap_penalty < remainsc) break;
+        }
+        int i_limit = i < (int)len ? i : (int)len;
+        int i2;
+        for (i2 = (int)len - 1; i2 >= 0; i2--) {
+            int rdc = rd[i2], rfc = refbuf2[i2];
+            ts2[i2] = ((uint32_t)(i2 + 1) < len) ? ts2[i2 + 1] : 0;
+            if (rdc != rfc) ts2[i2] += ht2_score(*P, rdc, 1 << rfc, (int)qu[i2] - 33);
+            if (ts2[i2] + gap_penalty < remainsc) break;
+        }
+        int i2_limit = (i2 < inslen ? 0 : i2 - inslen);
+        int64_t maxscore = HT2_MIN_I64;
+        for (i = i2_limit, i2 = i2_limit + 1 + inslen; i < i_limit && i2 < (int)len; i++, i2++) {
+            int64_t tempscore = ts[i] + ts2[i2] + gap_penalty;
+            if (maxscore < tempscore) { maxscore = tempscore; maxscorei = (uint32_t)i; }
+        }
+        if (maxscore == HT2_MIN_I64) return false;
+        return maxscore >= remainsc;
     }
 
     // GenomeHit::combineWith (hi_aligner.h:1420-2025), non-spliced paths
@@ -1682,43 +1742,9 @@ struct Ht2AlignerT {
             if (maxscore < remainsc) return false;
         }
 #endif
-        if (ins || del) {
-            int other_ref_ext = read_gaps;
-            int lim = (int)(other_toff + other_len - len);
-            if (lim < other_ref_ext) other_ref_ext = lim;
-            if ((int)len + other_ref_ext > (int)HT2_REFBUF || other_ref_ext < 0) { W->err |= HT2_ERR_RDLEN; return false; }
-            refbuf2 = getStretch(W->refbuf2, o.tidx, other_toff + other_len - len - (uint32_t)other_ref_ext, len + (uint32_t)other_ref_ext)
-                      + other_ref_ext;
-            int64_t* ts = W->tscores; int64_t* ts2 = W->tscores2;
-            int inslen = (ins ? (int)(rddif - refdif) : 0);
-            int dellen = (del ? (int)(refdif - rddif) : 0);
-            int64_t gap_penalty;
-            if (ins) gap_penalty = -((int64_t)(P->rfGapConst + P->rfGapLinear) + (int64_t)P->rfGapLinear * (inslen - 1));
-            else gap_penalty = -((int64_t)(P->rdGapConst + P->rdGapLinear) + (int64_t)P->rdGapLinear * (dellen - 1));
-            if (gap_penalty < remainsc) return false;
-            int i;
-            for (i = 0; i < (int)len; i++) {
-                int rdc = seq[this_rdoff + i], rfc = refbuf[i];
-                ts[i] = i > 0 ? ts[i - 1] : 0;
-                if (rdc != rfc) ts[i] += ht2_score(*P, rdc, 1 << rfc, (int)qual[this_rdoff + i] - 33);
-                if (ts[i] + gap_penalty < remainsc) break;
-            }
-            int i_limit = i < (int)len ? i : (int)len;
-            int i2;
-            for (i2 = (int)len - 1; i2 >= 0; i2--) {
-                int rdc = seq[this_rdoff + i2], rfc = refbuf2[i2];
-                ts2[i2] = ((uint32_t)(i2 + 1) < len) ? ts2[i2 + 1] : 0;
-                if (rdc != rfc) ts2[i2] += ht2_score(*P, rdc, 1 << rfc, (int)qual[this_rdoff + i2] - 33);
-                if (ts2[i2] + gap_penalty < remainsc) break;
-            }
-            int i2_limit = (i2 < inslen ? 0 : i2 - inslen);
-            for (i = i2_limit, i2 = i2_limit + 1 + inslen; i < i_limit && i2 < (int)len; i++, i2++) {
-                int64_t tempscore = ts[i] + ts2[i2] + gap_penalty;
-                if (maxscore < tempscore) { maxscore = tempscore; maxscorei = (uint32_t)i; }
-            }
-            if (maxscore == HT2_MIN_I64) return false;
-            if (maxscore < remainsc) return false;
-        }
+        if ((ins || del) && !gapJoinSplit(o.tidx, seq + this_rdoff, qual + this_rdoff, refbuf, len, other_toff + other_len, read_gaps,
+                                          ins ? (int)(rddif - refdif) : 0, ins ? 0 : (int)(refdif - rddif), remainsc, refbuf2, maxscorei))
+            return false;
         // drop this hit's trailing plain mismatches (hi_aligner.h:1818-1830)
         {
             bool clear = true;
@@ -1922,11 +1948,18 @@ struct Ht2AlignerT {
         r.editOff = W->nResEdits;
         W->nResEdits += hit.nedits;
         Ht2Edit* red = W->resEdits + r.editOff;
-        for (uint32_t i = 0; i < hit.nedits; i++) { red[i] = hit.edits[i]; red[i].pos += hit.trim5; }
-        if (!hit.fw) invertPoss(red, r.nedits, rdlen);
-        // AlnRes::setShape (aligner_result.cpp:111-129)
-        for (uint32_t i = 0; i < r.nedits; i++) red[i].pos -= r.trim5p;
+        moveEdits(red, hit.edits, hit.nedits);
+        // positions + trim5, Edit::invertPoss on the reverse strand, then - trim5p (AlnRes::setShape,
+        // aligner_result.cpp:111-129); on the forward strand trim5p is trim5 and the positions stay as they are
+        if (!hit.fw) {
+#pragma unroll 1
+            for (uint32_t i = 0; i < r.nedits; i++) red[i].pos += hit.trim5;
+            invertPoss(red, r.nedits, rdlen);
+#pragma unroll 1
+            for (uint32_t i = 0; i < r.nedits; i++) red[i].pos -= r.trim5p;
+        }
         uint32_t rfextent = rdlen - r.trim5p - r.trim3p;
+#pragma unroll 1
         for (uint32_t i = 0; i < r.nedits; i++) {
             if (red[i].type == HT2_EDIT_REF_GAP) rfextent--;
             else if (red[i].type == HT2_EDIT_READ_GAP) rfextent++;
@@ -1935,13 +1968,13 @@ struct Ht2AlignerT {
 #ifdef HT2_ENABLE_SPLICED
         {   // GenomeHit::spliced() -> AlnScore(..., splicescore, knownTranscripts, nearSpliceSites, ...) (hi_aligner.h:6100-6145)
             bool spl = false, known = true;
-            for (uint32_t i = 0; i < hit.nedits; i++) if (hit.edits[i].type == HT2_EDIT_SPL) { spl = true; known = known && ht2_spl_known(hit.edits[i]); }
+            for (uint32_t i = 0; i < hit.nedits; i++) if (isSpl(hit.edits[i])) { spl = true; known = known && ht2_spl_known(hit.edits[i]); }
             r.spliced = spl ? 1 : 0; r.knownTranscripts = (spl && known) ? 1 : 0; r.splicescore = hit.splicescore;
         }
 #endif
         {
             uint32_t nspl = 0;
-            for (uint32_t i = 0; i < hit.nedits; i++) if (hit.edits[i].type == HT2_EDIT_SPL) nspl++;
+            for (uint32_t i = 0; i < hit.nedits; i++) if (isSpl(hit.edits[i])) nspl++;
             reportUnpaired(slot, hit.score, nspl);
         }
         return true;
@@ -1959,7 +1992,7 @@ struct Ht2AlignerT {
                         // compare against hit.edits as Edit::invertPoss(edits, rdlen) would lay them out
                         Ht2Edit e = hit.fw ? hit.edits[eidx] : hit.edits[hit.nedits - eidx - 1];
                         if (!hit.fw) {
-                            if (e.type == HT2_EDIT_READ_GAP || e.type == HT2_EDIT_SPL) e.pos = (uint32_t)(rdlen - e.pos);
+                            if (e.type == HT2_EDIT_READ_GAP || isSpl(e)) e.pos = (uint32_t)(rdlen - e.pos);
                             else e.pos = (uint32_t)(rdlen - e.pos - 1);
                         }
                         if (!editEq(W->resEdits[rsi.editOff + eidx], e)) break;
@@ -1987,7 +2020,7 @@ struct Ht2AlignerT {
                 if (e.type == HT2_EDIT_READ_GAP) { if (oe.type != HT2_EDIT_READ_GAP) same = false; }
                 else if (e.type == HT2_EDIT_REF_GAP) { if (oe.type != HT2_EDIT_REF_GAP) same = false; }
 #ifdef HT2_ENABLE_SPLICED
-                else if (e.type == HT2_EDIT_SPL) {
+                else if (!NOSPL && e.type == HT2_EDIT_SPL) {
                     const uint32_t v = (ht2_spl_len(oe) & 0xfffffu) | (ht2_spl_dir(oe) << 20);
                     if (oe.type != HT2_EDIT_SPL || e.pos != oe.pos || e.chr != (uint8_t)v || e.qchr != (uint8_t)(v >> 8) || e.pad != (uint8_t)(v >> 16)) same = false;
                 }
@@ -2009,7 +2042,7 @@ struct Ht2AlignerT {
         for (uint32_t i = 0; i < hit.nedits; i++) {
             ed[i].pos = hit.edits[i].pos; ed[i].type = hit.edits[i].type; ed[i].chr = hit.edits[i].chr; ed[i].qchr = hit.edits[i].qchr; ed[i].pad = 0;
 #ifdef HT2_ENABLE_SPLICED
-            if (hit.edits[i].type == HT2_EDIT_SPL) {   // Edit::operator== compares splLen and splDir of splice edits (edit.h:195-210)
+            if (isSpl(hit.edits[i])) {   // Edit::operator== compares splLen and splDir of splice edits (edit.h:195-210)
                 const uint32_t v = (ht2_spl_len(hit.edits[i]) & 0xfffffu) | (ht2_spl_dir(hit.edits[i]) << 20);
                 ed[i].chr = (uint8_t)v; ed[i].qchr = (uint8_t)(v >> 8); ed[i].pad = (uint8_t)(v >> 16);
             }
@@ -2024,6 +2057,7 @@ struct Ht2AlignerT {
     HT2_NI int64_t searchScore(const Ht2ReadHits& h) const {
         int64_t score = 0;
         const int64_t penaltyPerOffset = (int64_t)P->minK * P->minK;
+#pragma unroll 1
         for (uint32_t i = 0; i < h.nhits; i++) { uint32_t len = h.hits[i].len; score += (int64_t)(uint32_t)(len * len); }
         uint32_t aps = h.numPartialSearch - h.numUniqueSearch;
         score -= (int64_t)aps * penaltyPerOffset;

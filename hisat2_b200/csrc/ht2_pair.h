@@ -52,8 +52,8 @@ template <bool GRAPH, bool NOSPL, bool DP> HT2_NI void Ht2AlignerT<GRAPH, NOSPL,
             int64_t left = r1.toff, right = (int64_t)r1.toff + r1.rfextent - 1;
             int64_t left2 = r2.toff, right2 = (int64_t)r2.toff + r2.rfextent - 1;
 #ifdef HT2_ENABLE_SPLICED   // AlnRes::refcoord_right adds the introns (aligner_result.h:1255-1268)
-            for (uint32_t e = 0; e < r1.nedits; e++) if (W->resEdits[r1.editOff + e].type == HT2_EDIT_SPL) right += ht2_spl_len(W->resEdits[r1.editOff + e]);
-            for (uint32_t e = 0; e < r2.nedits; e++) if (W->resEdits[r2.editOff + e].type == HT2_EDIT_SPL) right2 += ht2_spl_len(W->resEdits[r2.editOff + e]);
+            for (uint32_t e = 0; e < r1.nedits; e++) if (isSpl(W->resEdits[r1.editOff + e])) right += ht2_spl_len(W->resEdits[r1.editOff + e]);
+            for (uint32_t e = 0; e < r2.nedits; e++) if (isSpl(W->resEdits[r2.editOff + e])) right2 += ht2_spl_len(W->resEdits[r2.editOff + e]);
 #endif
             if ((r1.fw != 0) == (P->gMate1fw != 0)) {
                 if ((r2.fw != 0) != (P->gMate2fw != 0)) continue;
