@@ -73,7 +73,7 @@ class CSamResult(C.Structure):
     _fields_ = [("sam", C.c_void_p), ("sam_len", C.c_size_t), ("n_units", C.c_uint32), ("n_alns", C.c_uint32),
                 ("n_err_reads", C.c_uint32), ("n_launches", C.c_uint32),
                 ("ms_h2d", C.c_float), ("ms_align", C.c_float), ("ms_sam", C.c_float), ("ms_d2h", C.c_float),
-                ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64)]
+                ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("sam_unplanned", C.c_uint32), ("pad", C.c_uint32)]
 
 
 class CReadsInput(C.Structure):

@@ -538,26 +538,80 @@ ht2_seed_kernel(const uint8_t* __restrict__ blob, Ht2ParamsCore P, DevBatch b, u
 }
 
 // ---------------------------------------------------------------------------
-// The SAM back end on the device (ht2_sam.h).  One thread formats one unit (read or pair):
-//   ht2_sam_kernel<false> : counting pass -- bytes of SAM text per unit (lens) and per block (blk)
+// The SAM back end on the device (ht2_sam.h):
+//   ht2_sam_kernel<false> : counting pass, one thread per unit (read or pair) -- selects the unit's records
+//                           (finishPaired / finishUnpaired), stores them as plan records (Ht2SamRec) with their
+//                           bytes, and the bytes of SAM text per unit (lens) and per block (blk)
 //   ht2_sam_scan_kernel   : exclusive scan of the block sums (one block), blk[nBlk] = total
-//   ht2_sam_kernel<true>  : writing pass -- unit offset = block offset + in-block exclusive scan of lens
-// Records land in read order (= --reorder), exactly the bytes AlnSinkWrap::finishRead prints.
+//   ht2_sam_rec_kernel    : writing pass, one thread per plan record -- record offset = block offset + in-block
+//                           exclusive scan of lens + the record's offset in its unit
+//   ht2_sam_kernel<true>  : writing pass of a batch whose plan did not fit its arena, one thread per unit: selects
+//                           the unit's records again and prints each (offset = block offset + scan of lens)
+// Exactly one of the two writing passes does work; the other returns at once.  Records land in read order
+// (= --reorder), exactly the bytes AlnSinkWrap::finishRead prints.
 //
-// The block's units fill one contiguous byte range of the output, [blk[b], blk[b+1]).  The writing pass formats
+// The plan: a unit's first HT2_SAM_PLAN_INLINE records go to its own room (recs[HT2_SAM_PLAN_INLINE * u + k]), the
+// rest to the overflow arena at a range the unit claims with one atomic add; unitRecs[u] = (records, first arena
+// record).  An arena too small for the batch is never truncated: the counter ends above the capacity, and the
+// unit-per-thread writing pass runs instead.
+//
+// The block's units fill one contiguous byte range of the output, [blk[b], blk[b+1]).  A writing pass formats
 // them into shared memory at their in-block offsets and then copies the range out with aligned 16-byte stores:
-// one thread's text is a few hundred bytes long, so byte stores straight to global memory would have every store
+// one record is a few hundred bytes long, so byte stores straight to global memory would have every store
 // instruction touch 32 different sectors.  A block whose text does not fit the staging buffer (many multi-mapping
 // records, long reads) formats straight into global memory; the bytes are the same either way.
 // ---------------------------------------------------------------------------
-#define HT2_SAM_TPB 128
+#define HT2_SAM_TPB 128            // units per block of every SAM kernel
+#define HT2_SAM_REC_TPB 256        // threads per block of ht2_sam_rec_kernel: one per record of a concordant pair
 #define HT2_SAM_STAGE_BLOCKS 2     // writing-pass blocks per SM the staging buffer leaves room for
+#define HT2_SAM_PLAN_INLINE 2      // plan records per unit outside the overflow arena: a concordant pair, two unpaired mates
+
+struct Ht2SamPlan {
+    Ht2SamRec*    recs;        // HT2_SAM_PLAN_INLINE per unit
+    Ht2SamRec*    arena;       // the records of units with more
+    uint2*        unitRecs;    // per unit: (records, first arena record)
+    unsigned int* arenaUsed;   // arena records claimed; above arenaCap: the plan is incomplete
+    int64_t       arenaCap;    // -1: no plan is complete
+    __device__ bool complete() const { return (int64_t)*(volatile const unsigned int*)arenaUsed <= arenaCap; }
+};
+
+// The counting pass's sink: every record's bytes (appendMate without stores) and the record itself into the plan
+struct Ht2SamPlanSink {
+    const Ht2SamFmt* F;
+    const Ht2SamPlan* P;
+    uint32_t u, n, k, first;    // the unit, its bytes so far, its records so far, its first arena record
+    __device__ void begin(uint32_t cnt) {
+        first = cnt > HT2_SAM_PLAN_INLINE ? atomicAdd(P->arenaUsed, cnt - HT2_SAM_PLAN_INLINE) : 0;
+        P->unitRecs[u] = make_uint2(cnt, first);
+    }
+    __device__ void rec(Ht2SamRec r) {
+        r.off = n;
+        r.len = F->appendMate<false>(NULL, r);
+        n += r.len;
+        if (k < HT2_SAM_PLAN_INLINE) P->recs[(size_t)HT2_SAM_PLAN_INLINE * u + k] = r;
+        else if ((int64_t)(first + (k - HT2_SAM_PLAN_INLINE)) < P->arenaCap) P->arena[first + (k - HT2_SAM_PLAN_INLINE)] = r;
+        k++;
+    }
+};
+
+// The staged text of a block, [head, end) of stage, to dst + [head, end) with aligned 16-byte stores (dst 16-aligned)
+template <uint32_t TPB>
+__device__ __forceinline__ void ht2_sam_copy_out(char* dst, const uint4* sStage, uint32_t head, uint32_t end)
+{
+    const char* stage = (const char*)sStage;
+    for (uint32_t lo = threadIdx.x * 16; lo < end; lo += TPB * 16) {
+        if (lo >= head && lo + 16 <= end) *(uint4*)(dst + lo) = sStage[lo / 16];
+        else for (uint32_t i = lo < head ? head : lo; i < end && i < lo + 16; i++) dst[i] = stage[i];
+    }
+}
 
 template <bool WRITE>
 __global__ void __launch_bounds__(HT2_SAM_TPB)
-ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigned long long* __restrict__ blk, char* __restrict__ out,
-               unsigned long long cap, unsigned int* counters, unsigned long long* __restrict__ tally, uint32_t stageBytes)
+ht2_sam_kernel(Ht2SamIn in, uint32_t units, Ht2SamPlan plan, uint32_t* __restrict__ lens, unsigned long long* __restrict__ blk,
+               char* __restrict__ out, unsigned long long cap, unsigned int* counters, unsigned long long* __restrict__ tally,
+               uint32_t stageBytes)
 {
+    if (WRITE && plan.complete()) return;   // ht2_sam_rec_kernel writes the batch
     extern __shared__ uint4 sStage[];   // writing pass: stageBytes of dynamic shared memory
     __shared__ unsigned long long sWarp[HT2_SAM_TPB / 32];
     __shared__ uint32_t sTally[HT2_SAM_TPB / 32][HT2_T_N];
@@ -571,10 +625,10 @@ ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigne
 #pragma unroll
         for (int k = 0; k < HT2_T_N; k++) t.c[k] = 0;
         if (u < units) {
-            Ht2SamOut<false> o; o.p = NULL; o.n = 0;
-            F.unit(o, u, &t);
-            mine = o.n;
-            lens[u] = (uint32_t)o.n;
+            Ht2SamPlanSink s = {&F, &plan, u, 0, 0, 0};
+            F.plan(s, u, &t);
+            mine = s.n;
+            lens[u] = s.n;
             if (in.reads[u].err) atomicAdd(&counters[4], 1u);
         }
         // ReportingMetrics of the block: warp sums, then one 64-bit atomic per counter per block
@@ -614,12 +668,59 @@ ht2_sam_kernel(Ht2SamIn in, uint32_t units, uint32_t* __restrict__ lens, unsigne
     }
     if (!staged) return;
     __syncthreads();
-    char* const dst = out + (b0 - head);   // out is 16-byte aligned (cudaMalloc)
-    const uint32_t end = head + (uint32_t)(b1 - b0);
-    for (uint32_t lo = threadIdx.x * 16; lo < end; lo += HT2_SAM_TPB * 16) {
-        if (lo >= head && lo + 16 <= end) *(uint4*)(dst + lo) = sStage[lo / 16];
-        else for (uint32_t i = lo < head ? head : lo; i < end && i < lo + 16; i++) dst[i] = stage[i];
+    ht2_sam_copy_out<HT2_SAM_TPB>(out + (b0 - head), sStage, head, head + (uint32_t)(b1 - b0));   // out is 16-byte aligned (cudaMalloc)
+}
+
+// The writing pass over the plan: block b prints the records of the units of counting block b, one thread per record
+__global__ void __launch_bounds__(HT2_SAM_REC_TPB)
+ht2_sam_rec_kernel(Ht2SamIn in, uint32_t units, Ht2SamPlan plan, const uint32_t* __restrict__ lens,
+                   const unsigned long long* __restrict__ blk, char* __restrict__ out, unsigned long long cap, uint32_t stageBytes)
+{
+    if (!plan.complete()) return;   // ht2_sam_kernel<true> writes the batch
+    extern __shared__ uint4 sStage[];
+    __shared__ uint32_t sOff[HT2_SAM_TPB];        // the unit's first byte in the block's text
+    __shared__ uint32_t sRec[HT2_SAM_TPB + 1];    // the unit's first record in the block's records; [HT2_SAM_TPB] = all
+    __shared__ uint32_t sFirst[HT2_SAM_TPB];      // the unit's first arena record
+    __shared__ uint32_t sWarp[2][HT2_SAM_TPB / 32];
+    const uint32_t t = threadIdx.x, lane = t & 31, wib = t >> 5;
+    const uint32_t u0 = blockIdx.x * HT2_SAM_TPB;
+    // exclusive scans of the block's unit bytes and unit records
+    uint32_t nb = 0, nr = 0, ib = 0, ir = 0;
+    if (t < HT2_SAM_TPB) {
+        if (u0 + t < units) { nb = lens[u0 + t]; const uint2 ur = plan.unitRecs[u0 + t]; nr = ur.x; sFirst[t] = ur.y; }
+        ib = nb; ir = nr;
+        for (int off = 1; off < 32; off <<= 1) {
+            const uint32_t vb = __shfl_up_sync(0xffffffffu, ib, off), vr = __shfl_up_sync(0xffffffffu, ir, off);
+            if ((int)lane >= off) { ib += vb; ir += vr; }
+        }
+        if (lane == 31) { sWarp[0][wib] = ib; sWarp[1][wib] = ir; }
     }
+    __syncthreads();
+    if (t < HT2_SAM_TPB) {
+        for (uint32_t w = 0; w < wib; w++) { ib += sWarp[0][w]; ir += sWarp[1][w]; }
+        sOff[t] = ib - nb; sRec[t] = ir - nr;
+        if (t == HT2_SAM_TPB - 1) sRec[HT2_SAM_TPB] = ir;
+    }
+    __syncthreads();
+    const unsigned long long b0 = blk[blockIdx.x], b1 = blk[blockIdx.x + 1];
+    const uint32_t head = (uint32_t)(b0 & 15);
+    const bool staged = b1 <= cap && b1 - b0 + head <= stageBytes;   // the same for the whole block
+    Ht2SamFmt F;
+    F.bind(&in);
+    const uint32_t nRec = sRec[HT2_SAM_TPB];
+    for (uint32_t r = t; r < nRec; r += HT2_SAM_REC_TPB) {
+        uint32_t lo = 0, hi = HT2_SAM_TPB - 1;   // the record's unit: the last one whose first record is at or before r
+        while (lo < hi) { const uint32_t m = (lo + hi + 1) >> 1; if (sRec[m] <= r) lo = m; else hi = m - 1; }
+        const uint32_t k = r - sRec[lo];
+        const Ht2SamRec& rec = k < HT2_SAM_PLAN_INLINE ? plan.recs[(size_t)HT2_SAM_PLAN_INLINE * (u0 + lo) + k]
+                                                       : plan.arena[sFirst[lo] + (k - HT2_SAM_PLAN_INLINE)];
+        const uint32_t at = sOff[lo] + rec.off;   // in the block
+        if (staged) F.appendMate<true>((char*)sStage + head + at, rec);
+        else if (b0 + at + rec.len <= cap) F.appendMate<true>(out + b0 + at, rec);
+    }
+    if (!staged) return;
+    __syncthreads();
+    ht2_sam_copy_out<HT2_SAM_REC_TPB>(out + (b0 - head), sStage, head, head + (uint32_t)(b1 - b0));
 }
 
 __global__ void __launch_bounds__(1024)
@@ -691,6 +792,9 @@ struct SamSlot {
     DevBuf<uint32_t> dPairs;                      // one pair: the two uint16_t alignment indexes of ht2gpu_result_batch_t.pairs
     DevBuf<unsigned int> dCounters;
     DevBuf<uint32_t> dSamLen;                     // bytes of SAM text per unit
+    DevBuf<Ht2SamRec> dPlanRecs, dPlanArena;      // the batch's SAM plan (Ht2SamPlan): HT2_SAM_PLAN_INLINE records per unit, overflow
+    DevBuf<uint2> dUnitRecs;                      // ... per unit: (records, first arena record)
+    int64_t arenaCap = 0;                         // ... arena records the counting pass may fill (counter in dCounters[5])
     DevBuf<unsigned long long> dBlk;              // per-block sums, then exclusive block offsets; [nBlk] = total
     DevBuf<char> dSam;
     DevBuf<Ht2SsRec> dColRecs;                    // --novel-splicesite-outfile: junction records of the batch (count in dCounters[6])
@@ -960,17 +1064,22 @@ static int setKernelLimits(ht2gpu_handle* h)
     cudaFuncAttributes fa;
     if (h->graph) { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, true, false, true>)); need = fa.localSizeBytes + 36 * 1024; }
     else { CK(cudaFuncGetAttributes(&fa, ht2_align_pool_kernel<8, 4, false, false, true>)); need = fa.localSizeBytes + 4 * 1024; }
-    CK(cudaFuncGetAttributes(&fa, ht2_sam_kernel<true>));
-    if (fa.localSizeBytes + 2048 > need) need = fa.localSizeBytes + 2048;
-    // the writing pass's staging buffer: what leaves room for HT2_SAM_STAGE_BLOCKS blocks per SM (1 KB of every
-    // block's shared memory is reserved by the system)
+    // the writing passes' staging buffer: what leaves room for HT2_SAM_STAGE_BLOCKS blocks per SM (1 KB of every
+    // block's shared memory is reserved by the system) beside the larger static shared memory of the two
+    size_t statSmem = 0;
+    for (const void* k : {(const void*)ht2_sam_kernel<true>, (const void*)ht2_sam_rec_kernel}) {
+        CK(cudaFuncGetAttributes(&fa, k));
+        if (fa.localSizeBytes + 2048 > need) need = fa.localSizeBytes + 2048;
+        if (fa.sharedSizeBytes > statSmem) statSmem = fa.sharedSizeBytes;
+    }
     int smemSM = 0, smemBlk = 0;
     CK(cudaDeviceGetAttribute(&smemSM, cudaDevAttrMaxSharedMemoryPerMultiprocessor, h->device));
     CK(cudaDeviceGetAttribute(&smemBlk, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-    size_t stage = (size_t)smemSM / HT2_SAM_STAGE_BLOCKS - 1024 - fa.sharedSizeBytes;
-    if (stage > (size_t)smemBlk - fa.sharedSizeBytes) stage = (size_t)smemBlk - fa.sharedSizeBytes;
+    size_t stage = (size_t)smemSM / HT2_SAM_STAGE_BLOCKS - 1024 - statSmem;
+    if (stage > (size_t)smemBlk - statSmem) stage = (size_t)smemBlk - statSmem;
     h->samStage = (uint32_t)(stage & ~(size_t)15);
     CK(cudaFuncSetAttribute(ht2_sam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->samStage));
+    CK(cudaFuncSetAttribute(ht2_sam_rec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->samStage));
     size_t cur = 0;
     CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
     if (cur < need) CK(cudaDeviceSetLimit(cudaLimitStackSize, need));
@@ -1404,36 +1513,57 @@ static Ht2SamIn samIn(const ht2gpu_handle* h, const SamSlot& S)
 }
 
 // Enqueue [align, SAM count, block scan, SAM write] for the slot's uploaded batch.  withAlign = false re-runs
-// only the SAM kernels (after the text buffer was grown).
+// only the writing passes, from the batch's plan (after the text buffer was grown).
 static int enqueueKernels(ht2gpu_handle* h, SamSlot& S, bool withAlign)
 {
     const uint32_t units = S.units;
     const uint32_t nBlk = (units + HT2_SAM_TPB - 1) / HT2_SAM_TPB;
     CK(S.dSamLen.reserve(units));
     CK(S.dBlk.reserve((size_t)nBlk + 2));
+    if (withAlign) {
+        // The overflow arena: a unit prints at most 2 * min(khits, HT2_SAM_MAXSEL) records, but nearly every unit
+        // prints at most HT2_SAM_PLAN_INLINE; room for half a record more per unit on average keeps the plan's memory
+        // a tenth of the text's.  HT2GPU_SAM_PLAN_ARENA=<records> sets another capacity, -1 none at all (tests of the
+        // unit-per-thread writing pass).
+        const int64_t perUnit = 2 * (int64_t)(h->P.khits < HT2_SAM_MAXSEL ? h->P.khits : HT2_SAM_MAXSEL);
+        int64_t cap = perUnit > HT2_SAM_PLAN_INLINE ? std::min<int64_t>((int64_t)units * (perUnit - HT2_SAM_PLAN_INLINE), units / 2 + 1024) : 0;
+        if (const char* e = getenv("HT2GPU_SAM_PLAN_ARENA")) cap = std::max<int64_t>(strtoll(e, NULL, 10), -1);
+        S.arenaCap = std::min<int64_t>(cap, 0x7fffffff);
+        CK(S.dPlanRecs.reserve((size_t)units * HT2_SAM_PLAN_INLINE));
+        CK(S.dPlanArena.reserve((size_t)std::max<int64_t>(S.arenaCap, 0)));
+        CK(S.dUnitRecs.reserve(units));
+    }
     if (h->collectSs) CK(S.dColRecs.reserve((size_t)S.batch.n_reads * 4 + 1024, 1, 1));
     if (h->recordOut) {
         CK(S.dOut.reserve(units));
         CK(S.hOut.reserve(units));
     }
+    Ht2SamPlan plan;
+    plan.recs = S.dPlanRecs; plan.arena = S.dPlanArena; plan.unitRecs = S.dUnitRecs; plan.arenaUsed = S.dCounters + 5; plan.arenaCap = S.arenaCap;
     std::lock_guard<std::mutex> lk(h->pool->mu);
     CK(cudaStreamWaitEvent(S.stream, h->pool->evDone, 0));
-    if (withAlign) { int rc = launchAlign(h, S, &S.batch, units, S.ev[EV_ALIGN_START]); if (rc) return rc; S.nLaunch++; }
+    if (withAlign) { int rc = launchAlign(h, S, &S.batch, units, S.ev[EV_ALIGN_START]); if (rc) return rc; S.nLaunch++; }   // zeroes dCounters
     else CK(cudaEventRecord(S.ev[EV_ALIGN_START], S.stream));
     CK(cudaEventRecord(S.ev[EV_ALIGN_END], S.stream));
-    if (h->collectSs) CK(cudaMemsetAsync(S.dCounters + 6, 0, sizeof(unsigned int), S.stream));
-    // the counting pass tallies the batch's ReportingMetrics; a re-run (ht2gpu_wait_sam) must not count it twice
-    CK(cudaMemsetAsync(S.dTally, 0, HT2_T_N * sizeof(unsigned long long), S.stream));
     const Ht2SamIn in = samIn(h, S);
     if (S.evSplit[0]) CK(cudaEventRecord(S.evSplit[0], S.stream));
-    ht2_sam_kernel<false><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, S.dSamLen, S.dBlk, NULL, 0, S.dCounters, S.dTally, 0);
-    if (S.evSplit[1]) CK(cudaEventRecord(S.evSplit[1], S.stream));
-    ht2_sam_scan_kernel<<<1, 1024, 0, S.stream>>>(S.dBlk, nBlk);
+    if (withAlign) {
+        // the counting pass tallies the batch's ReportingMetrics once; a re-run of the writing passes keeps them
+        CK(cudaMemsetAsync(S.dTally, 0, HT2_T_N * sizeof(unsigned long long), S.stream));
+        ht2_sam_kernel<false><<<nBlk, HT2_SAM_TPB, 0, S.stream>>>(in, units, plan, S.dSamLen, S.dBlk, NULL, 0, S.dCounters, S.dTally, 0);
+        if (S.evSplit[1]) CK(cudaEventRecord(S.evSplit[1], S.stream));
+        ht2_sam_scan_kernel<<<1, 1024, 0, S.stream>>>(S.dBlk, nBlk);
+        S.nLaunch += 2;
+    } else if (S.evSplit[1]) CK(cudaEventRecord(S.evSplit[1], S.stream));
     if (S.evSplit[2]) CK(cudaEventRecord(S.evSplit[2], S.stream));
-    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, h->samStage, S.stream>>>(in, units, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.dSam.cap, S.dCounters,
-                                                                        S.dTally, h->samStage);
+    // the junctions of the printed records are collected by the writing pass that prints them
+    if (h->collectSs) CK(cudaMemsetAsync(S.dCounters + 6, 0, sizeof(unsigned int), S.stream));
+    ht2_sam_rec_kernel<<<nBlk, HT2_SAM_REC_TPB, h->samStage, S.stream>>>(in, units, plan, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.dSam.cap,
+                                                                         h->samStage);
+    ht2_sam_kernel<true><<<nBlk, HT2_SAM_TPB, h->samStage, S.stream>>>(in, units, plan, S.dSamLen, S.dBlk, S.dSam, (unsigned long long)S.dSam.cap,
+                                                                        S.dCounters, S.dTally, h->samStage);
     CK(cudaGetLastError());
-    S.nLaunch += 3;
+    S.nLaunch += 2;
     CK(cudaEventRecord(S.ev[EV_SAM_END], S.stream));
     CK(cudaEventRecord(h->pool->evDone, S.stream));
     // meta: total SAM bytes, result counters, reads with errors
@@ -1536,16 +1666,18 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
         for (int k = 0; k < HT2_T_N; k++) tot[k] += S.hMeta[HT2_META_TALLY + k];
     }
     if (h->dStats) dumpStats(h);
-    if (S.evSplit[0]) {   // HT2GPU_SAM_SPLIT=1: the three SAM kernels of the batch's last SAM pass (investigation aid)
+    const unsigned int* c = (const unsigned int*)&S.hMeta[1];
+    const bool planned = (int64_t)c[5] <= S.arenaCap;
+    if (S.evSplit[0]) {   // HT2GPU_SAM_SPLIT=1: the SAM kernels of the batch's last SAM pass (investigation aid; count and scan
+                          // are 0 after a re-run of the writing passes alone)
         float ms[3];
         CK(cudaEventElapsedTime(&ms[0], S.evSplit[0], S.evSplit[1]));
         CK(cudaEventElapsedTime(&ms[1], S.evSplit[1], S.evSplit[2]));
         CK(cudaEventElapsedTime(&ms[2], S.evSplit[2], S.ev[EV_SAM_END]));
-        fprintf(stderr, "sam kernels: count %.3f ms  scan %.3f ms  write %.3f ms  total %.3f ms  |  %zu bytes of SAM, %u units  |  "
-                "%.1f GB/s over the three, %.1f GB/s over the writing pass\n", ms[0], ms[1], ms[2], ms[0] + ms[1] + ms[2], total, S.units,
-                total / ((ms[0] + ms[1] + ms[2]) * 1e6), total / (ms[2] * 1e6));
+        fprintf(stderr, "sam kernels: count %.3f ms  scan %.3f ms  write %.3f ms (%s)  total %.3f ms  |  %zu bytes of SAM, %u units  |  "
+                "%.1f GB/s over the three, %.1f GB/s over the writing pass\n", ms[0], ms[1], ms[2], planned ? "one thread per record" : "one thread per unit",
+                ms[0] + ms[1] + ms[2], total, S.units, total / ((ms[0] + ms[1] + ms[2]) * 1e6), total / (ms[2] * 1e6));
     }
-    const unsigned int* c = (const unsigned int*)&S.hMeta[1];
     S.outValid = h->recordOut;
     out->sam = S.hSam; out->sam_len = total;
     out->n_alns = c[0]; out->n_err_reads = c[4];
@@ -1555,6 +1687,7 @@ extern "C" int ht2gpu_wait_sam(ht2gpu_handle_t* h, int slot, ht2gpu_sam_result_t
     CK(cudaEventElapsedTime(&out->ms_d2h, S.ev[EV_SAM_END], S.ev[EV_COPIED]));
     out->h2d_bytes = S.h2dBytes; out->d2h_bytes = total + 9 * sizeof(unsigned long long) + (h->recordOut ? S.units : 0);
     out->n_launches = S.nLaunch;
+    out->sam_unplanned = !planned;
     if (c[4]) {
         char buf[160]; snprintf(buf, sizeof(buf), "device capacity exceeded for %u read(s) of the batch; their SAM records are unreliable", c[4]);
         h->err = buf;

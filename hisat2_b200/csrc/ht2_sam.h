@@ -1,7 +1,7 @@
 // ht2_sam.h -- the SAM back end of one read (pair): AlnSinkWrap::finishRead, allocation-free, host + device.
 //
-// One source serves the device kernel (ht2_sam_kernel in ht2_gpu.cu: one thread per unit, a counting pass
-// and a writing pass) and the host entry points (ht2gpu_format_sam, tests/hostsim).  It turns the flat result
+// One source serves the device kernels (ht2_gpu.cu: a counting pass that plans each unit's records, and a writing
+// pass that prints one plan record per thread) and the host entry points (ht2gpu_format_sam, tests/hostsim).  It turns the flat result
 // records of the alignment kernel (ht2gpu_read_result_t / ht2gpu_aln_t / ht2gpu_edit_t) plus the read batch
 // into the reference's SAM records, byte for byte:
 //   AlnSinkWrap::finishRead            aln_sink.h:1939-2560   (concordant > discordant > unpaired > unaligned)
@@ -209,11 +209,10 @@ struct Ht2SamSumm {   // AlnSetSumm (aligner_result.cpp:1167-1260)
     Ht2SamKey best[2], secbest[2], bestPaired, secbestPaired;
     bool paired;
     uint32_t numAlns[2], numAlnsPaired;
-    int64_t orefid, orefoff;
     HT2_HD void reset() {
         best[0].valid = best[1].valid = secbest[0].valid = secbest[1].valid = false;
         bestPaired.valid = secbestPaired.valid = false;
-        paired = false; numAlns[0] = numAlns[1] = numAlnsPaired = 0; orefid = -1; orefoff = -1;
+        paired = false; numAlns[0] = numAlns[1] = numAlnsPaired = 0;
     }
 };
 
@@ -229,10 +228,36 @@ struct Ht2SamFlags {
     HT2_HD bool unpairedMate() const { return pairing == HT2_PAIR_UNPAIRED_MATE1 || pairing == HT2_PAIR_UNPAIRED_MATE2; }
 };
 
+// One SAM record as finishPaired / finishUnpaired decide it: the alignment to print and every value of the record
+// that depends on the rest of the unit (selection, AlnSetSumm, MAPQ, fragment length, the read's filters).  What
+// follows from the alignment alone (CIGAR, MD:Z, AS / XM / XO / XG / NM, XS:A, Zs:Z) and from the read (QNAME,
+// SEQ, QUAL) is left to appendMate.  The device's counting pass stores these records and the writing pass prints
+// them one per thread (ht2_gpu.cu); the host prints each one as it is planned.
+#define HT2_SAM_NONE 0xffffffffu
+enum { HT2_REC_PRIMARY = 1, HT2_REC_OPP_ALIGNED = 2, HT2_REC_ZS = 4, HT2_REC_YS = 8 };
+enum { HT2_REC_YF_NONE, HT2_REC_YF_LN, HT2_REC_YF_NS, HT2_REC_YF_SC };
+struct Ht2SamRec {
+    int64_t  tlen;      // TLEN (0 when the fragment length is not set)
+    uint32_t read;      // the read's index in the batch
+    uint32_t ai;        // in->alns index of the printed alignment, or HT2_SAM_NONE: an unaligned record
+    uint32_t oi;        // aligned: the opposite mate's alignment (RNEXT, PNEXT, flag 0x20, YS:i) or HT2_SAM_NONE;
+                        // unaligned: the alignment whose RNAME / POS it takes (AlnSetSumm::orefid / orefoff) or HT2_SAM_NONE
+    int32_t  zs;        // ZS:i (HT2_REC_ZS): the second-best score of the read's mate
+    uint32_t nh;        // NH:i
+    uint32_t off;       // the record's first byte in its unit's text (device plan only)
+    uint32_t len;       // the record's bytes (device plan only)
+    uint8_t  pairing;   // HT2_PAIR_*
+    uint8_t  mapq;
+    uint8_t  bits;      // HT2_REC_*
+    uint8_t  yf;        // HT2_REC_YF_*
+};
+static_assert(sizeof(Ht2SamRec) == 40, "Ht2SamRec is a 40-byte plan record");
+
 // One read of the batch as the formatter sees it.
 struct Ht2SamRead {
     const uint8_t* seq; const uint8_t* qual; const char* name;
     uint32_t len; int mate;            // 0 unpaired, 1, 2
+    uint32_t idx;                      // the read's index in the batch
     uint8_t lenfilt, nfilt, scfilt;    // 1 = passes (hisat2.cpp:3417-3440)
 };
 
@@ -252,12 +277,15 @@ struct Ht2SamFmt {
     }
     HT2_HD int64_t minscOf(uint32_t len) const { return in->minscTab[len <= HT2_PARAMS_MAX_RDLEN ? len : HT2_PARAMS_MAX_RDLEN]; }
 
-    HT2_HD void mkRead(uint32_t i, int mate, Ht2SamRead& rd) const {
+    HT2_HD void readAt(uint32_t i, Ht2SamRead& rd) const {
         const uint64_t o0 = in->offs[i];
         rd.seq = in->seq + o0; rd.qual = in->qual ? in->qual + o0 : NULL;
         rd.len = (uint32_t)(in->offs[i + 1] - o0);
         rd.name = in->names + in->nameOffs[i];
-        rd.mate = mate;
+    }
+    HT2_HD void mkRead(uint32_t i, int mate, Ht2SamRead& rd) const {
+        readAt(i, rd);
+        rd.idx = i; rd.mate = mate;
         // ht2_filters (hisat2.cpp:3417-3440; Scoring::nFilter)
         int64_t m = minscOf(rd.len); if (m > 0) m = 0;
         const uint32_t maxns = (uint32_t)ht2_nceil(in->minscTab + HT2_PARAMS_NCEIL, rd.len);
@@ -536,10 +564,10 @@ struct Ht2SamFmt {
         else if (fw) o.run(n, fwQual, fwQual4);
         else o.run(n, rcQual, rcQual4);
     }
-    template <bool W> HT2_HD void putYF(Ht2SamCur<W>& o, const Ht2SamRead& rd) const {
-        if (!rd.lenfilt) o.s("\tYF:Z:LN");
-        else if (!rd.nfilt) o.s("\tYF:Z:NS");
-        else if (!rd.scfilt) o.s("\tYF:Z:SC");
+    template <bool W> HT2_HD void putYF(Ht2SamCur<W>& o, uint32_t yf) const {
+        if (yf == HT2_REC_YF_LN) o.s("\tYF:Z:LN");
+        else if (yf == HT2_REC_YF_NS) o.s("\tYF:Z:NS");
+        else if (yf == HT2_REC_YF_SC) o.s("\tYF:Z:SC");
     }
     // the read group follows YT:Z / YF:Z and precedes XS:A / NH:i (sam.h:780, 1102)
     template <bool W> HT2_HD void putRG(Ht2SamCur<W>& o) const {
@@ -729,15 +757,15 @@ struct Ht2SamFmt {
         return o.n;
     }
 
-    // the fields of an unaligned record after FLAG
+    // the fields of an unaligned record after FLAG; oref = the alignment of AlnSetSumm::orefid / orefoff, or NULL
     template <bool W>
-    HT2_NI uint32_t putUnaligned(char* d, const Ht2SamRead& rd, const Ht2SamSumm& summ, const Ht2SamFlags& fl) const {
+    HT2_NI uint32_t putUnaligned(char* d, const Ht2SamRead& rd, const ht2gpu_aln_t* oref, const Ht2SamFlags& fl, uint32_t yf) const {
         Ht2SamCur<W> o = {d, 0};
-        if (summ.orefid != -1) { putRefName(o, (uint32_t)summ.orefid); o.c('\t'); o.i64(summ.orefoff + 1); o.s("\t0\t*\t=\t"); o.i64(summ.orefoff + 1); o.s("\t0\t"); }
+        if (oref) { putRefName(o, oref->tidx); o.c('\t'); o.i64((int64_t)oref->toff + 1); o.s("\t0\t*\t=\t"); o.i64((int64_t)oref->toff + 1); o.s("\t0\t"); }
         else o.s("*\t0\t0\t*\t*\t0\t0\t");
         putSeqQual(o, rd, true);
         putYT(o, fl);
-        putYF(o, rd);
+        putYF(o, yf);
         putRG(o);
         o.c('\n');
         return o.n;
@@ -820,13 +848,16 @@ struct Ht2SamFmt {
         return o.n;
     }
 
-    // AlnSinkSam::appendMate (aln_sink.h:3024-3250): one record at d; returns its length.  The common record (aligned,
-    // gapless, no ALTs) runs in this frame; gapped CIGAR / MD:Z, unaligned records, XS:A, Zs:Z and the junction
-    // collection are out of line.
+    // AlnSinkSam::appendMate (aln_sink.h:3024-3250): the text of plan record r at d; returns its length.  The common
+    // record (aligned, gapless, no ALTs) runs in this frame; gapped CIGAR / MD:Z, unaligned records, XS:A, Zs:Z and
+    // the junction collection are out of line.
     template <bool W>
-    HT2_NI uint32_t appendMate(char* d, const Ht2SamRead& rd, uint32_t ordlen, const ht2gpu_aln_t* rs, const ht2gpu_aln_t* rso,
-                               const Ht2SamSumm& summ, const Ht2SamFlags& fl, bool fraglenSet, int64_t fraglen, bool haveOscore) const {
-        if (rs == NULL && in->noUnal) return 0;
+    HT2_NI uint32_t appendMate(char* d, const Ht2SamRec& r) const {
+        Ht2SamRead rd; readAt(r.read, rd);
+        const Ht2SamFlags fl = {(int)r.pairing, (r.bits & HT2_REC_PRIMARY) != 0, (r.bits & HT2_REC_OPP_ALIGNED) != 0};
+        const bool mate1 = fl.pairing == HT2_PAIR_UNPAIRED || fl.readMate1();   // AlnRes::readMate1
+        const ht2gpu_aln_t* rs = r.ai != HT2_SAM_NONE ? in->alns + r.ai : NULL;
+        const ht2gpu_aln_t* rso = r.oi != HT2_SAM_NONE ? in->alns + r.oi : NULL;
         Ht2SamCur<W> o = {d, 0};
         const bool trunc = !in->noQnameTrunc;
         o.name(rd.name, fl.partOfPair(), trunc ? 255 : 0xffffffffu, trunc);
@@ -837,14 +868,14 @@ struct Ht2SamFmt {
             if (fl.concordant()) flag |= 2;
             if (!fl.oppAligned) flag |= 8;
             flag |= fl.readMate1() ? 64 : 128;
-            if (fl.oppAligned && rso != NULL && !rso->fw) flag |= 32;
+            if (fl.oppAligned && rs != NULL && rso != NULL && !rso->fw) flag |= 32;
         }
         if (!fl.primary) flag |= 256;
         if (rs != NULL && !rs->fw) flag |= 16;
         if (rs == NULL) flag |= 4;
         o.i64(flag);
         o.c('\t');
-        if (rs == NULL) return o.n + putUnaligned<W>(o.at(), rd, summ, fl);
+        if (rs == NULL) return o.n + putUnaligned<W>(o.at(), rd, rso, fl, r.yf);
         if (W && in->colCount != NULL) collectSites(rs, rd.len);   // AlnSinkSam::append (aln_sink.h:1571, 1579)
         const ht2gpu_edit_t* ed = in->edits + rs->edit_off;
         const uint32_t ned = rs->n_edits;
@@ -860,7 +891,7 @@ struct Ht2SamFmt {
         o.c('\t');
         o.i64((int64_t)rs->toff + 1);
         o.c('\t');
-        o.i64(mapqV2(summ, rd.mate < 2, rd.len, ordlen));
+        o.i64(r.mapq);
         o.c('\t');
         if (gapless) {
             if (trimLS > 0) { o.i64(trimLS); o.c('S'); }
@@ -874,14 +905,13 @@ struct Ht2SamFmt {
             o.i64((int64_t)(rso ? rso->toff : rs->toff) + 1);
             o.c('\t');
         } else o.s("*\t0\t");
-        o.i64(fraglenSet ? fraglen : 0);
+        o.i64(r.tlen);
         o.c('\t');
         if (!fl.primary && in->omitSecSeq) o.s("*\t*");
         else putSeqQual(o, rd, rs->fw != 0);
         // optional flags (sam.h:525-1010)
         o.s("\tAS:i:"); o.i64(rs->score);
-        const Ht2SamKey& sb = summ.secbest[rd.mate < 2 ? 0 : 1];
-        if (sb.valid) { o.s("\tZS:i:"); o.i64(sb.score); }
+        if (r.bits & HT2_REC_ZS) { o.s("\tZS:i:"); o.i64(r.zs); }
         o.s("\tXN:i:0");
         // counts exclude edits that are known ALTs (snpID < #alts, sam.h:574-647)
         uint32_t num_mm = 0, num_go = 0, num_gx = 0, NM = 0;
@@ -917,26 +947,50 @@ struct Ht2SamFmt {
             }
             o.i64((int64_t)(len_trimmed - prevEnd));
         } else o.n += putStacked<W>(o.at(), rd.seq, rd.len, rs, true);
-        if (summ.paired && haveOscore && rso) { o.s("\tYS:i:"); o.i64(rso->score); }
+        if (r.bits & HT2_REC_YS) { o.s("\tYS:i:"); o.i64(rso->score); }
         putYT(o, fl);
-        putYF(o, rd);
+        putYF(o, r.yf);
         putRG(o);
-        if (in->rnaStrandness) { o.s("\tXS:A:"); o.c(xsStrand(rd.mate < 2, rs->fw != 0)); }
+        if (in->rnaStrandness) { o.s("\tXS:A:"); o.c(xsStrand(mate1, rs->fw != 0)); }
 #ifdef HT2_ENABLE_SPLICED
         else if (spliced) { const char xs = xsSense(ed, ned); if (xs) { o.s("\tXS:A:"); o.c(xs); } }
 #else
         (void)spliced;
 #endif
         o.s("\tNH:i:");
-        if (fl.concordant() || fl.discordant()) o.i64(summ.numAlnsPaired);
-        else o.i64((fl.pairing == HT2_PAIR_UNPAIRED || fl.readMate1()) ? summ.numAlns[0] : summ.numAlns[1]);
+        o.i64(r.nh);
         if (nAlts > 0) o.n += putZs<W>(o.at(), rs, len_trimmed);
         o.c('\n');
         return o.n;
     }
 
-    // finishRead for an unpaired read (aln_sink.h:2213-2557, unpaired branches)
-    template <bool W> HT2_HD void finishUnpaired(Ht2SamCur<W>& o, uint32_t u, Ht2SamTally* t) const {
+    // The plan record of one appendMate call of AlnSinkWrap::finishRead (the reference's arguments: the read, the
+    // opposite mate's length, the alignment or NULL, the opposite alignment, the summary, the flags, the fragment
+    // length and whether YS:i is printed).  For an unaligned record, rso is the alignment of summ's orefid / orefoff.
+    HT2_HD Ht2SamRec mkRec(const Ht2SamRead& rd, uint32_t ordlen, const ht2gpu_aln_t* rs, const ht2gpu_aln_t* rso,
+                           const Ht2SamSumm& summ, const Ht2SamFlags& fl, int64_t tlen, bool haveOscore) const {
+        Ht2SamRec r;
+        r.tlen = tlen; r.read = rd.idx; r.off = 0; r.len = 0;
+        r.ai = rs ? (uint32_t)(rs - in->alns) : HT2_SAM_NONE;
+        r.oi = rso ? (uint32_t)(rso - in->alns) : HT2_SAM_NONE;
+        r.pairing = (uint8_t)fl.pairing;
+        r.bits = (fl.primary ? HT2_REC_PRIMARY : 0) | (fl.oppAligned ? HT2_REC_OPP_ALIGNED : 0);
+        r.yf = !rd.lenfilt ? HT2_REC_YF_LN : !rd.nfilt ? HT2_REC_YF_NS : !rd.scfilt ? HT2_REC_YF_SC : HT2_REC_YF_NONE;
+        r.mapq = 0; r.zs = 0; r.nh = 0;
+        if (rs) {
+            r.mapq = (uint8_t)mapqV2(summ, rd.mate < 2, rd.len, ordlen);
+            const Ht2SamKey& sb = summ.secbest[rd.mate < 2 ? 0 : 1];
+            if (sb.valid) { r.bits |= HT2_REC_ZS; r.zs = (int32_t)sb.score; }
+            if (summ.paired && haveOscore && rso) r.bits |= HT2_REC_YS;
+            if (fl.concordant() || fl.discordant()) r.nh = summ.numAlnsPaired;
+            else r.nh = (fl.pairing == HT2_PAIR_UNPAIRED || fl.readMate1()) ? summ.numAlns[0] : summ.numAlns[1];
+        }
+        return r;
+    }
+
+    // finishRead for an unpaired read (aln_sink.h:2213-2557, unpaired branches).  The sink takes begin(number of
+    // records) once and then each record (Ht2SamRec) in output order; records --no-unal drops are not planned.
+    template <class S> HT2_HD void finishUnpaired(S& sink, uint32_t u, Ht2SamTally* t) const {
         const ht2gpu_read_result_t& rr = in->reads[u];
         Ht2SamRead rd; mkRead(u, 0, rd);
         Ht2Rng rnd; rnd.last = rr.rng_state;
@@ -952,18 +1006,20 @@ struct Ht2SamFmt {
             const uint32_t nsel = selectByScore(rs, n, rd.len, NULL, 0, NULL, 0, false, nunpair1, sel, rnd);
             summ.numAlns[0] = nsel;
             if (t) { t->c[HT2_T_NUNP_UNI1] += (uint32_t)(nsel == 1); t->c[HT2_T_NUNP_UNI2] += (uint32_t)(nsel != 1); }   // aln_sink.h:2290-2299
+            sink.begin(nsel);
             for (uint32_t i = 0; i < nsel; i++) {
                 fl.primary = (i == 0);
-                o.n += appendMate<W>(o.at(), rd, 0, &rs[sel[i]], NULL, summ, fl, false, 0, false);
+                sink.rec(mkRec(rd, 0, &rs[sel[i]], NULL, summ, fl, 0, false));
             }
         } else {
             if (t) t->c[HT2_T_NUNP_0]++;
-            o.n += appendMate<W>(o.at(), rd, 0, NULL, NULL, summ, fl, false, 0, false);
+            sink.begin(in->noUnal ? 0 : 1);
+            if (!in->noUnal) sink.rec(mkRec(rd, 0, NULL, NULL, summ, fl, 0, false));
         }
     }
 
     // AlnSinkWrap::finishRead for a pair (aln_sink.h:1939-2557)
-    template <bool W> HT2_HD void finishPaired(Ht2SamCur<W>& o, uint32_t u, Ht2SamTally* t) const {
+    template <class S> HT2_HD void finishPaired(S& sink, uint32_t u, Ht2SamTally* t) const {
         const ht2gpu_read_result_t& rr = in->reads[u];
         if (t) { t->c[HT2_T_NREAD]++; t->c[HT2_T_NPAIRED]++; }
         Ht2SamRead rd1, rd2; mkRead(2 * u, 1, rd1); mkRead(2 * u + 1, 2, rd2);
@@ -1002,11 +1058,12 @@ struct Ht2SamFmt {
                 t->outcome = HT2GPU_OUTCOME_AL1 | HT2GPU_OUTCOME_AL2 | HT2GPU_OUTCOME_CONC;
             }
             Ht2SamFlags fl1 = {HT2_PAIR_CONCORD_MATE1, true, true}, fl2 = {HT2_PAIR_CONCORD_MATE2, true, true};
+            sink.begin(2 * nsel);
             for (uint32_t i = 0; i < nsel; i++) {
                 const ht2gpu_aln_t& a = rs1u[pairs[2 * sel[i]]]; const ht2gpu_aln_t& b = rs2u[pairs[2 * sel[i] + 1]];
                 fl1.primary = fl2.primary = (i == 0);
-                o.n += appendMate<W>(o.at(), rd1, rd2.len, &a, &b, summ, fl1, true, fragmentLength(a, b, true, true), true);
-                o.n += appendMate<W>(o.at(), rd2, rd1.len, &b, &a, summ, fl2, true, fragmentLength(b, a, false, true), true);
+                sink.rec(mkRec(rd1, rd2.len, &a, &b, summ, fl1, fragmentLength(a, b, true, true), true));
+                sink.rec(mkRec(rd2, rd1.len, &b, &a, summ, fl2, fragmentLength(b, a, false, true), true));
             }
             return;
         } else if (discordant) {
@@ -1021,8 +1078,9 @@ struct Ht2SamFmt {
             (void)selectByScore(rs1u, n1, rd1.len, rs2u, rd2.len, dp, 1, true, 1, sel, rnd);
             Ht2SamFlags fl1 = {HT2_PAIR_DISCORD_MATE1, true, true}, fl2 = {HT2_PAIR_DISCORD_MATE2, true, true};
             const bool sameRef = a.tidx == b.tidx; // setMateParams (aligner_result.h:1594-1618)
-            o.n += appendMate<W>(o.at(), rd1, rd2.len, &a, &b, summ, fl1, sameRef, sameRef ? fragmentLength(a, b, true) : 0, true);
-            o.n += appendMate<W>(o.at(), rd2, rd1.len, &b, &a, summ, fl2, sameRef, sameRef ? fragmentLength(b, a, false) : 0, true);
+            sink.begin(2);
+            sink.rec(mkRec(rd1, rd2.len, &a, &b, summ, fl1, sameRef ? fragmentLength(a, b, true) : 0, true));
+            sink.rec(mkRec(rd2, rd1.len, &b, &a, summ, fl2, sameRef ? fragmentLength(b, a, false) : 0, true));
             return;
         }
         uint64_t nunpair1 = 0, nunpair2 = 0;
@@ -1057,54 +1115,57 @@ struct Ht2SamFmt {
             t->c[HT2_T_NUNP_0_UNI2] += (uint32_t)(rep1 && nsel1 != 1) + (uint32_t)(rep2 && nsel2 != 1);
             t->outcome = (rep1 ? HT2GPU_OUTCOME_AL1 : 0) | (rep2 ? HT2GPU_OUTCOME_AL2 : 0);
         }
+        // aligned records of both mates, and an unaligned record for each mate without any (unless --no-unal)
+        const uint32_t nUnal = in->noUnal ? 0 : (uint32_t)!rep1 + (uint32_t)!rep2;
+        sink.begin(nsel1 + nsel2 + nUnal);
         Ht2SamFlags fl1 = {HT2_PAIR_UNPAIRED_MATE1, true, repRs2 != NULL}, fl2 = {HT2_PAIR_UNPAIRED_MATE2, true, repRs1 != NULL};
-        int64_t refid = -1, refoff = -1;
         if (rep1) {
             // AlnSink::reportHits (aln_sink.h:730-790)
             if (repRs2 != NULL) {
-                const ht2gpu_aln_t* r1pri = &rs1u[sel[0]]; const ht2gpu_aln_t* r2pri = &rs2u[sel2[0]];
-                o.n += appendMate<W>(o.at(), rd1, rd2.len, r1pri, r2pri, summ1, fl1, false, 0, false);
-                o.n += appendMate<W>(o.at(), rd2, rd1.len, r2pri, r1pri, summ1, fl2, false, 0, false);
+                sink.rec(mkRec(rd1, rd2.len, repRs1, repRs2, summ1, fl1, 0, false));
+                sink.rec(mkRec(rd2, rd1.len, repRs2, repRs1, summ1, fl2, 0, false));
                 fl1.primary = fl2.primary = false;
-                for (uint32_t i = 1; i < nsel1; i++) o.n += appendMate<W>(o.at(), rd1, rd2.len, &rs1u[sel[i]], r2pri, summ1, fl1, false, 0, false);
-                for (uint32_t i = 1; i < nsel2; i++) o.n += appendMate<W>(o.at(), rd2, rd1.len, &rs2u[sel2[i]], r1pri, summ1, fl2, false, 0, false);
+                for (uint32_t i = 1; i < nsel1; i++) sink.rec(mkRec(rd1, rd2.len, &rs1u[sel[i]], repRs2, summ1, fl1, 0, false));
+                for (uint32_t i = 1; i < nsel2; i++) sink.rec(mkRec(rd2, rd1.len, &rs2u[sel2[i]], repRs1, summ1, fl2, 0, false));
                 fl1.primary = fl2.primary = true;
             } else {
                 for (uint32_t i = 0; i < nsel1; i++) {
                     fl1.primary = (i == 0);
-                    o.n += appendMate<W>(o.at(), rd1, 0, &rs1u[sel[i]], NULL, summ1, fl1, false, 0, false);
+                    sink.rec(mkRec(rd1, 0, &rs1u[sel[i]], NULL, summ1, fl1, 0, false));
                 }
                 fl1.primary = true;
             }
-            refid = rs1u[sel[0]].tidx; refoff = rs1u[sel[0]].toff;
         }
         if (rep2 && !rep1) {
             for (uint32_t i = 0; i < nsel2; i++) {
                 fl2.primary = (i == 0);
-                o.n += appendMate<W>(o.at(), rd2, 0, &rs2u[sel2[i]], NULL, summ2, fl2, false, 0, false);
+                sink.rec(mkRec(rd2, 0, &rs2u[sel2[i]], NULL, summ2, fl2, 0, false));
             }
             fl2.primary = true;
-            refid = rs2u[sel2[0]].tidx; refoff = rs2u[sel2[0]].toff;
         }
-        if (nunpair1 == 0) {
+        if (!in->noUnal) {   // RNAME / POS of an unaligned mate: the other mate's primary alignment (orefid / orefoff)
             Ht2SamSumm s; s.reset();
-            if (nunpair2 > 0) { s.orefid = refid; s.orefoff = refoff; }
-            Ht2SamFlags fl = {HT2_PAIR_UNPAIRED_MATE1, true, repRs2 != NULL};
-            o.n += appendMate<W>(o.at(), rd1, 0, NULL, NULL, s, fl, false, 0, false);
-        }
-        if (nunpair2 == 0) {
-            Ht2SamSumm s; s.reset();
-            if (nunpair1 > 0) { s.orefid = refid; s.orefoff = refoff; }
-            Ht2SamFlags fl = {HT2_PAIR_UNPAIRED_MATE2, true, repRs1 != NULL};
-            o.n += appendMate<W>(o.at(), rd2, 0, NULL, NULL, s, fl, false, 0, false);
+            if (!rep1) { const Ht2SamFlags fl = {HT2_PAIR_UNPAIRED_MATE1, true, repRs2 != NULL}; sink.rec(mkRec(rd1, 0, NULL, repRs2, s, fl, 0, false)); }
+            if (!rep2) { const Ht2SamFlags fl = {HT2_PAIR_UNPAIRED_MATE2, true, repRs1 != NULL}; sink.rec(mkRec(rd2, 0, NULL, repRs1, s, fl, 0, false)); }
         }
     }
 
-    // t != NULL: also tally the unit's outcome (the counting pass)
+    // Every record of unit u through the sink; t != NULL: also tally the unit's outcome (the counting pass)
+    template <class S> HT2_HD void plan(S& sink, uint32_t u, Ht2SamTally* t) const {
+        if (in->paired) finishPaired(sink, u, t); else finishUnpaired(sink, u, t);
+        if (t && in->unitOut) in->unitOut[u] = (uint8_t)t->outcome;
+    }
+
+    // The sink that prints each record as it is planned (the host formatter; the device's unit-per-thread writing pass)
+    template <bool W> struct PrintSink {
+        const Ht2SamFmt* F; Ht2SamCur<W>* o;
+        HT2_HD void begin(uint32_t) {}
+        HT2_HD void rec(const Ht2SamRec& r) { o->n += F->template appendMate<W>(o->at(), r); }
+    };
     template <bool W> HT2_HD void unit(Ht2SamOut<W>& o, uint32_t u, Ht2SamTally* t = NULL) const {
         Ht2SamCur<W> c = {W ? o.p + o.n : NULL, 0};
-        if (in->paired) finishPaired(c, u, t); else finishUnpaired(c, u, t);
-        if (t && in->unitOut) in->unitOut[u] = (uint8_t)t->outcome;
+        PrintSink<W> s = {this, &c};
+        plan(s, u, t);
         o.n += c.n;
     }
 };

@@ -250,6 +250,8 @@ typedef struct {
     uint32_t n_launches;   /* kernels launched for this batch */
     float    ms_h2d, ms_align, ms_sam, ms_d2h;   /* CUDA events on the slot's stream */
     uint64_t h2d_bytes, d2h_bytes;
+    uint32_t sam_unplanned; /* 1: the batch's records did not fit the SAM plan's arena and were printed one unit per thread */
+    uint32_t pad;
 } ht2gpu_sam_result_t;
 
 int ht2gpu_sam_slots(const ht2gpu_handle_t* h);

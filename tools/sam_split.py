@@ -4,9 +4,10 @@
   python tools/sam_split.py [--pairs 2000000] [--index tests/golden/tiny] [--repeat 3]
 
 Aligns one batch of bench.py's synthetic 2x101-bp pairs (the same generator and seed, default options) with
-HT2GPU_SAM_SPLIT=1, which makes the library print, after every batch, the CUDA-event time of each of the three SAM
-kernels (counting pass ht2_sam_kernel<false>, block scan ht2_sam_scan_kernel, writing pass ht2_sam_kernel<true>),
-the batch's SAM bytes and the bytes per second.  A first, unmeasured pass warms the kernels up; --repeat measured
+HT2GPU_SAM_SPLIT=1, which makes the library print, after every batch, the CUDA-event time of each SAM step (counting
+pass ht2_sam_kernel<false>, block scan ht2_sam_scan_kernel, writing pass: ht2_sam_rec_kernel over the plan, or
+ht2_sam_kernel<true> when the plan did not fit its arena -- the line names which one worked; the other returns at
+once and its launch is part of the writing time), the batch's SAM bytes and the bytes per second.  A first, unmeasured pass warms the kernels up; --repeat measured
 passes follow.  The card's name and power limit are printed first: times are only comparable on the same card and
 limit.
 """
