@@ -724,7 +724,9 @@ class Index(object):
         return np.frombuffer(C.string_at(p.value, n.value), dtype=np.uint8).copy() if n.value else np.zeros(0, np.uint8)
 
     def load_splicesites(self, known=None, novel=None):
-        """ht2gpu_load_splicesites: --known-splicesite-infile / --novel-splicesite-infile; returns the number of sites kept."""
+        """ht2gpu_load_splicesites: --known-splicesite-infile / --novel-splicesite-infile; returns the number of sites kept.
+        On an index built with splice sites / exons (_tran, _snp_tran) the index's own sites come first and the files'
+        sites are added to them; with neither file the DB is the index's again (empty on other indexes)."""
         n = C.c_uint32(0)
         self._check(self._lib.ht2gpu_load_splicesites(self._h, known.encode() if known else None, novel.encode() if novel else None, C.byref(n)),
                     "ht2gpu_load_splicesites")

@@ -2,10 +2,15 @@
 // struct Ht2AlignerT (ht2_core.h); everything here is a member.
 //
 // Restates GenomeHit::alignWithALTs / alignWithALTs_recur (hi_aligner.h:683-783, 2763-3550) for
-// SNP ALTs (single-base, deletion, insertion): a mismatch-bounded scan, then for every ALT in reach
-// of the scanned stretch a recursive continuation that consumes the ALT with a zero-penalty edit
-// carrying its id.  Haplotype filtering (off by default, hisat2.cpp:522), CODIS and splice-site ALTs
-// are not built; indexes holding splice-site / exon ALTs are refused at open.
+// SNP ALTs (single-base, deletion, insertion) and splice-site ALTs: a mismatch-bounded scan, then for
+// every ALT in reach of the scanned stretch a recursive continuation that consumes the ALT with a
+// zero-penalty edit carrying its id, or with a known splice edit across the site's intron.  Exon ALTs
+// are skipped there (they only feed the splice-site DB).  Haplotype filtering (off by default,
+// hisat2.cpp:522) and CODIS are not built.
+//
+// Under --no-spliced-alignment the reference drops the splice-site ALTs when it loads the index
+// (gfm.h:760-771).  The image keeps them, so that its ALT ids do not depend on options; every walk here
+// skips them instead (altSs), which visits the same ALTs in the same order.
 //
 // Scratch state of one alignWithALTs call lives in W->alt (Ht2AltScratch).
 #if !defined(__CUDA_ARCH__) && defined(HT2_TRACE)
@@ -24,6 +29,23 @@
         return lo;
     }
     HT2_HD static bool altIsSnp(const Ht2Alt& a) { return a.type == HT2_ALT_SNP_SGL || a.type == HT2_ALT_SNP_DEL || a.type == HT2_ALT_SNP_INS; }
+    // a splice-site ALT the run loaded (see above); altSsFw: the site as read (left < right), else its reversed copy
+    HT2_HD bool altSs(const Ht2Alt& a) const { return a.type == HT2_ALT_SPLICESITE && !noSpl(); }
+    HT2_HD bool altSsFw(const Ht2Alt& a) const { return altSs(a) && a.pos < a.len; }
+    // the known splice edit of a splice-site ALT [left, right] (hi_aligner.h:3030-3040, 3430-3440)
+    HT2_HD bool pushSsEdit(uint32_t pos, const Ht2Alt& a, uint32_t left, uint32_t right, bool front) {
+        const uint32_t intronLen = right - left + 1;
+        if (intronLen > HT2_MAX_SPL_LEN) { HT2_GERR(12); return false; }
+        Ht2Edit e = mkAltEdit(pos, 'A', 'A', HT2_EDIT_SPL, 0);
+        ht2_spl_set(e, intronLen, (a.seq & 0xff) ? HT2_SPL_FW : HT2_SPL_RC, true, 0.0f);
+        return front ? tmpInsertFront(e) : tmpPush(e);
+    }
+    // a splice site as read among ALTs [a, b)
+    HT2_HD bool ssInRange(uint32_t a, uint32_t b) const {
+        const Ht2Alt* alts = altTable();
+        for (uint32_t s = a; s < b; s++) if (altSsFw(alts[s])) return true;
+        return false;
+    }
 
     // tmp_edits helpers
     HT2_HD bool tmpPush(const Ht2Edit& e) {
@@ -78,7 +100,7 @@
     // alignWithALTs_recur, left == true (hi_aligner.h:2822-3167)
     HT2_NI uint32_t altLeft(Ht2Hit& h, const uint8_t* seq, uint32_t joinedOff, uint32_t rdoff, uint32_t rdlen,
                             const uint8_t* rfseq, uint32_t tidx, int rfoff, uint32_t rflen, uint32_t mm,
-                            uint32_t tmp_numNs, uint32_t* numNs, uint32_t dep) {
+                            uint32_t tmp_numNs, uint32_t* numNs, uint32_t dep, bool prevSs) {
         Ht2AltScratch& S = W->alt;
         if (S.numALTsTried > P->maxAltsTried + dep) return 0;
         if (dep >= HT2_ALT_MAXDEP) { HT2_GERR(3); return 0; }
@@ -130,6 +152,9 @@
                     if (altIsSnp(alt)) {
                         if (alt.type == HT2_ALT_SNP_DEL && !alt.reversed) continue;
                         if (alt.pos + rdlen < joinedOff) break;
+                    } else if (altSs(alt)) {
+                        if (alt.pos < alt.len) continue;
+                        if (alt.pos + rdlen - 1 < joinedOff) break;
                     } else continue;
                 }
             }
@@ -137,11 +162,16 @@
             for (; second > first; second--) {
                 Ht2Alt alt = alts[second];
                 if (alt.pos >= joinedOff) continue;
+                const bool ss = altSs(alt);
+                if (ss) {   // the reversed copy, turned back into [left, right] = [pos, len]
+                    if (alt.pos < alt.len) continue;
+                    const uint32_t t = alt.pos; alt.pos = alt.len; alt.len = t;
+                }
                 if (alt.type == HT2_ALT_SNP_DEL) {
                     if (!alt.reversed) continue;
                     alt.pos = alt.pos - alt.len + 1;
                 }
-                if (!altIsSnp(alt)) continue;
+                if (!altIsSnp(alt) && !ss) continue;
                 bool alt_compatible = false;
                 int rf_i = (int)rflen - 1, rd_i = (int)rdoff;
                 int diff = 0;
@@ -149,7 +179,8 @@
                 else if (alt.type == HT2_ALT_SNP_DEL) {
                     if (alt.pos + alt.len >= joinedOff) continue;
                     diff = (int)(joinedOff - (alt.pos + alt.len));
-                } else diff = (int)(joinedOff - alt.pos);
+                } else if (ss) diff = (int)(joinedOff - (alt.len + 1));
+                else diff = (int)(joinedOff - alt.pos);
                 if (rf_i < diff || rd_i < diff) continue;
                 rf_i -= diff; rd_i -= diff;
                 int rd_bp = seq[rd_i];
@@ -187,6 +218,12 @@
                         rf_i -= (int)alt.len;
                         alt_compatible = true;
                     }
+                } else if (ss) {
+                    // no splice right after a splice (hi_aligner.h:3021-3024)
+                    if (!(rd_i == (int)rdoff && prevSs)) {
+                        if (!pushSsEdit((uint32_t)(rd_i + 1), alt, alt.pos, alt.len, true)) break;
+                        alt_compatible = true;
+                    }
                 } else { // insertion
                     if (rd_i > (int)alt.len) {
                         bool same_seq = true;
@@ -213,6 +250,10 @@
                     const uint8_t* next_rfseq = rfseq;
                     int next_rflen = rf_i + 1;
                     const int next_rdlen = rd_i + 1;
+                    if (ss) {   // continue left of the intron
+                        next_rfoff -= (int)(alt.len - alt.pos + 1);
+                        next_rfseq = NULL;
+                    }
                     if (next_rflen < next_rdlen) {
                         int add_len = next_rdlen + 10 - next_rflen;
                         if (next_rfoff < add_len) add_len = next_rfoff;
@@ -221,7 +262,7 @@
                         next_rfseq = NULL;
                     }
                     const uint32_t alignedLen = altLeft(h, seq, next_joinedOff, (uint32_t)next_rdoff, (uint32_t)next_rdlen, next_rfseq,
-                                                        tidx, next_rfoff, (uint32_t)next_rflen, mm, tmp_numNs, numNs, dep + 1);
+                                                        tidx, next_rfoff, (uint32_t)next_rflen, mm, tmp_numNs, numNs, dep + 1, ss);
                     if (alignedLen == (uint32_t)next_rdlen) { S.nbuf = bufMark; return rdlen; }
                 }
                 // restore
@@ -281,16 +322,18 @@
             if (first >= nalts) { S.nbuf = bufMark; return 0; }
             for (; second < nalts; second++) {
                 const Ht2Alt& alt = alts[second];
+                if (alt.type == HT2_ALT_SPLICESITE && !altSsFw(alt)) continue;
                 if (alt.type == HT2_ALT_SNP_DEL && alt.reversed) continue;
                 if (alt.pos > joinedOff + max_rd_i) break;
             }
         }
-        if (mm_max_rd_i == rdlen) { S.nbuf = bufMark; return mm_max_rd_i; }   // no splice-site ALTs to search further
+        if (mm_max_rd_i == rdlen && !ssInRange(first, second)) { S.nbuf = bufMark; return mm_max_rd_i; }   // a splice site in reach is still tried
         if (tmp_mm > 0) { S.ntmp -= tmp_mm; tmp_mm = 0; }
         const uint32_t orig_nedits = S.ntmp;
         for (; first < second; first++) {
             const Ht2Alt& alt = alts[first];
-            if (!altIsSnp(alt)) continue;
+            const bool ss = altSsFw(alt);
+            if (!altIsSnp(alt) && !ss) continue;
             if (alt.type == HT2_ALT_SNP_DEL && alt.reversed) continue;
             bool alt_compatible = false;
             uint32_t rf_i, rd_i;
@@ -333,6 +376,16 @@
                         alt_compatible = true;
                     }
                 }
+            } else if (ss) {
+                // no two introns in a row (hi_aligner.h:3413-3421)
+                bool try_splice = rd_i > 0;
+                if (rd_i == 0 && dep > 0) {
+                    if (S.ntmp > 0 && S.tmp[S.ntmp - 1].type != HT2_EDIT_SPL) try_splice = true;
+                }
+                if (try_splice) {
+                    if (!pushSsEdit(rd_i + rdoff_add, alt, alt.pos, alt.len, false)) break;
+                    alt_compatible = true;
+                }
             } else { // insertion
                 if (rd_i + alt.len <= rdlen && rf_i > 0) {
                     bool same_seq = true;
@@ -356,19 +409,25 @@
                     return rd_i;
                 }
                 uint32_t next_joinedOff = 0;
-                const int next_rfoff = rfoff + (int)rf_i;
+                int next_rfoff = rfoff + (int)rf_i;
                 const uint32_t next_rdoff = rdoff + rd_i;
                 const uint8_t* next_rfseq = rfseq + rf_i;
                 uint32_t next_rflen = rflen - rf_i;     // wraps like the reference's index_t when rf_i > rflen (long deletion)
                 const uint32_t next_rdlen = rdlen - rd_i;
                 if (alt.type == HT2_ALT_SNP_SGL) next_joinedOff = alt.pos + 1;
                 else if (alt.type == HT2_ALT_SNP_DEL) { next_joinedOff = alt.pos + alt.len; if (rflen <= rf_i) next_rflen = 0; }
+                else if (ss) {   // continue right of the intron
+                    next_joinedOff = alt.len + 1;
+                    next_rfoff += (int)(alt.len - alt.pos + 1);
+                    next_rfseq = NULL;
+                }
                 else next_joinedOff = alt.pos;
                 if (next_rflen < next_rdlen) { next_rflen = next_rdlen + 10; next_rfseq = NULL; }
                 const uint32_t alignedLen = altRight(h, seq, next_joinedOff, rdoff_add + rd_i, next_rdoff, next_rdlen, next_rfseq, tidx,
                                                      next_rfoff, next_rflen, mm, tmp_numNs, numNs, dep + 1);
                 if (alignedLen > 0) {
-                    if (rd_i + alignedLen == rdlen) { S.nbuf = bufMark; return rd_i + alignedLen; }
+                    // after a splice, a later splice site in reach is still tried (hi_aligner.h:3517-3530)
+                    if (!(ss && ssInRange(first + 1, second)) && rd_i + alignedLen == rdlen) { S.nbuf = bufMark; return rd_i + alignedLen; }
                 }
             }
             if (orig_nedits < S.ntmp) S.ntmp = orig_nedits;
@@ -390,7 +449,7 @@
         for (uint32_t i = 0; i < h.nedits; i++) S.tmp[i] = h.edits[i];
         S.ntmp = h.nedits;
         const uint32_t nedits = h.nedits;
-        if (left) altLeft(h, seq, joinedOff, rdoff, rdlen, NULL, tidx, rfoff, rflen, mm, 0, numNs, 0);
+        if (left) altLeft(h, seq, joinedOff, rdoff, rdlen, NULL, tidx, rfoff, rflen, mm, 0, numNs, 0, false);
         else altRight(h, seq, joinedOff, rdoff - base_rdoff, rdoff, rdlen, NULL, tidx, rfoff, rflen, mm, 0, numNs, 0);
         uint32_t extlen = left ? (rdoff - (uint32_t)S.best_rdoff) : ((uint32_t)S.best_rdoff - rdoff);
         if (left && S.best_rdoff < 0) extlen = rdoff + 1;
@@ -568,7 +627,7 @@
         return ok;
     }
 
-    // GenomeHit::findOffDiffs (hi_aligner.h:2545-2650), SNP indels only.  Entries are (|diff|, sign) with
+    // GenomeHit::findOffDiffs (hi_aligner.h:2545-2650), SNP indels only (splice sites are skipped).  Entries are (|diff|, sign) with
     // sign stored as 0 / 1 / 2 for -1 / 0 / +1 so that the pair ordering of the reference's sort is the
     // ordering of the two unsigned values.  Returns single_offDiffs_size.
     HT2_NI uint32_t findOffDiffs(uint32_t start, uint32_t end) {
@@ -580,6 +639,7 @@
         uint32_t first = altLoBound(start), second;
         for (second = first; second < nalts; second++) {
             const Ht2Alt& alt = alts[second];
+            if (alt.type == HT2_ALT_SPLICESITE && !altSsFw(alt)) continue;
             if (alt.type == HT2_ALT_SNP_DEL && alt.reversed) continue;
             if (alt.pos >= end) break;
         }
@@ -684,14 +744,77 @@
         return adjustTry(h, rdi, false);
     }
 
-    // GenomeHit::adjustWithALT, static version used by getAnchorHits (hi_aligner.h:2239-2388): appends the
-    // adjusted hit (and its equally good alternatives) to W->genomeHits.
+    // GenomeHit::findSSOffs (hi_aligner.h:2485-2540): the joined-offset shifts a BWT hit whose path crossed splice
+    // edges of the graph may need -- every intron of a site in [start, end), and the distances from a site's left
+    // end to the right ends of other sites near its right end -- as sorted, unique (|shift|, sign) pairs with sign
+    // 0 / 1 / 2 for -1 / 0 / +1, the first being (0, 0).  Returns the number of pairs.
+    HT2_NI uint32_t findSSOffs(uint32_t start, uint32_t end, uint32_t (*so)[2]) {
+        uint32_t n = 0;
+        so[n][0] = 0; so[n][1] = 1; n++;
+        if (H->nSpliceSites == 0 || noSpl()) return n;
+        const Ht2Alt* alts = altTable();
+        const uint32_t nalts = numAlts();
+        for (uint32_t i = altLoBound(start); i < nalts; i++) {
+            const Ht2Alt& alt = alts[i];
+            if (alt.pos >= end) break;
+            if (alt.type != HT2_ALT_SPLICESITE) continue;
+            if (n >= HT2_SS_OFFS) { HT2_GERR(13); return n; }
+            if (alt.pos < alt.len) {
+                so[n][0] = alt.len - alt.pos + 1; so[n][1] = 2; n++;
+                const uint32_t relax = 5;
+                for (uint32_t j = altLoBound(alt.len > relax ? alt.len - relax : 0); j < nalts; j++) {
+                    const Ht2Alt& alt2 = alts[j];
+                    if (alt2.type != HT2_ALT_SPLICESITE) continue;
+                    if (alt2.pos < alt2.len) continue;
+                    if (alt2.pos + alt2.len == alt.pos + alt.len) continue;
+                    if (alt2.pos > alt.len + relax) break;
+                    if (n >= HT2_SS_OFFS) { HT2_GERR(13); return n; }
+                    if (alt2.len < alt.pos) { so[n][0] = alt.pos - alt2.len; so[n][1] = 0; }
+                    else { so[n][0] = alt2.len - alt.pos; so[n][1] = 2; }
+                    n++;
+                }
+            } else {
+                so[n][0] = alt.pos - alt.len + 1; so[n][1] = 0; n++;
+            }
+        }
+        if (n > 1) {   // sort + unique on (first, second)
+            for (uint32_t i = 1; i < n; i++) {
+                const uint32_t a0 = so[i][0], a1 = so[i][1]; uint32_t j = i;
+                while (j > 0 && (so[j - 1][0] > a0 || (so[j - 1][0] == a0 && so[j - 1][1] > a1))) { so[j][0] = so[j - 1][0]; so[j][1] = so[j - 1][1]; j--; }
+                so[j][0] = a0; so[j][1] = a1;
+            }
+            uint32_t m = 1;
+            for (uint32_t i = 1; i < n; i++) if (so[i][0] != so[m - 1][0] || so[i][1] != so[m - 1][1]) { so[m][0] = so[i][0]; so[m][1] = so[i][1]; m++; }
+            n = m;
+        }
+        return n;
+    }
+
+    // GenomeHit::adjustWithALT, static version used by getAnchorHits (hi_aligner.h:2239-2388): for each splice shift
+    // of findSSOffs, appends the adjusted hit (and its equally good alternatives) to W->genomeHits.  The result is
+    // the last shift's, as in the reference.
     HT2_NI bool adjustWithALTCoord(uint32_t rdoff, uint32_t len, const Ht2Coord& coord, uint32_t rdi) {
-        const uint32_t before = W->nGenomeHits;
-        if (W->nGenomeHits >= HT2_MAX_GHITS) { W->err |= HT2_ERR_GHITS; return false; }
-        Ht2Hit& gh = W->genomeHits[W->nGenomeHits++];
-        initHit(gh, coord.fw != 0, rdoff, len, 0, 0, coord.ref, coord.off, coord.joinedOff);
-        if (!GRAPH) return true;
-        if (!adjustTry(gh, rdi, true)) W->nGenomeHits = before;
-        return W->nGenomeHits > before;
+        if (!GRAPH) {
+            if (W->nGenomeHits >= HT2_MAX_GHITS) { W->err |= HT2_ERR_GHITS; return false; }
+            initHit(W->genomeHits[W->nGenomeHits++], coord.fw != 0, rdoff, len, 0, 0, coord.ref, coord.off, coord.joinedOff);
+            return true;
+        }
+        const uint32_t width = 1u << (gfm.g->offRate + 2);
+        uint32_t ssOffs[HT2_SS_OFFS][2];
+        const uint32_t nss = findSSOffs(coord.joinedOff >= width ? coord.joinedOff - width : 0, coord.joinedOff + width, ssOffs);
+        bool found = false;
+        for (uint32_t s = 0; s < nss; s++) {
+            uint32_t off = coord.off, joinedOff = coord.joinedOff;
+            if (ssOffs[s][0] > 0) {
+                if (ssOffs[s][1] > 1) { off += ssOffs[s][0]; joinedOff += ssOffs[s][0]; }
+                else { off -= ssOffs[s][0]; joinedOff -= ssOffs[s][0]; }
+            }
+            const uint32_t before = W->nGenomeHits;
+            if (W->nGenomeHits >= HT2_MAX_GHITS) { W->err |= HT2_ERR_GHITS; return false; }
+            Ht2Hit& gh = W->genomeHits[W->nGenomeHits++];
+            initHit(gh, coord.fw != 0, rdoff, len, 0, 0, coord.ref, off, joinedOff);
+            if (!adjustTry(gh, rdi, true)) W->nGenomeHits = before;
+            found = W->nGenomeHits > before;
+        }
+        return found;
     }

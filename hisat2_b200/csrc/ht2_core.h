@@ -214,6 +214,7 @@ struct Ht2Frame {
 // Scratch of one alignWithALTs call (graph indexes; ht2_alt.h)
 #define HT2_ALT_TMP_EDITS 72     /* trial edit list of the ALT recursion: a 27-base deletion ALT alone is 27 read-gap edits */
 #define HT2_ALT_CANDS 4
+#define HT2_SS_OFFS 32           /* splice shifts findSSOffs lists for one BWT hit (a local array of adjustWithALTCoord) */
 #define HT2_ALT_BUFS 4
 #define HT2_ALT_MAXDEP 24
 struct Ht2AltScratch {
@@ -1445,6 +1446,7 @@ struct Ht2AlignerT {
                 for (uint32_t i = 0; i < added_edits; i++) {
                     if (h.edits[i].type == HT2_EDIT_REF_GAP) ref_ext--;
                     else if (h.edits[i].type == HT2_EDIT_READ_GAP) ref_ext++;
+                    else if (GRAPH && isSpl(h.edits[i])) ref_ext += (int)ht2_spl_len(h.edits[i]);   // across a splice-site ALT
                 }
                 h.rdoff -= best_ext;
                 h.toff -= (uint32_t)ref_ext;
@@ -1916,8 +1918,15 @@ struct Ht2AlignerT {
             }
         }
         if ((P->tranFilter & HT2_TRAN_XS_ONLY) && spl && (conflict || dir == HT2_SPL_UNKNOWN)) return false;
-        if ((P->tranFilter & HT2_TRAN_TMO) && !(spl && known)) return false;
+        if ((P->tranFilter & HT2_TRAN_TMO) && !(spl && known) && !(GRAPH && !spl && insideExon(hit))) return false;
         return true;
+    }
+    // --avoid-pseudogene on an index with exons (only graph indexes have them): an unspliced hit inside an exon maps
+    // to a known transcript, which lets it pass --tmo (hi_aligner.h:6105-6127)
+    HT2_NI bool insideExon(const Ht2Hit& hit) const {
+        if (!(P->tranFilter & HT2_TRAN_AVOID_PSEUDOGENE) || ssT == NULL) return false;
+        Ht2SsView v; v.init(ssT);
+        return v.insideExon(hit.tidx, hit.toff, hit.toff + hit.len - 1);
     }
 #endif
     // HI_Aligner::reportHit (hi_aligner.h:6064-6198), unpaired form.

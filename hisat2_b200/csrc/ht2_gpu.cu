@@ -1116,6 +1116,8 @@ static int startOpen(ht2gpu_handle* h)
     return HT2GPU_OK;
 }
 
+static int loadIndexSsdb(ht2gpu_handle* h);
+
 // Every ht2gpu_open*.  load(h) brings the host image (h->img) and the device blob (h->dBlob).  *out
 // holds the handle from the start: after a failure, ht2gpu_last_error explains it and ht2gpu_close frees the handle.
 template <typename Load>
@@ -1130,6 +1132,7 @@ static int openHandle(const ht2gpu_options_t* opt, ht2gpu_handle_t** out, Load l
     if (!rc && !h->dBlob) h->dBlob = h->blobCopy;   // the handle's own copy, unless it borrows the caller's
     if (!rc) rc = checkImage(h);
     if (!rc) rc = loadNamesAndParams(h);
+    if (!rc) rc = loadIndexSsdb(h);
     if (!rc) rc = chooseGeometry(h);
     if (!rc) rc = acquirePool(h);
     if (!rc) rc = setKernelLimits(h);
@@ -1392,8 +1395,8 @@ static int checkBatch(ht2gpu_handle* h, const ht2gpu_read_batch_t* b)
 {
     if (b->paired && (b->n_reads & 1)) { h->err = "paired batch needs an even number of reads"; return HT2GPU_ERR_ARG; }
     if (h->graph && h->img->header()->altsUnsupported) {
-        h->err = "this graph index holds splice-site / exon ALTs; alignment through them is not implemented in this build "
-                 "(SNP / indel ALTs are; ht2gpu_seed_search works on any graph index)";
+        h->err = "this graph index holds ALT_SNP_ALT records; alignment through them is not implemented in this build "
+                 "(SNP / indel / splice-site / exon ALTs are; ht2gpu_seed_search works on any graph index)";
         return HT2GPU_ERR_UNSUPPORTED;
     }
     return HT2GPU_OK;
@@ -2011,8 +2014,42 @@ static int refuseInFlight(ht2gpu_handle* h, const char* call)
     return HT2GPU_OK;
 }
 
-// The run's read-only splice-site DB: --known-splicesite-infile / --novel-splicesite-infile (hisat2.cpp:4101-4116,
-// SpliceSiteDB::read splice_site.cpp:727).  Replaces a DB loaded earlier.  Refused while a batch is in flight.
+#ifdef HT2_ENABLE_SPLICED
+// An index built with splice sites or exons (hisat2-build --ss / --exon) brings its own DB (hisat2.cpp:4093-4100)
+static bool indexHasSsdb(const ht2gpu_handle* h) { return h->img->header()->nSpliceSites > 0 || h->img->header()->nExons > 0; }
+
+// (Re)builds the handle's DB: the index's sites and exons, then the files' sites.  No DB at all when neither gives one.
+static int buildSsdb(ht2gpu_handle* h, const std::vector<Ht2SsFile>& files, uint32_t* n_sites)
+{
+    h->dSsT.release();
+    h->ssBlob.clear();
+    if (n_sites) *n_sites = 0;
+    const bool indexSites = !h->P.noSplicedAlignment;   // without spliced alignment the reference does not load them
+    if (files.empty() && !(indexSites && indexHasSsdb(h))) return HT2GPU_OK;
+    std::string err; uint32_t ns = 0;
+    if (!ht2_ssdb_build(*h->img, files, h->ssBlob, ns, err, &h->refNames, indexSites)) { h->err = err; h->ssBlob.clear(); return HT2GPU_ERR_INDEX; }
+    CK(cudaSetDevice(h->device));
+    CK(h->dSsT.upload(h->ssBlob.data(), h->ssBlob.size()));
+    if (n_sites) *n_sites = ns;
+    return HT2GPU_OK;
+}
+#endif
+
+// Every open path: the DB of an index with splice sites / exons, built from the image, so that replicas have the same
+static int loadIndexSsdb(ht2gpu_handle* h)
+{
+#ifdef HT2_ENABLE_SPLICED
+    return buildSsdb(h, std::vector<Ht2SsFile>(), NULL);
+#else
+    (void)h;
+    return HT2GPU_OK;
+#endif
+}
+
+// The run's read-only splice-site DB: the index's own sites and exons, then --known-splicesite-infile and
+// --novel-splicesite-infile (hisat2.cpp:4093-4116, SpliceSiteDB::read splice_site.cpp:653-775).  Replaces a DB loaded
+// earlier; with no files it is the index's DB again (empty for an index without sites).  Refused while a batch is in
+// flight.
 extern "C" int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_path, const char* novel_path, uint32_t* n_sites)
 {
     if (!h) return HT2GPU_ERR_ARG;
@@ -2022,17 +2059,8 @@ extern "C" int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_pat
     if (known_path && *known_path) files.push_back({known_path, true});
     if (novel_path && *novel_path) files.push_back({novel_path, false});
     if (h->collectSs && files.size()) { h->err = "ht2gpu: a splice-site DB cannot be loaded while novel splice sites are collected"; return HT2GPU_ERR_UNSUPPORTED; }
-    h->dSsT.release();
-    h->ssBlob.clear();
-    if (n_sites) *n_sites = 0;
-    if (files.empty()) return HT2GPU_OK;
     for (const Ht2SsFile& f : files) { FILE* t = fopen(f.path.c_str(), "rb"); if (!t) { h->err = "ht2gpu: cannot open " + f.path; return HT2GPU_ERR_INDEX; } fclose(t); }
-    std::string err; uint32_t ns = 0;
-    if (!ht2_ssdb_build(*h->img, files, h->ssBlob, ns, err, &h->refNames)) { h->err = err; h->ssBlob.clear(); return HT2GPU_ERR_INDEX; }
-    CK(cudaSetDevice(h->device));
-    CK(h->dSsT.upload(h->ssBlob.data(), h->ssBlob.size()));
-    if (n_sites) *n_sites = ns;
-    return HT2GPU_OK;
+    return buildSsdb(h, files, n_sites);
 #else
     (void)known_path; (void)novel_path; (void)n_sites;
     h->err = "ht2gpu: built without spliced alignment"; return HT2GPU_ERR_UNSUPPORTED;
@@ -2046,7 +2074,13 @@ extern "C" int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_pat
 extern "C" int ht2gpu_collect_splicesites(ht2gpu_handle_t* h, int enable)
 {
     if (!h) return HT2GPU_ERR_ARG;
-    if (enable && h->dSsT) { h->err = "ht2gpu: --novel-splicesite-outfile together with a loaded splice-site DB is order dependent in the reference; not supported"; return HT2GPU_ERR_UNSUPPORTED; }
+    if (enable && h->dSsT) {
+        h->err = h->img->header()->nSpliceSites > 0 || h->img->header()->nExons > 0
+            ? "ht2gpu: --novel-splicesite-outfile is not supported on an index built with splice sites / exons: the index's "
+              "sites form a splice-site DB, and with a DB loaded the reference's novel sites depend on the order reads finish in"
+            : "ht2gpu: --novel-splicesite-outfile together with a loaded splice-site DB is order dependent in the reference; not supported";
+        return HT2GPU_ERR_UNSUPPORTED;
+    }
     if (enable && h->P.noSplicedAlignment) { h->err = "ht2gpu: novel splice sites need spliced alignment"; return HT2GPU_ERR_UNSUPPORTED; }
     std::lock_guard<std::mutex> lk(h->novelMu);
     if (enable && !h->collectSs) h->novel.sites.clear();

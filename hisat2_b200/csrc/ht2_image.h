@@ -102,9 +102,11 @@ struct Ht2RefRecord {
     uint32_t pad;
 };
 
-// ALT record (alt.h:43-204); 'left'/'right' alias pos/len for splice sites.  As in the reference's
-// union, the low byte of 'seq' doubles as the 'reversed' flag of the deletion copies the loader
-// appends (gfm.h:856-872); 'reversed' mirrors it for convenience.
+// ALT record (alt.h:43-204); 'left'/'right' alias pos/len for splice sites and exons.  As in the
+// reference's union, the low byte of 'seq' doubles as the 'reversed' flag of the deletion copies the
+// loader appends (gfm.h:856-872) and as the strand ('fw') of a splice site; 'reversed' mirrors it for
+// deletions only.  A splice site is stored twice: as read (left < right) and as the loader's reversed
+// copy with left and right swapped (left > right), which the leftward ALT extension walks.
 #define HT2_ALT_NONE 0u
 #define HT2_ALT_SNP_SGL 1u
 #define HT2_ALT_SNP_INS 2u
@@ -141,12 +143,12 @@ struct Ht2ImageHeader {
     uint64_t refBufBytes;
     // ALTs
     uint32_t nAlts;
-    uint32_t pad2;
-    uint64_t o_alts;       // Ht2Alt[nAlts]: augmented with reversed deletions and sorted like the reference's loader
+    uint32_t nSpliceSites;    // ALT_SPLICESITE records of the .7.ht2 (each also has its reversed copy in the table)
+    uint64_t o_alts;       // Ht2Alt[nAlts]: augmented with reversed deletions and splice sites, sorted like the reference's loader
     uint64_t o_altNames;   // '\0'-separated, nAlts entries (host side: Zs:Z)
     uint64_t altNamesBytes;
-    uint32_t altsUnsupported; // 1 when the ALT list holds splice sites / exons (not handled by this build)
-    uint32_t pad3;
+    uint32_t altsUnsupported; // 1 when the ALT list holds ALT_SNP_ALT records (which the reference never handles either)
+    uint32_t nExons;          // ALT_EXON records of the .7.ht2
     // reference names (host side only, for SAM headers)
     uint64_t o_names;      // '\0'-separated, nRefs entries
     uint64_t namesBytes;

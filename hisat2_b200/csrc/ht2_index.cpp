@@ -451,8 +451,15 @@ Ht2Image* ht2_image_load(const char* base_c, std::string& err)
             const size_t nalts = alts.size();
             for (size_t s2 = 0; s2 < nalts; s2++) {
                 const Ht2Alt a = alts[s2];
-                if (a.type == HT2_ALT_SPLICESITE || a.type == HT2_ALT_EXON || a.type == HT2_ALT_SNP_ALT) h.altsUnsupported = 1;
-                if (a.type == HT2_ALT_SNP_DEL) {       // reversed copy at the deletion's last base (gfm.h:866-872)
+                if (a.type == HT2_ALT_SNP_ALT) h.altsUnsupported = 1;
+                if (a.type == HT2_ALT_EXON) h.nExons++;
+                if (a.type == HT2_ALT_SPLICESITE) {    // reversed copy: left and right swapped, named "ssr" (gfm.h:873-879)
+                    h.nSpliceSites++;
+                    Ht2Alt r = a;
+                    r.pos = a.len; r.len = a.pos;
+                    alts.push_back(r);
+                    names.push_back("ssr");
+                } else if (a.type == HT2_ALT_SNP_DEL) {       // reversed copy at the deletion's last base (gfm.h:880-885)
                     Ht2Alt r = a;
                     r.pos = a.pos + a.len - 1;
                     r.reversed = 1;
@@ -546,7 +553,7 @@ std::string Ht2RefNames::token(uint32_t i) const
 }
 
 bool ht2_ssdb_build(const Ht2Image& img, const std::vector<Ht2SsFile>& files, std::vector<uint8_t>& blob, uint32_t& nSites, std::string& err,
-                    const Ht2RefNames* refNames)
+                    const Ht2RefNames* refNames, bool indexSites)
 {
     const uint32_t nRefs = img.header()->nRefs;
     Ht2RefNames own;
@@ -555,6 +562,42 @@ bool ht2_ssdb_build(const Ht2Image& img, const std::vector<Ht2SsFile>& files, st
     for (uint32_t r = 0; r < nRefs; r++) names[r] = refNames->token(r);
     std::vector<std::vector<Ht2SsSite>> per(nRefs);
     std::vector<std::set<std::tuple<uint32_t, uint32_t, uint32_t>>> seen(nRefs);
+    std::vector<Ht2SsExon> exons;
+    {   // the index's splice sites and exons first (SpliceSiteDB::read(gfm, alts), splice_site.cpp:653-720)
+        const Ht2ImageHeader* H = img.header();
+        const uint8_t* blob0 = img.blob.data();
+        const Ht2Alt* alts = (const Ht2Alt*)(blob0 + H->o_alts);
+        const uint32_t* rstarts = (const uint32_t*)(blob0 + H->global.o_rstarts);
+        const uint32_t* plen = (const uint32_t*)(blob0 + H->global.o_plen);
+        const uint32_t nFrag = H->global.nFrag;
+        for (uint32_t i = 0; i < H->nAlts; i++) {
+            const Ht2Alt& a = alts[i];
+            if (a.type != HT2_ALT_EXON && (a.type != HT2_ALT_SPLICESITE || !indexSites)) continue;
+            if (a.pos > a.len) continue;   // the reversed copy of a splice site
+            // joinedToTextOff(1, left, ...) with straddlers rejected (gfm.h:5527-5600)
+            uint32_t lo = 0, hi = nFrag;
+            while (lo < hi) { const uint32_t m = lo + ((hi - lo) >> 1); if (rstarts[m * 3] <= a.pos) lo = m + 1; else hi = m; }
+            const uint32_t elt = lo - 1;
+            const uint32_t upper = elt + 1 == nFrag ? H->global.len : rstarts[(elt + 1) * 3];
+            if (lo == 0 || a.pos >= upper) { err = "ht2: a splice-site / exon ALT of the index lies outside the reference"; return false; }
+            const uint32_t ref = rstarts[elt * 3 + 1], tlen = plen[ref];
+            uint32_t left = a.pos - rstarts[elt * 3] + rstarts[elt * 3 + 2];
+            uint32_t right = left + (a.len - a.pos);
+            const uint32_t fw = (uint32_t)(a.seq & 0xff);
+            if (a.type == HT2_ALT_SPLICESITE) {
+                left -= 1; right += 1;
+                Ht2SsSite st; st.left = left; st.right = right; st.dir = fw ? HT2_SPL_FW : HT2_SPL_RC; st.known = 1;
+                if (seen[ref].insert(std::make_tuple(st.left, st.right, st.dir)).second) per[ref].push_back(st);
+            } else {
+                left = left >= 10 ? left - 10 : 0;
+                right = right + 10 < tlen ? right + 10 : tlen - 1;
+                Ht2SsExon e; e.ref = ref; e.left = left; e.right = right; e.pad = 0;
+                exons.push_back(e);
+            }
+        }
+        std::stable_sort(exons.begin(), exons.end(), [](const Ht2SsExon& x, const Ht2SsExon& y) {
+            return x.ref != y.ref ? x.ref < y.ref : (x.left != y.left ? x.left < y.left : x.right < y.right); });
+    }
     for (const Ht2SsFile& f : files) {
         std::ifstream in(f.path.c_str(), std::ios::in);
         if (!in.is_open()) continue;
@@ -574,9 +617,10 @@ bool ht2_ssdb_build(const Ht2Image& img, const std::vector<Ht2SsFile>& files, st
     nSites = 0;
     for (auto& v : per) nSites += (uint32_t)v.size();
     const size_t offWords = ((size_t)nRefs + 1 + 3) & ~(size_t)3;
-    blob.assign(sizeof(Ht2SsHeader) + offWords * 4 + (size_t)nSites * 2 * sizeof(Ht2SsSite), 0);
+    blob.assign(sizeof(Ht2SsHeader) + offWords * 4 + (size_t)nSites * 2 * sizeof(Ht2SsSite) + exons.size() * sizeof(Ht2SsExon), 0);
     Ht2SsHeader* h = (Ht2SsHeader*)blob.data();
-    h->magic = HT2_SS_MAGIC; h->nRefs = nRefs; h->nSites = nSites; h->pad = 0;
+    h->magic = HT2_SS_MAGIC; h->nRefs = nRefs; h->nSites = nSites; h->nExons = (uint32_t)exons.size();
+    if (!exons.empty()) memcpy(blob.data() + sizeof(Ht2SsHeader) + offWords * 4 + (size_t)nSites * 2 * sizeof(Ht2SsSite), exons.data(), exons.size() * sizeof(Ht2SsExon));
     uint32_t* refOff = (uint32_t*)(blob.data() + sizeof(Ht2SsHeader));
     Ht2SsSite* fw = (Ht2SsSite*)(blob.data() + sizeof(Ht2SsHeader) + offWords * 4);
     Ht2SsSite* bw = fw + nSites;

@@ -37,7 +37,10 @@ struct Ht2RefNames {
     std::string token(uint32_t i) const;   // name i up to its first white space
 };
 
-// The read-only splice-site DB of a run (ht2_ssdb.h) from the text files of --known-splicesite-infile ('known' = true)
+// The read-only splice-site DB of a run (ht2_ssdb.h): first the splice sites (unless indexSites is false, as under
+// --no-spliced-alignment, where the reference does not load them: gfm.h:760-771) and exons of the index
+// (SpliceSiteDB::read(gfm, alts), splice_site.cpp:653-720: each site known, at left - 1 / right + 1, each exon widened
+// by 10 bases at both ends), then the sites of the text files of --known-splicesite-infile ('known' = true)
 // and --novel-splicesite-infile (false): "<chr> <left> <right> <+|->" per site, 0-based, as hisat2_extract_splice_sites.py
 // writes them (SpliceSiteDB::read, splice_site.cpp:727-775: names compared up to the first white space, unknown
 // names skipped, a site already present is dropped).  Files are read in the order given.  An unreadable file is
@@ -55,6 +58,6 @@ struct Ht2NovelSites {
     bool write(const Ht2Image& img, const char* path, uint64_t* nWritten, std::string& err, const Ht2RefNames* names = NULL) const;
 };
 bool ht2_ssdb_build(const Ht2Image& img, const std::vector<Ht2SsFile>& files, std::vector<uint8_t>& blob, uint32_t& nSites, std::string& err,
-                    const Ht2RefNames* names = NULL);
+                    const Ht2RefNames* names = NULL, bool indexSites = true);
 
 #endif

@@ -325,6 +325,12 @@ struct Ht2SamFmt {
         while (l < r) { const uint32_t m = l + ((r - l) >> 1); if (v.fw[m].left < left) l = m + 1; else r = m; }
         return l < b && v.fw[l].left <= right;
     }
+    // --avoid-pseudogene on an index with exons (hi_aligner.h:6119-6121): an unspliced alignment inside an exon of
+    // the index maps to a known transcript
+    HT2_NI bool insideExon(const ht2gpu_aln_t& al, uint32_t rdlen) const {
+        Ht2SsView v; v.init(in->nearSsT);
+        return v.h->nExons > 0 && v.insideExon(al.tidx, al.toff, al.toff + (rdlen - al.trim5 - al.trim3) - 1);
+    }
 #endif
     // AlnScore::calculate_hisat2_score (aligner_result.h:322-348), repeat = 0.  The splice part of the key
     // follows from the edits alone: GenomeHit::spliced() and the splicescore rule of calculateScore
@@ -361,6 +367,7 @@ struct Ht2SamFmt {
             splicescore = (int64_t)(ss / 100);     // TAlScore splicescore = splicescore_ / 100 (aligner_result.h:339)
             if (splicescore > 255) splicescore = 0; else splicescore = 255 - splicescore;
             transcript_score = (spl && known) ? 2 : (spl || (in->nearSsT != NULL && nearSpliceSites(al, rdlen))) ? 1 : 0;
+            if (!spl && in->nearSsT != NULL && insideExon(al, rdlen)) transcript_score = 2;
         }
 #else
         (void)rdlen;

@@ -467,7 +467,10 @@ typedef struct {
 int ht2gpu_seed_search(ht2gpu_handle_t* h, const ht2gpu_read_batch_t* batch, uint32_t max_range,
                        ht2gpu_seed_result_t* res);
 void ht2gpu_free_seed_results(ht2gpu_seed_result_t* res);
-/* 1 when the opened index is a graph (SNP / splice-site) index. */
+/* 1 when the opened index is a graph index: built with SNPs, splice sites or exons (hisat2-build --snp / --ss /
+ * --exon: the _snp, _tran and _snp_tran indexes).  Alignment crosses SNP, indel and splice-site ALTs; an index with
+ * splice sites or exons also brings its own splice-site DB (ht2gpu_load_splicesites).  ALT_SNP_ALT records, which the
+ * reference never handles either, make alignment calls fail with HT2GPU_ERR_UNSUPPORTED. */
 int ht2gpu_index_is_graph(const ht2gpu_handle_t* h);
 
 /* Host back end: selection, MAPQ and SAM text for a batch (finishRead).
@@ -532,9 +535,13 @@ uint32_t ht2gpu_ref_len(const ht2gpu_handle_t* h, uint32_t i);
 uint32_t ht2gpu_read_seed(const uint8_t* seq, const uint8_t* qual, uint32_t len,
                           const char* name, uint32_t global_seed);
 
-/* The run's read-only splice-site DB (spliced mode): the sites of --known-splicesite-infile and
- * --novel-splicesite-infile ("<chr> <left> <right> <+|->" per line, 0-based; hisat2.cpp:4101-4116,
- * SpliceSiteDB::read splice_site.cpp:727-775; either path may be NULL).  With a DB loaded, alignment runs the
+/* The run's read-only splice-site DB (spliced mode): the index's own splice sites and exons when it was built with
+ * --ss / --exon (known sites, inserted first; SpliceSiteDB::read splice_site.cpp:653-720), then the sites of
+ * --known-splicesite-infile and --novel-splicesite-infile ("<chr> <left> <right> <+|->" per line, 0-based;
+ * hisat2.cpp:4093-4116, splice_site.cpp:727-775; either path may be NULL; a site already present is dropped).  Such an
+ * index's handle holds its DB from ht2gpu_open on (also replicas made by ht2gpu_open_peer or from a device image), and
+ * ht2gpu_load_splicesites(h, NULL, NULL) returns to it; on other indexes that call empties the DB.  Without spliced
+ * alignment the index's sites are left out, as the reference does.  With a DB loaded, alignment runs the
  * three `if(!ssdb.empty())` branches of hybridSearch_recur (spliced_aligner.h:409-668, 685-811, 1365-1494):
  * short exon ends next to a listed site are aligned across it, and the template length of a concordant pair
  * excludes the longest listed intron between the mates (aligner_result.h:1631-1690).  Replaces a DB loaded
@@ -548,7 +555,8 @@ int ht2gpu_load_splicesites(ht2gpu_handle_t* h, const char* known_path, const ch
  * ht2gpu_wait_sam aggregates them per handle; ht2gpu_write_novel_splicesites merges the handles of a run and writes
  * "<chr> <left> <right> <+|-|.>" with the reference's read-count cutoffs and near-duplicate suppression -- the
  * first pass of the two-pass use (second pass: ht2gpu_load_splicesites(h, NULL, file)).  Refused while a DB is
- * loaded: the reference would let such sites steer later reads, i.e. depend on read order. */
+ * loaded: the reference would let such sites steer later reads, i.e. depend on read order.  So it is always refused on
+ * an index built with splice sites / exons in spliced mode, whose DB is always loaded; the message names the index. */
 int ht2gpu_collect_splicesites(ht2gpu_handle_t* h, int enable);
 int ht2gpu_write_novel_splicesites(ht2gpu_handle_t** hs, int n, const char* path, uint64_t* n_written);
 
